@@ -81,7 +81,17 @@ def parse_args() -> argparse.Namespace:
                     help="after the timed loop: the same step launched after 250 ms of idle, six times (is the scan slower inside a "
                          "loop of steps than timed alone?)")
     ap.add_argument("--filtered", action="store_true", help="also time metadata-filtered searches (both reference branches)")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="GPU arm: after the timed steps, write what the timed path returned in its last step as DIR/<name>.npy "
+                         "(float32 / float64; a fixed sample of rows where the output is large).  Inputs are seeded, so two "
+                         "builds run with the same arguments can be compared output for output.  Not with --workload c5 "
+                         "on more than one GPU: each rank scores only its own share of the pairs")
+    args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.dump_outputs and args.workload == "c5" and args.gpus > 1:
+        ap.error("--dump-outputs with --workload c5 needs --gpus 1 (each rank scores only its own share of the pairs)")
+    return args
 
 
 def resolve(args: argparse.Namespace) -> dict:
@@ -97,7 +107,24 @@ def resolve(args: argparse.Namespace) -> dict:
     return w
 
 
-# ---- clocks sampler (B200_PROFILING.md "clocks line") ---------------------------------------------
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(dirname: str, arrays: dict) -> None:
+    """``--dump-outputs``: every array as DIR/<name>.npy, float32 outputs as float32, everything else as float64."""
+    out = Path(dirname)
+    out.mkdir(parents=True, exist_ok=True)
+    conv = {}
+    for name, a in arrays.items():
+        a = np.asarray(a)
+        conv[name] = a.astype(np.float32 if a.dtype in (np.float16, np.float32) else np.float64)
+    total = sum(a.nbytes for a in conv.values())
+    assert total <= DUMP_LIMIT_BYTES, f"--dump-outputs: {total} bytes > {DUMP_LIMIT_BYTES}"
+    for name, a in conv.items():
+        np.save(out / f"{name}.npy", a)
+
+
+# ---- clocks sampler: SM clock, power and throttle reasons over the timed windows --------------------
 class ClockSampler:
     FIELDS = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
               "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
@@ -278,10 +305,14 @@ def run_rerank(args: argparse.Namespace, w: dict) -> None:
         types = [np.r_[np.zeros(12, np.int32), np.ones(L - 12, np.int32)] for L in lens[:n]]
         torch.set_num_threads(len(os.sched_getaffinity(0)))
         orr.hf_logits(model, ids[:4], types[:4])     # first call pays thread-pool / allocator start-up
-        t0 = time.perf_counter(); orr.hf_logits(model, ids, types); dt = time.perf_counter() - t0
+        steps = max(1, args.steps)
+        t0 = time.perf_counter()
+        for _ in range(steps):
+            orr.hf_logits(model, ids, types)
+        dt = (time.perf_counter() - t0) / steps
         v = n / dt
         print(json.dumps({"impl": "reference", "metric": "cross-encoder pairs/sec", "value": v, "unit": "pairs/s", "n_gpus": args.gpus,
-                          "steps": 1, "warmup": 0, "ms_per_step": dt * 1e3, "higher_is_better": True, "scaling": "strong",
+                          "steps": steps, "warmup": 0, "ms_per_step": dt * 1e3, "higher_is_better": True, "scaling": "strong",
                           "vs_baseline": None, "dtype": "f32", "data": "synthetic", "config": {"workload": w["desc"]},
                           "cpu_baseline": {"value": v, "unit": "pairs/s", "cores": torch.get_num_threads(), "kind": "port",
                                            "sample": f"{n} pairs, transformers BertForSequenceClassification fp32"},
@@ -296,22 +327,25 @@ def run_rerank(args: argparse.Namespace, w: dict) -> None:
     sel = np.concatenate([np.arange(q * n_c, (q + 1) * n_c) for q in mine])
     ids = [rng.integers(1000, 30000, size=L).astype(np.int32) for L in lens[sel]]
     types = [np.r_[np.zeros(12, np.int32), np.ones(L - 12, np.int32)] for L in lens[sel]]
-    eng.score_tokens(ids[:256], types[:256])
+    for _ in range(max(1, args.warmup)):
+        eng.score_tokens(ids[:256], types[:256])
     torch.cuda.synchronize()
     if world > 1:
         dist.barrier()
     t0 = time.perf_counter()
-    _, scores = eng.score_tokens(ids, types)                  # host ids in -> host scores out
-    order = np.argsort(-scores.reshape(len(mine), n_c), axis=1, kind="stable")   # rerank_chunks' reorder
+    for _ in range(args.steps):
+        logits, scores = eng.score_tokens(ids, types)             # host ids in -> host scores out
+        order = np.argsort(-scores.reshape(len(mine), n_c), axis=1, kind="stable")   # rerank_chunks' reorder
     torch.cuda.synchronize()
-    dt = torch.tensor([time.perf_counter() - t0], dtype=torch.float64, device="cuda")
+    dt = torch.tensor([(time.perf_counter() - t0) / args.steps], dtype=torch.float64, device="cuda")
     if world > 1:
         dist.all_reduce(dt, op=dist.ReduceOp.MAX)
     if rank == 0:
         total = n_q * n_c
         v = total / float(dt.item())
         tok = int(lens.sum())
-        line = {"metric": "cross-encoder pairs/sec", "value": v, "unit": "pairs/s", "n_gpus": world, "steps": 1, "warmup": 1,
+        line = {"metric": "cross-encoder pairs/sec", "value": v, "unit": "pairs/s", "n_gpus": world, "steps": args.steps,
+                "warmup": max(1, args.warmup),
                 "ms_per_step": float(dt.item()) * 1e3, "higher_is_better": True, "scaling": "strong", "vs_baseline": None,
                 "dtype": "f16", "data": "synthetic (seeded weights, random token pairs, mean 200 tokens)",
                 "config": {"workload": w["desc"], "pairs": total, "tokens": tok, "parallelism": f"dp{world} over queries"},
@@ -326,11 +360,11 @@ def run_rerank(args: argparse.Namespace, w: dict) -> None:
             peaks = json.loads((ROOT / "MEASURED_PEAKS.json").read_text())
         except (OSError, ValueError):
             pass
-        peak_tf = float(peaks.get("bf16_tflops", 1720.0))
+        peak_tf = float(peaks.get("bf16_tflops", 989.0))   # fallback: H100 SXM data sheet, dense FP16 / BF16
         ach = flops / float(dt.item()) / 1e12
         line["roofline"] = {"bound": "tensor", "achieved": ach, "peak": peak_tf * world, "unit": "TFLOP/s", "frac": ach / (peak_tf * world),
-                            "traffic": None, "kernel": "whole cross-encoder forward (linear_tcgen05 + attention + LayerNorm), wall clock incl. host packing",
-                            "peak_source": "MEASURED_PEAKS.json bf16_tflops" if peaks else "fallback 1720 TFLOP/s"}
+                            "traffic": None, "kernel": "whole cross-encoder forward (linear_wgmma + attention + LayerNorm), wall clock incl. host packing",
+                            "peak_source": "MEASURED_PEAKS.json bf16_tflops" if peaks else "fallback 989 TFLOP/s (H100 SXM data sheet)"}
         if world == 1 and not args.no_cpu_baseline:
             from oracle import rerank as orr     # checker / CPU arm only: float32 transformers forward on a bounded sample
             model = orr.seeded_model(seed=0)
@@ -340,6 +374,8 @@ def run_rerank(args: argparse.Namespace, w: dict) -> None:
             t1 = time.perf_counter(); orr.hf_logits(model, ids[:n], types[:n]); cdt = time.perf_counter() - t1
             line["cpu_baseline"] = {"value": n / cdt, "unit": "pairs/s", "cores": torch.get_num_threads(), "kind": "port",
                                     "sample": f"{n} pairs, transformers BertForSequenceClassification fp32 (oracle.rerank.hf_logits)"}
+        if args.dump_outputs:   # (one GPU: every pair is this rank's)
+            dump_outputs(args.dump_outputs, {"logits": logits, "scores": scores, "order": order})
         sys.stdout.flush(); os.dup2(saved, 1); print(json.dumps(line), flush=True); os.dup2(2, 1)
     if world > 1:
         dist.barrier(); dist.destroy_process_group()
@@ -513,7 +549,7 @@ def run_pool(args: argparse.Namespace, w: dict) -> None:
         peaks = json.loads((ROOT / "MEASURED_PEAKS.json").read_text())
     except (OSError, ValueError):
         pass
-    hbm = float(peaks.get("hbm_gbs", 6650.0))
+    hbm = float(peaks.get("hbm_gbs", 3350.0))   # fallback: H100 SXM data sheet
     ach = alg_bytes / (ms * 1e-3) / 1e9
     line = {"metric": "late-chunking pool token rows/sec", "value": T / (ms * 1e-3), "unit": "token rows/s", "n_gpus": 1,
             "steps": args.steps, "warmup": max(args.warmup, 3), "ms_per_step": ms, "higher_is_better": True, "scaling": "weak",
@@ -525,7 +561,7 @@ def run_pool(args: argparse.Namespace, w: dict) -> None:
             "gpu_launches": args.steps, "roofline": {"bound": "hbm", "achieved": ach, "peak": hbm, "unit": "GB/s", "frac": ach / hbm,
                                                      "traffic": None, "kernel": "segment_mean_pool_kernel", "kernel_ms": ms,
                                                      "algorithmic_bytes": alg_bytes,
-                                                     "peak_source": "MEASURED_PEAKS.json hbm_gbs" if peaks else "fallback 6650 GB/s"},
+                                                     "peak_source": "MEASURED_PEAKS.json hbm_gbs" if peaks else "fallback 3350 GB/s (H100 SXM data sheet)"},
             "clocks": clocks, "check": {"segments": 4, "max_fp16_ulp": ulp_max}}
     if not args.no_cpu_baseline:
         n = 32
@@ -536,6 +572,9 @@ def run_pool(args: argparse.Namespace, w: dict) -> None:
         cdt = time.perf_counter() - t1
         line["cpu_baseline"] = {"value": n * T_seg / cdt, "unit": "token rows/s", "cores": 1, "kind": "port",
                                 "sample": f"{n} segments x {T_seg} x {d} (oracle.pool.late_chunk_pool, NumPy float64, 1 thread of pooling)"}
+    if args.dump_outputs:   # the pooled fp16 rows of the last timed launch: a fixed sample of 4096 of them
+        pick = np.sort(np.random.default_rng(0).choice(S, size=min(S, 4096), replace=False))
+        dump_outputs(args.dump_outputs, {"pooled_rows": got[pick], "pooled_row_index": pick})
     sys.stdout.flush(); os.dup2(saved, 1); print(json.dumps(line), flush=True); os.dup2(2, 1)
     _ = world
 
@@ -636,6 +675,8 @@ def main() -> None:  # noqa: PLR0915
         out = device_step(flags=RL_FLAG_TIME_KERNELS)
     ev1.record()
     barrier()
+    if args.dump_outputs and rank == 0:   # (sim, chunk, count, status) of the last timed step, as the pipeline returns them
+        dump_outputs(args.dump_outputs, {name: t.cpu().numpy() for name, t in zip(("hit_sim", "hit_chunk", "hit_count", "status"), out)})
     windows.append((w0, time.perf_counter()))
     ms_total = ev0.elapsed_time(ev1)
     t = torch.tensor([ms_total], dtype=torch.float64, device=device)
@@ -679,40 +720,27 @@ def main() -> None:  # noqa: PLR0915
     S = max(1, stats["sample_stride"])
     n_blocks = (n_rows + 127) // 128
     main_rows = min(n_rows, (n_blocks - (n_blocks + S - 1) // S) * 128)
-    groups = (B + 255) // 256
+    groups = (B + 127) // 128   # query groups of the tensor-core scan
     alg_bytes = main_rows * d * esize + main_rows * 4 + B * d * 4    # corpus rows once + inv_norm + queries (SURVEY 8d)
     peaks = {}
     try:
         peaks = json.loads((ROOT / "MEASURED_PEAKS.json").read_text())
     except Exception:  # noqa: BLE001
         pass
-    hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
-    traffic = None
-    try:   # dram__bytes_read.sum + dram__bytes_write.sum of this kernel from the committed ncu --set full capture
-        for name in ("r02_traffic.json", "r01_traffic.json"):
-            f = ROOT / "profiles" / name
-            if not f.exists():
-                continue
-            tr = json.loads(f.read_text()).get(w["name"])
-            if (tr and w["chunks"] == WORKLOADS[w["name"]]["chunks"] and B == WORKLOADS[w["name"]]["batch"]
-                    and not args.exact_maxsim and args.storage == "fp32" and args.data == "gaussian"):
-                traffic = tr["traffic_bytes_per_launch"]
-                break
-    except Exception:  # noqa: BLE001
-        pass
+    hbm_peak = float(peaks.get("hbm_gbs", 3350.0))   # fallback: H100 SXM data sheet
+    traffic = None   # measured DRAM bytes of the launch: not available without a hardware profiler
     achieved = alg_bytes / (scan_ms * 1e-3) / 1e9 if scan_ms > 0 else 0.0
     flops = 2.0 * B * main_rows * d
     tensor_peak = peaks.get("bf16_tflops_sustained") or peaks.get("bf16_tflops")
     roofline = {"bound": "hbm", "achieved": achieved, "peak": hbm_peak, "unit": "GB/s", "frac": achieved / hbm_peak,
                 "traffic": traffic, "kernel": "main scan (emit mode), algo=%s" % {1: "fp32", 2: "tcgen05"}.get(stats["algo"], "?"),
                 "kernel_ms": scan_ms, "algorithmic_bytes": alg_bytes, "query_groups_per_launch": groups,
-                "peak_source": "MEASURED_PEAKS.json hbm_gbs (of measured)" if peaks else "fallback 6650 GB/s (of fallback)",
+                "peak_source": "MEASURED_PEAKS.json hbm_gbs (of measured)" if peaks else "fallback 3350 GB/s (H100 SXM data sheet)",
                 "tensor_tflops": flops / (scan_ms * 1e-3) / 1e12 if scan_ms > 0 else 0.0,
                 "tensor_peak_tflops": tensor_peak,
                 "tensor_frac": (flops / (scan_ms * 1e-3) / 1e12 / tensor_peak) if (tensor_peak and scan_ms > 0) else None}
     # Which roof binds: the arithmetic intensity of the launch (2*B*d flop per row of esize*d bytes) against the ridge of
-    # the measured peaks.  fp32 corpus, B = 256: 128 flop/B, below the ridge (~229) -> HBM.  configs[2] (B = 1024) and the
-    # fp16 layout at B = 256 (256 flop/B; ncu: tensor pipe 81 % active at the power-capped clock) are past it -> tensor.
+    # the measured peaks (2*B*d / (esize*d) = 128 flop/B for an fp32 corpus at B = 256).
     ridge = (tensor_peak * 1e12) / (hbm_peak * 1e9) if tensor_peak else None
     roofline["flop_per_byte"] = flops / alg_bytes
     roofline["ridge_flop_per_byte"] = ridge

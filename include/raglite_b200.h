@@ -1,4 +1,4 @@
-/* raglite_b200 -- C-ABI of the B200-native RAGLite retrieval hot path.
+/* raglite_b200 -- C-ABI of the H100-native (sm_90a) RAGLite retrieval hot path.
  *
  * Every entry point takes plain device/host pointers, sizes and a CUDA stream handle
  * (`void* stream` == cudaStream_t); there are no torch / C++ types in any signature.
@@ -38,7 +38,7 @@ extern "C" {
 /* Scan kernel selection. */
 #define RL_ALGO_AUTO 0
 #define RL_ALGO_FP32 1    /* exact fp32 CUDA-core scan (any d) */
-#define RL_ALGO_TCGEN05 2 /* fp16-input tcgen05/TMEM coarse scan + exact rescoring (d % 4 == 0) */
+#define RL_ALGO_TCGEN05 2 /* fp16-input tensor-core (wgmma) coarse scan + exact rescoring (d % 4 == 0) */
 
 /* rl_maxsim_topk flags. */
 #define RL_FLAG_REUSE_THRESHOLDS 1u /* skip the sample pass; use thresholds left in the workspace */

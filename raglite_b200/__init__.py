@@ -1,4 +1,4 @@
-"""raglite_b200 -- B200-native (sm_100a) implementation of RAGLite's retrieval hot path.
+"""raglite_b200 -- H100-native (sm_90a) implementation of RAGLite's retrieval hot path.
 
 Drop-in surface (reference ``raglite/__init__.py`` names for this path): ``RAGLiteConfig``,
 ``vector_search``, ``rerank_chunks``, ``embed_strings``; plus the device-resident ``CorpusIndex`` /

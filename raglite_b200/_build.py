@@ -1,4 +1,4 @@
-"""Build libraglite_b200.so in-tree with nvcc for sm_100a (no torch extension machinery: the library
+"""Build libraglite_b200.so in-tree with nvcc for sm_90a (no torch extension machinery: the library
 is a plain C-ABI shared object, see include/raglite_b200.h)."""
 
 from __future__ import annotations
@@ -15,7 +15,7 @@ LIB_PATH = LIB_DIR / "libraglite_b200.so"
 
 NVCC_FLAGS = [
     "-shared", "-Xcompiler", "-fPIC", "-std=c++17", "-O3", "-lineinfo",
-    "-gencode", "arch=compute_100a,code=sm_100a", "--expt-extended-lambda",
+    "-gencode", "arch=compute_90a,code=sm_90a", "--expt-extended-lambda",
 ]
 
 
@@ -39,7 +39,7 @@ def is_stale() -> bool:
 
 
 def build(force: bool = False, verbose: bool = False) -> Path:
-    """Compile every CUDA source into ``raglite_b200/lib/libraglite_b200.so`` (sm_100a only)."""
+    """Compile every CUDA source into ``raglite_b200/lib/libraglite_b200.so`` (sm_90a only)."""
     if not force and not is_stale():
         return LIB_PATH
     nvcc = _nvcc()
@@ -57,7 +57,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
             if not force and not is_stale():
                 return LIB_PATH
             tmp = LIB_PATH.with_suffix(f".so.tmp{os.getpid()}")
-            extra = os.environ.get("RL_NVCC_EXTRA", "").split()   # A/B builds on the GPU box (e.g. -DRL_EPI_SIGN=0)
+            extra = os.environ.get("RL_NVCC_EXTRA", "").split()   # extra nvcc flags for experimental builds
             cmd = [nvcc, *NVCC_FLAGS, *extra, "-o", str(tmp), *[str(s) for s in sources()]]
             if verbose:
                 cmd.insert(1, "-Xptxas=-v")

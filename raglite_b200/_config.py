@@ -42,7 +42,7 @@ def _vector_search(
 
 def _default_reranker() -> Any:
     """``_config.py:73-79``: ``{"en": ms-marco-MiniLM-L-12-v2, "other": ms-marco-MultiBERT-L-12}``,
-    here as B200 cross-encoder rankers that load their weights lazily from ``cache_path``."""
+    here as GPU cross-encoder rankers that load their weights lazily from ``cache_path``."""
     from ._rerank import B200CrossEncoderRanker
 
     return {

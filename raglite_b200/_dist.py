@@ -1,7 +1,7 @@
 """Row-sharded corpus across the GPUs of one box: one process per GPU, each scans its shard, then a
 SINGLE all-gather of the per-shard hit lists (NCCL over NVLink) and a local merge on every rank.
 
-The reference has no distributed path (SURVEY.md section 2.1); this is the B200-native equivalent of
+The reference has no distributed path (SURVEY.md section 2.1); this is the H100-native equivalent of
 "one big chunk_embedding table": chunks are partitioned into contiguous ranges (never splitting a
 chunk's vectors), queries are replicated, and ``GROUP BY chunk / ORDER BY / LIMIT`` (_search.py:143-150)
 runs over the gathered top-``num_hits`` vectors, which is exactly what a single table would produce.

@@ -3,7 +3,7 @@
 The reference calls ``reranker.rank(query=, docs=)`` (``_search.py:395``) on a ``rerankers``
 FlashRankRanker: tokenise (query, passage) pairs, run ms-marco-MiniLM-L-12-v2 (BERT, 12 layers, H=384,
 12 heads, FFN=1536) with onnxruntime, sigmoid the logit, sort.  Here the forward runs in
-``rl_xenc_score`` (hand-written CUDA: tcgen05 linear layers with fused bias/GELU, attention,
+``rl_xenc_score`` (hand-written CUDA: wgmma linear layers with fused bias/GELU, attention,
 LayerNorm, pooler+classifier) on packed variable-length batches -- no padding tokens are computed.
 """
 

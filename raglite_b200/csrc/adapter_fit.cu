@@ -1,4 +1,4 @@
-// Query-adapter FIT on the device (SURVEY.md section 8f-4; reference _query_adapter.py:21-38, 172-183), sm_100a.
+// Query-adapter FIT on the device (SURVEY.md section 8f-4; reference _query_adapter.py:21-38, 172-183), sm_90a.
 //
 //   rl_best_vectors     For every (eval, retrieved chunk): the chunk's vector with the largest inner product with
 //                       the eval's query -- argmax(chunk.embedding_matrix @ q), _query_adapter.py:172-183 -- copied

@@ -5,7 +5,7 @@
 #include <mutex>
 
 #include "scan_common.cuh"
-#include "scan_tcgen05.cuh"
+#include "scan_wgmma.cuh"
 #include "select_finalize.cuh"
 
 namespace rl {
@@ -78,11 +78,11 @@ int make_layout(const rl_scan_params* p, int sm_count, Layout* L) {
   L->n_blocks = (p->n_rows + kBlockRows - 1) / kBlockRows;
 
   int algo = p->algo;
-  const bool tc_ok = tcgen05_supported(p);
+  const bool tc_ok = wgmma_scan_supported(p);
   if (algo == RL_ALGO_AUTO) algo = tc_ok ? RL_ALGO_TCGEN05 : RL_ALGO_FP32;
   RL_REQUIRE(algo == RL_ALGO_FP32 || algo == RL_ALGO_TCGEN05, RL_EINVAL, "unknown algo %d", p->algo);
   RL_REQUIRE(p->e_dtype == 0 || algo == RL_ALGO_TCGEN05, RL_EUNSUPPORTED,
-             "float16 storage needs the tcgen05 scan (d %% 8 == 0, ld %% 8 == 0, 16-byte aligned E)");
+             "float16 storage needs the tensor-core scan (d %% 8 == 0, ld %% 8 == 0, 16-byte aligned E)");
   RL_REQUIRE(algo != RL_ALGO_TCGEN05 || tc_ok, RL_EUNSUPPORTED,
              "RL_ALGO_TCGEN05 needs d %% 4 == 0, ld %% 4 == 0, 16-byte aligned E and a supported metric");
   L->algo = algo;
@@ -134,7 +134,7 @@ int make_layout(const rl_scan_params* p, int sm_count, Layout* L) {
   L->off_hist = take(B * kHistBins * 4);
   L->off_histw = take(B * 4);
   L->off_cntall = take(B * 4);
-  L->off_qimg = take(algo == RL_ALGO_TCGEN05 ? tcgen05_qimg_bytes(p->B, p->d) : 0);
+  L->off_qimg = take(algo == RL_ALGO_TCGEN05 ? wgmma_qimg_bytes(p->B, p->d) : 0);
   L->off_dump = take(B * (size_t)L->n_sample_rows * 4);
   L->off_cand = take(B * (size_t)L->cap * sizeof(Cand));
   L->total = off;
@@ -169,14 +169,14 @@ extern "C" int rl_device_info(int* sm_count, int* cc_major, int* cc_minor, size_
 
 extern "C" size_t rl_maxsim_workspace_bytes(const rl_scan_params* p) {
   Layout L;
-  if (make_layout(p, 148, &L) != RL_OK) return 0;
+  if (make_layout(p, 132, &L) != RL_OK) return 0;
   return L.total;
 }
 
 extern "C" int rl_maxsim_topk(const rl_scan_params* p, float* hit_sim, int64_t* hit_chunk, int32_t* hit_count,
                               int32_t* status, void* workspace, size_t workspace_bytes, void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
-  int sms = 148;
+  int sms = 132;
   int rc = device_sm_count(&sms);
   if (rc != RL_OK) return rc;
   Layout L;
@@ -225,7 +225,7 @@ extern "C" int rl_maxsim_topk(const rl_scan_params* p, float* hit_sim, int64_t* 
   if (rc != RL_OK) return rc;
   ++launches;
   if (L.algo == RL_ALGO_TCGEN05) {
-    rc = tcgen05_prepare_queries(p, q_inv, q_scale, qimg, stream);
+    rc = wgmma_prepare_queries(p, q_inv, q_scale, qimg, stream);
     if (rc != RL_OK) return rc;
     ++launches;
   }
@@ -245,7 +245,7 @@ extern "C" int rl_maxsim_topk(const rl_scan_params* p, float* hit_sim, int64_t* 
     a.dump_mode = dump_mode;
     a.n_mode_blocks = n_mode_blocks;
     ++launches;
-    if (L.algo == RL_ALGO_TCGEN05) return launch_scan_tcgen05(a, p, q_scale, qimg, sms, stream);
+    if (L.algo == RL_ALGO_TCGEN05) return launch_scan_wgmma(a, p, q_scale, qimg, sms, stream);
     return launch_scan_fp32(a, stream);
   };
 
@@ -285,7 +285,7 @@ extern "C" int rl_maxsim_topk(const rl_scan_params* p, float* hit_sim, int64_t* 
 extern "C" int rl_maxsim_count_at_least(const rl_scan_params* p, const float* sim_floor, int bound, int32_t* counts,
                                         void* workspace, size_t workspace_bytes, void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
-  int sms = 148;
+  int sms = 132;
   int rc = device_sm_count(&sms);
   if (rc != RL_OK) return rc;
   Layout L;
@@ -319,7 +319,7 @@ extern "C" int rl_maxsim_count_at_least(const rl_scan_params* p, const float* si
   rc = launch_query_prep(p->Q, p->B, p->d, p->metric, L.algo, p->row_stats, q_sq, q_inv, eps, stream);
   if (rc != RL_OK) return rc;
   if (L.algo == RL_ALGO_TCGEN05) {
-    rc = tcgen05_prepare_queries(p, q_inv, q_scale, qimg, stream);
+    rc = wgmma_prepare_queries(p, q_inv, q_scale, qimg, stream);
     if (rc != RL_OK) return rc;
   }
   rc = launch_sim_floor_to_thr(sim_floor, q_sq, eps, p->metric, bound, p->B, thr, stream);
@@ -337,7 +337,7 @@ extern "C" int rl_maxsim_count_at_least(const rl_scan_params* p, const float* si
   a.sel_count = 0x7fffffff;
   a.dump_mode = 0;
   a.n_mode_blocks = L.n_blocks;
-  rc = L.algo == RL_ALGO_TCGEN05 ? launch_scan_tcgen05(a, p, q_scale, qimg, sms, stream) : launch_scan_fp32(a, stream);
+  rc = L.algo == RL_ALGO_TCGEN05 ? launch_scan_wgmma(a, p, q_scale, qimg, sms, stream) : launch_scan_fp32(a, stream);
   if (rc != RL_OK) return rc;
   RL_CUDA_CHECK(cudaMemcpyAsync(counts, cand_cnt, (size_t)p->B * 4, cudaMemcpyDeviceToDevice, stream));
   return RL_OK;
@@ -382,7 +382,7 @@ extern "C" int rl_maxsim_stats(const rl_scan_params* p, const void* workspace, r
   cudaStream_t stream = (cudaStream_t)stream_;
   RL_REQUIRE(p && workspace && out, RL_EINVAL, "rl_maxsim_stats: null pointer");
   Layout L;
-  int rc = make_layout(p, 148, &L);
+  int rc = make_layout(p, 132, &L);
   if (rc != RL_OK) return rc;
   memset(out, 0, sizeof(*out));
   if (p->B == 0 || p->n_rows == 0) return RL_OK;
@@ -417,7 +417,7 @@ extern "C" int rl_maxsim_copy_dump(const rl_scan_params* p, const void* workspac
                                    void* stream) {
   RL_REQUIRE(p && workspace && n_sample_rows, RL_EINVAL, "rl_maxsim_copy_dump: null pointer");
   Layout L;
-  int rc = make_layout(p, 148, &L);
+  int rc = make_layout(p, 132, &L);
   if (rc != RL_OK) return rc;
   *n_sample_rows = L.n_sample_rows;
   if (dst != nullptr && p->B > 0 && L.n_sample_rows > 0) {
@@ -479,7 +479,7 @@ __global__ void unfiltered_bound_kernel(const Header* hdr, const int32_t* cand_c
 extern "C" int rl_maxsim_unfiltered_bound(const rl_scan_params* p, const void* workspace, int64_t* bound, void* stream) {
   RL_REQUIRE(p && workspace && bound, RL_EINVAL, "rl_maxsim_unfiltered_bound: null pointer");
   Layout L;
-  int rc = make_layout(p, 148, &L);
+  int rc = make_layout(p, 132, &L);
   if (rc != RL_OK) return rc;
   if (p->B == 0) return RL_OK;
   const unsigned char* ws = static_cast<const unsigned char*>(workspace);
@@ -490,5 +490,3 @@ extern "C" int rl_maxsim_unfiltered_bound(const rl_scan_params* p, const void* w
   return RL_OK;
 }
 
-// (not declared in the public header: a build-time diagnostic used by tools/probe_attrs.py)
-extern "C" int rl_debug_scan_kernel_attrs(int which, int* out) { return rl::debug_scan_kernel_attrs(which, out); }

@@ -1,4 +1,4 @@
-// Shared helpers for the raglite_b200 CUDA sources (sm_100a only).
+// Shared helpers for the raglite_b200 CUDA sources (sm_90a only).
 #pragma once
 
 #include <cuda_runtime.h>

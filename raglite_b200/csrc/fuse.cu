@@ -1,4 +1,4 @@
-// The steps right after the scan, batched on device chunk indices (SURVEY.md section 8f-3, sm_100a):
+// The steps right after the scan, batched on device chunk indices (SURVEY.md section 8f-3, sm_90a):
 //
 //   rl_rrf_fuse      Reciprocal Rank Fusion of R rankings per query (reference _search.py:233-254, as used by
 //                    hybrid_search :257-280): score(c) = sum_r w_r / (k + position of c in ranking r), ordered

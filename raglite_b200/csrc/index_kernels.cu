@@ -1,4 +1,4 @@
-// Index-build kernels, query-adapter apply and the late-chunking pool (sm_100a).
+// Index-build kernels, query-adapter apply and the late-chunking pool (sm_90a).
 //
 //   rl_row_stats         -- per-row norms of the resident embedding matrix
 //   rl_chunk_row_map     -- CSR chunk offsets -> per-row owner
@@ -269,7 +269,7 @@ extern "C" int rl_row_stats(const float* E, int64_t n_rows, int d, int64_t ld, f
   if (n_rows == 0) return RL_OK;
   RL_REQUIRE(E && inv_norm && sq_norm, RL_EINVAL, "rl_row_stats: null pointer");
   const int64_t blocks = (n_rows + 7) / 8;
-  const int grid = (int)(blocks < 148 * 16 ? blocks : 148 * 16);
+  const int grid = (int)(blocks < 132 * 16 ? blocks : 132 * 16);
   row_stats_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(E, n_rows, d, ld, inv_norm, sq_norm, stats);
   RL_CUDA_CHECK(cudaGetLastError());
   return RL_OK;
@@ -283,7 +283,7 @@ extern "C" int rl_row_stats_f16(const void* E, int64_t n_rows, int d, int64_t ld
   if (n_rows == 0) return RL_OK;
   RL_REQUIRE(E && inv_norm && sq_norm, RL_EINVAL, "rl_row_stats_f16: null pointer");
   const int64_t blocks = (n_rows + 7) / 8;
-  const int grid = (int)(blocks < 148 * 16 ? blocks : 148 * 16);
+  const int grid = (int)(blocks < 132 * 16 ? blocks : 132 * 16);
   row_stats_f16_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const __half*>(E), n_rows, d, ld, inv_norm,
                                                                sq_norm, stats);
   RL_CUDA_CHECK(cudaGetLastError());
@@ -295,7 +295,7 @@ extern "C" int rl_chunk_row_map(const int64_t* chunk_off, int64_t n_chunks, int3
   if (n_chunks == 0) return RL_OK;
   RL_REQUIRE(chunk_off && row_chunk, RL_EINVAL, "rl_chunk_row_map: null pointer");
   const int64_t blocks = (n_chunks + 255) / 256;
-  const int grid = (int)(blocks < 148 * 8 ? blocks : 148 * 8);
+  const int grid = (int)(blocks < 132 * 8 ? blocks : 132 * 8);
   chunk_row_map_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(chunk_off, n_chunks, row_chunk);
   RL_CUDA_CHECK(cudaGetLastError());
   return RL_OK;
@@ -340,7 +340,7 @@ extern "C" int rl_row_mask(const uint8_t* chunk_ok, const int32_t* row_chunk, co
                  (reinterpret_cast<uintptr_t>(alive) & 15) == 0,
              RL_EINVAL, "rl_row_mask: row_chunk, alive and out must be 16-byte aligned");
   const int64_t blocks = (n_rows / 16 + 255) / 256 + 1;
-  const int grid = (int)(blocks < 148 * 8 ? blocks : 148 * 8);
+  const int grid = (int)(blocks < 132 * 8 ? blocks : 132 * 8);
   row_mask_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(chunk_ok, row_chunk, alive, n_rows, out);
   RL_CUDA_CHECK(cudaGetLastError());
   return RL_OK;

@@ -1,4 +1,4 @@
-// Arguments shared by the two scan kernels (fp32 CUDA-core and tcgen05) and their epilogues.
+// Arguments shared by the two scan kernels (fp32 CUDA-core and tensor-core wgmma) and their epilogues.
 #pragma once
 #include "common.cuh"
 

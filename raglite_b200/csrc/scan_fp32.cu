@@ -1,5 +1,5 @@
 // Exact fp32 CUDA-core scan (RL_ALGO_FP32): S = Q E^T tile by tile with a fused key / threshold /
-// emit epilogue.  General shapes (any d, any alignment); the tcgen05 scan is the fast path.
+// emit epilogue.  General shapes (any d, any alignment); the wgmma scan is the fast path.
 //
 // Replaces the per-row distance expression DuckDB evaluates for vector_search
 // (reference _search.py:69-79, _typing.py:123-134).

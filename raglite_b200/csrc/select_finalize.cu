@@ -1,4 +1,4 @@
-// Selection side of the MaxSim scan (sm_100a): query prep, the radix select that turns the sampled
+// Selection side of the MaxSim scan (sm_90a): query prep, the radix select that turns the sampled
 // scores into per-query emission thresholds, the finalize pass (radix select over the candidate
 // list, exact float64 rescoring with warp-shuffle reductions, bitonic sort, GROUP BY chunk) and the
 // cross-shard merge.
@@ -203,7 +203,7 @@ __global__ void __launch_bounds__(128) query_prep_kernel(const float* __restrict
     q_inv[b] = nq > 0.0 ? (float)(1.0 / sqrt(nq)) : 0.f;
     const float max_norm = row_stats ? row_stats[0] : 1.f;
     // Worst-case error of the approximate key in key units.  fp32 scan: accumulation error
-    // <= d * 2^-24 * |q||e| (doubled for slack); fp16-input tcgen05 scan: inputs rounded to 11 bits
+    // <= d * 2^-24 * |q||e| (doubled for slack); fp16-input tensor-core scan: inputs rounded to 11 bits
     // => 2^-10 (1 + 2^-11) |q||e| plus fp32 accumulation plus fp16 subnormal absolute terms.
     const float base = algo == RL_ALGO_TCGEN05 ? (1.25e-3f + (float)(d + 8) * 1.1920929e-7f)
                                                : (float)(d + 8) * 1.1920929e-7f;

@@ -1,12 +1,12 @@
-// BERT cross-encoder forward (ms-marco-MiniLM-L-12 architecture) for sm_100a: the arithmetic behind
+// BERT cross-encoder forward (ms-marco-MiniLM-L-12 architecture) for sm_90a: the arithmetic behind
 // rerank_chunks (reference _search.py:364-397 -> rerankers FlashRankRanker -> onnxruntime, all
 // third-party).  Variable-length packed batches (no padding): tokens [T, H], cu_seqlens [P + 1].
 //
 //   embed_ln_kernel      word + position + token-type embeddings, LayerNorm          (fp32 math, fp16 out)
-//   linear_tcgen05_kernel  Y = act(X W^T + b): tcgen05.mma (M=128 tokens, N<=256 outputs per pass, K
-//                        sliced by 64), X copied into 128B-swizzled smem by loader warps, W as a
-//                        pre-swizzled fp16 image fetched with cp.async.bulk, fp32 accumulate in TMEM,
-//                        bias / GELU(erf) fused in the TMEM epilogue
+//   linear_wgmma_kernel  Y = act(X W^T + b): wgmma (M=128 tokens, N<=128 outputs per pass, K
+//                        sliced by 64), X through a TMA tensor map into 128B-swizzled smem, W as a
+//                        pre-swizzled fp16 image fetched with cp.async.bulk, fp32 accumulate in
+//                        registers, bias / GELU(erf) fused in the epilogue
 //   attention_kernel     softmax(Q K^T / sqrt(dh)) V per (sequence, head), fp32 math
 //   add_ln_kernel        LayerNorm(x + residual)
 //   cls_head_kernel      pooler (dense + tanh on [CLS]) -> classifier -> logit, sigmoid score
@@ -18,30 +18,28 @@
 #include <mutex>
 
 #include "common.cuh"
-#include "tcgen05_ptx.cuh"
+#include "hopper_ptx.cuh"
 
 namespace rl {
 namespace {
 
 using namespace tc;
 
-constexpr int kTileM = 128;
-constexpr int kSliceK = 64;
-constexpr int kMaxN = 256;
-constexpr int kNumEpiWarps = 8;   // warp w reads TMEM lane quarter w % 4; warps 4..7 take the odd 32-column chunks
-constexpr int kMmaWarp = 8;
-constexpr int kWWarp = 9;
-constexpr int kFirstLoaderWarp = 10;
-constexpr int kNumLoaderWarps = 8;
-constexpr int kLoadDepth = 3;     // activation K-slices in flight per loader thread (registers)
-constexpr uint32_t kBarBytes = 256;                         // mbarriers + TMEM base pointer
-constexpr uint32_t kEpiPitch = 80;                          // bytes per staged row: 64 B of fp16 + pad (conflict-free 16 B stores)
-constexpr uint32_t kEpiWarpBytes = 32 * kEpiPitch;          // one 32 x 32 output chunk per epilogue warp
-constexpr uint32_t kEpiBytes = kNumEpiWarps * kEpiWarpBytes;
-constexpr int kThreads = (kFirstLoaderWarp + kNumLoaderWarps) * 32;
+constexpr int kTileM = 128;          // tokens per tile (two consumer warpgroups of M = 64)
+constexpr int kSliceK = 64;          // fp16 elements per K slice = one 128-byte swizzle row
+constexpr int kPassN = 128;          // output columns per pass (wgmma N)
+constexpr int kLinConsumerWarps = 8;
+constexpr int kLinProdWarp = 8;
+constexpr int kLinThreads = (kLinConsumerWarps + 1) * 32;
 constexpr int kMaxStages = 8;
 constexpr int kABytes = kTileM * 128;
-constexpr uint32_t kSmemBudget = 226 * 1024;
+// Activations + weight slice: 32 KB.  The wgmma always reads kPassN weight rows; the short last pass of a layer
+// copies only its nb rows, so the rest of the stage's weight region holds stale rows.  They stay inside the stage and
+// only feed accumulator columns >= nb, which the epilogue never stores.
+constexpr uint32_t kLinStageBytes = kABytes + kPassN * 128u;
+constexpr uint32_t kEpiPitch = kPassN * 2 + 16;                 // bytes per staged row: 256 B of fp16 + pad (conflict-free)
+constexpr uint32_t kEpiBytes = kTileM * kEpiPitch;
+constexpr uint32_t kSmemBudget = 227 * 1024;
 
 __device__ __forceinline__ uint32_t pack_half2(float a, float b) {
   const __half2 h = __floats2half2_rn(a, b);
@@ -73,482 +71,156 @@ __device__ __forceinline__ float gelu_erf(float x) {
   return half_x * (x >= 0.f ? 2.f - tail : tail);
 }
 
-// ---- weight image: W[N, K] fp32 row-major -> per (pass, k-slice) swizzled fp16 UMMA B tiles -------------
-// Output columns per pass.  Short-K layers whose width is a multiple of 192 (QKV, out-proj, FFN-up of the
-// MiniLM shapes: K = 384, N = 1152 / 384 / 1536) use 192-column passes: the whole K extent of such a pass
-// (192 x 384 fp16 = 144 KB) stays RESIDENT in shared memory while the CTA walks the token tiles
-// (linear_wres_kernel).  Everything else streams 256-column weight slices (linear_tcgen05_kernel).
-constexpr int kResN = 192;
-constexpr int kResMaxKs = 6;
-__host__ __device__ inline bool use_resident(int N, int K) { return K % kSliceK == 0 && K / kSliceK <= kResMaxKs && N % kResN == 0; }
-__host__ __device__ inline int pass_width(int N, int K) { return use_resident(N, K) ? kResN : kMaxN; }
-
-__host__ __device__ inline int pass_rows(int N, int pass, int pw = kMaxN) {
-  const int rem = N - pass * pw;
-  return rem < pw ? rem : pw;
+// ---- weight image: W[N, K] fp32 row-major -> per (pass, k-slice) swizzled fp16 wgmma B tiles -------------
+// A pass is kPassN output columns; the last pass may be shorter (its slices have that pitch).
+__host__ __device__ inline int pass_rows(int N, int pass) {
+  const int rem = N - pass * kPassN;
+  return rem < kPassN ? rem : kPassN;
 }
-__host__ __device__ inline size_t pass_offset_halves(int N, int K, int pass, int pw = kMaxN) {
+__host__ __device__ inline size_t pass_offset_halves(int K, int pass) {
   const int n_ks = (K + kSliceK - 1) / kSliceK;
-  return (size_t)pass * pw * n_ks * kSliceK;  // full passes precede; only the last pass is short
+  return (size_t)pass * kPassN * n_ks * kSliceK;  // full passes precede; only the last pass is short
 }
 
-__global__ void pack_linear_kernel(const float* __restrict__ W, int N, int K, int pw, __half* __restrict__ img) {
+__global__ void pack_linear_kernel(const float* __restrict__ W, int N, int K, __half* __restrict__ img) {
   const int n_ks = (K + kSliceK - 1) / kSliceK;
   const int64_t total = (int64_t)((N + 15) / 16 * 16) * n_ks * kSliceK;
   for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
        idx += (int64_t)gridDim.x * blockDim.x) {
     const int n = (int)(idx / (n_ks * kSliceK));
     const int kk = (int)(idx % (n_ks * kSliceK));
-    const int pass = n / pw, r = n % pw;
-    const int nb = (pass_rows(N, pass, pw) + 15) / 16 * 16;
+    const int pass = n / kPassN, r = n % kPassN;
+    const int nb = (pass_rows(N, pass) + 15) / 16 * 16;
     const int ks = kk / kSliceK, e = kk % kSliceK;
     const float v = (n < N && kk < K) ? W[(size_t)n * K + kk] : 0.f;
-    const size_t off = pass_offset_halves(N, K, pass, pw) + ((size_t)ks * nb + r) * kSliceK +
+    const size_t off = pass_offset_halves(K, pass) + ((size_t)ks * nb + r) * kSliceK +
                        (size_t)((((e >> 3) ^ (r & 7)) << 3) + (e & 7));
     img[off] = __float2half_rn(v);
   }
 }
 
-// ---- tcgen05 linear layer ---------------------------------------------------------------------------------
+// ---- wgmma linear layer ---------------------------------------------------------------------------------
+// Y[T, N] = act(X W^T + b).  A work item is one (128-token tile, kPassN-column pass); CTA c takes items c, c + grid, ...
+// (passes fastest, so the CTAs working at the same time share their activation tiles in L2).  Per K slice the
+// producer thread issues one TMA tensor-map copy of the activations (box 64 x 128, SWIZZLE_128B: rows past T and
+// columns past K arrive as zeros) and one bulk copy of the pre-swizzled weight slice into a stage; two consumer
+// warpgroups (64 tokens each) run wgmma.m64n128k16 on it and, after the last slice, add the bias, apply the
+// activation, round to fp16 and stage the tile in shared memory so that it leaves as 16-byte row-contiguous stores.
 struct LinArgs {
-  const __half* X;     // [T, K]
   const __half* img;   // packed weights
   const float* bias;   // [N]
   __half* Y;           // [T, N]
   int T, N, K, act;    // act: 0 none, 1 GELU(erf)
   int n_pass, n_ks, stages;
-  int cp_async;        // 1: activation tile through cp.async (no register staging; every free stage in flight)
-  int pw;              // output columns per pass of the weight image (pass_width(N, K))
 };
 
-// 16-byte asynchronous global -> shared copy (zero-fills when src_bytes == 0) and the mbarrier arrive
-// that fires once all of this thread's earlier cp.async have landed.
-__device__ __forceinline__ void cp_async_16(uint32_t dst_smem, const void* src, uint32_t src_bytes) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst_smem), "l"(src), "r"(src_bytes) : "memory");
-}
-__device__ __forceinline__ void cp_async_mbar_arrive_noinc(uint64_t* bar) {
-  asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
-__host__ __device__ inline uint32_t lin_stage_bytes() { return kABytes + kMaxN * 128u; }
-
-// MC: a cluster of two CTAs works on two token tiles of the SAME output pass; every weight slice is fetched from
-// L2 once per cluster -- CTA r issues half r with .multicast::cluster, it lands at the same offset in both CTAs --
-// so the L2 -> SM weight stream, which bounds the K = 1536 layer (FFN-down: 590 KB of weights per 128-token
-// tile, 788 MB per launch at ~8.7 TB/s), halves.  A stage is refilled only when BOTH CTAs' MMAs have released
-// it: the commit that frees a stage is multicast to both CTAs' empty barriers (count 2).
-template <bool MC>
-__global__ void __launch_bounds__(kThreads, 1) linear_tcgen05_kernel(const LinArgs t) {
+__global__ void __launch_bounds__(kLinThreads, 1) linear_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const LinArgs t) {
   extern __shared__ unsigned char smem_dyn[];
   unsigned char* base = smem_dyn + ((1024u - (smem_u32(smem_dyn) & 1023u)) & 1023u);
-  const uint32_t sbytes = lin_stage_bytes();
-  uint64_t* full = reinterpret_cast<uint64_t*>(base + (size_t)t.stages * sbytes);
+  uint64_t* full = reinterpret_cast<uint64_t*>(base + (size_t)t.stages * kLinStageBytes);
   uint64_t* empty = full + kMaxStages;
-  uint64_t* tmem_full = empty + kMaxStages;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-  unsigned char* epi_stage = base + (size_t)t.stages * sbytes + kBarBytes;
+  unsigned char* epi = reinterpret_cast<unsigned char*>(empty + kMaxStages);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m_tiles = (t.T + kTileM - 1) / kTileM;
-  // item = m_unit * n_pass + pass; a unit is one token tile, or (MC) the pair of tiles 2u, 2u + 1 of a cluster
-  const uint32_t crank = MC ? cluster_ctarank() : 0u;
-  const int m_units = MC ? (m_tiles + 1) / 2 : m_tiles;
-  const int64_t n_items = (int64_t)m_units * t.n_pass;
-  const int64_t first = MC ? blockIdx.x >> 1 : blockIdx.x, stride = MC ? gridDim.x >> 1 : gridDim.x;
+  const int64_t n_items = (int64_t)m_tiles * t.n_pass;
+  const int64_t first = blockIdx.x, stride = gridDim.x;
   const int64_t my_items = first < n_items ? (n_items - first + stride - 1) / stride : 0;
-  auto tile_of = [&](int64_t item) -> int { const int u = (int)(item / t.n_pass); return MC ? 2 * u + (int)crank : u; };
 
   if (threadIdx.x == 0) {
     for (int i = 0; i < t.stages; ++i) {
-      mbar_init(&full[i], (t.cp_async ? kNumLoaderWarps * 32 : kNumLoaderWarps) + 1);
-      mbar_init(&empty[i], MC ? 2 : 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], kNumEpiWarps);
+      mbar_init(&full[i], 1);                    // the producer's expect_tx
+      mbar_init(&empty[i], kLinConsumerWarps);
     }
     fence_barrier_init();
   }
-  if (warp == kMmaWarp) tmem_alloc(tmem_ptr, 512);
-  tc_fence_before();
   __syncthreads();
-  if (MC) cluster_sync_all();   // the peer's barriers are initialised before any multicast / remote commit reaches them
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
-  if (warp >= kFirstLoaderWarp) {
-    // activations: fp16 rows -> swizzled K-major smem tile (UMMA A), 4 x 16-byte chunks per thread and
-    // slice.  The loads of kLoadDepth slices are in flight at once (a register ring that runs across
-    // item boundaries): one memory latency per slice would otherwise bound the whole kernel.
-    const int lt = threadIdx.x - kFirstLoaderWarp * 32;
-    const int j = lt & 7, r0 = lt >> 3;  // chunk j of rows r0 + 32 i
-    const int64_t n_slices = my_items * t.n_ks;
-    auto issue = [&](int64_t g, uint4 (&v)[4]) {
-      if (g >= n_slices) return;
-      const int64_t it = g / t.n_ks;
-      const int ks = (int)(g - it * t.n_ks);
-      const int m_tile = tile_of(first + it * stride);
-      const int col = ks * kSliceK + j * 8;
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int row = m_tile * kTileM + r0 + 32 * i;
-        v[i] = make_uint4(0u, 0u, 0u, 0u);
-        if (row < t.T && col < t.K) v[i] = __ldg(reinterpret_cast<const uint4*>(t.X + (size_t)row * t.K + col));
-      }
-    };
-    int stage = 0;
-    uint32_t phase = 0;
-    auto commit = [&](int64_t g, const uint4 (&v)[4]) {
-      if (g >= n_slices) return;
-      mbar_wait(&empty[stage], phase ^ 1u);
-      unsigned char* A = base + (size_t)stage * sbytes;
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int r = r0 + 32 * i;
-        *reinterpret_cast<uint4*>(A + (uint32_t)r * 128u + (((uint32_t)j ^ ((uint32_t)r & 7u)) << 4)) = v[i];
-      }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&full[stage]);
-      if (++stage == t.stages) { stage = 0; phase ^= 1u; }
-    };
-    if (t.cp_async) {
-      // Experimental (RL_XENC_CPASYNC=1): each thread fires its four 16-byte copies straight into the
-      // swizzled tile and lets the hardware arrive on the stage's barrier when they land, so the
-      // loaders run ahead by as many stages as are free instead of by the depth of a register ring.
-      for (int64_t g = 0; g < n_slices; ++g) {
-        const int64_t it = g / t.n_ks;
-        const int ks = (int)(g - it * t.n_ks);
-        const int m_tile = tile_of(first + it * stride);
-        const int col = ks * kSliceK + j * 8;
-        mbar_wait(&empty[stage], phase ^ 1u);
-        const uint32_t A = smem_u32(base + (size_t)stage * sbytes);
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const int r = r0 + 32 * i;
-          const int row = m_tile * kTileM + r;
-          const bool ok = row < t.T && col < t.K;
-          cp_async_16(A + (uint32_t)r * 128u + (((uint32_t)j ^ ((uint32_t)r & 7u)) << 4),
-                      ok ? t.X + (size_t)row * t.K + col : t.X, ok ? 16u : 0u);
-        }
-        cp_async_mbar_arrive_noinc(&full[stage]);
-        if (++stage == t.stages) { stage = 0; phase ^= 1u; }
-      }
-    } else {
-      static_assert(kLoadDepth == 3, "the register ring below is written out for three slices");
-      uint4 v0[4], v1[4], v2[4];
-      issue(0, v0);
-      issue(1, v1);
-      for (int64_t g = 0; g < n_slices; g += 3) {
-        issue(g + 2, v2);
-        commit(g, v0);
-        issue(g + 3, v0);
-        commit(g + 1, v1);
-        issue(g + 4, v1);
-        commit(g + 2, v2);
-      }
-    }
-  } else if (warp == kWWarp) {
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int64_t it = 0; it < my_items; ++it) {
-        const int64_t item = first + it * stride;
-        const int pass = (int)(item % t.n_pass);
-        const int nb = (pass_rows(t.N, pass, t.pw) + 15) / 16 * 16;
-        const uint32_t wbytes = (uint32_t)nb * 128u;
-        const __half* src = t.img + pass_offset_halves(t.N, t.K, pass, t.pw);
-        for (int ks = 0; ks < t.n_ks; ++ks) {
-          mbar_wait(&empty[stage], phase ^ 1u);
-          mbar_arrive_expect_tx(&full[stage], wbytes);
-          if (MC) {   // this CTA's half of the slice, to both CTAs of the cluster
-            const uint32_t half = wbytes / 2;
-            bulk_g2s_multicast(base + (size_t)stage * sbytes + kABytes + (size_t)crank * half,
-                               reinterpret_cast<const unsigned char*>(src + (size_t)ks * nb * kSliceK) + (size_t)crank * half, half,
-                               &full[stage], (uint16_t)3);
-          } else {
-            bulk_g2s(base + (size_t)stage * sbytes + kABytes, src + (size_t)ks * nb * kSliceK, wbytes, &full[stage]);
-          }
-          if (++stage == t.stages) { stage = 0; phase ^= 1u; }
-        }
-      }
-    }
-  } else if (warp == kMmaWarp) {
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int64_t it = 0; it < my_items; ++it) {
-        const int64_t item = first + it * stride;
-        const int pass = (int)(item % t.n_pass);
-        const int nb = (pass_rows(t.N, pass, t.pw) + 15) / 16 * 16;
-        const uint32_t idesc = make_idesc_f16(kTileM, nb);
-        const int buf = (int)(it & 1);
-        mbar_wait(&tmem_empty[buf], (uint32_t)(((it >> 1) & 1) ^ 1));
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(buf * kMaxN);
-        for (int ks = 0; ks < t.n_ks; ++ks) {
-          mbar_wait(&full[stage], phase);
-          fence_proxy_async();
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(base + (size_t)stage * sbytes);
-          const uint64_t a_desc = make_kmajor_sw128_desc(a_addr);
-          const uint64_t b_desc = make_kmajor_sw128_desc(a_addr + kABytes);
-#pragma unroll
-          for (int k = 0; k < kSliceK / 16; ++k)
-            umma_f16(d_tmem, a_desc + (uint64_t)(2 * k), b_desc + (uint64_t)(2 * k), idesc, (ks | k) != 0 ? 1u : 0u);
-          if (MC) umma_commit_mc(&empty[stage], (uint16_t)3);   // frees the stage in both CTAs (count 2)
-          else umma_commit(&empty[stage]);
-          if (++stage == t.stages) { stage = 0; phase ^= 1u; }
-        }
-        umma_commit(&tmem_full[buf]);
-      }
-    }
-  } else {
-    // epilogue: TMEM -> + bias -> activation -> fp16 -> shared staging -> global.  A thread owns one token
-    // row of the accumulator; the two warps of a lane quarter split the 32-column chunks (even / odd).
-    // Storing straight from the row owner would issue 32 separate 16-byte requests per instruction
-    // (one per row) -- the L2 request rate, not bytes, then bounds the kernel -- so a chunk is staged in
-    // shared memory and written out with 4 lanes per row: 64 contiguous bytes per request.
-    const int q = warp & 3, half = warp >> 2;
-    unsigned char* stg = epi_stage + (size_t)warp * kEpiWarpBytes;
-    for (int64_t it = 0; it < my_items; ++it) {
-      const int64_t item = first + it * stride;
-      const int m_tile = tile_of(item), pass = (int)(item % t.n_pass);
-      const int nb = pass_rows(t.N, pass, t.pw);
-      const int n0 = pass * t.pw;
-      const int buf = (int)(it & 1);
-      const int row_base = m_tile * kTileM + q * 32;
-      mbar_wait(&tmem_full[buf], (uint32_t)((it >> 1) & 1));
-      tc_fence_after();
-      const uint32_t taddr0 = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * kMaxN);
-      // chunks half*32, half*32 + 64, ...  (the sibling warp on the same scheduler hides the TMEM latency)
-      for (int c0 = half * 32; c0 < nb; c0 += 64) {
-        uint32_t v[32];
-        tmem_ld32_async(taddr0 + (uint32_t)c0, v);
-        tmem_ld_wait(v);
-        const float4* b4 = reinterpret_cast<const float4*>(t.bias + n0 + c0);   // n0, c0 multiples of 32
-#pragma unroll
-        for (int jj = 0; jj < 4; ++jj) {
-          uint32_t packed[4];
-#pragma unroll
-          for (int h2 = 0; h2 < 2; ++h2) {
-            const float4 bb = __ldg(b4 + 2 * jj + h2);
-            const int e = 8 * jj + 4 * h2;
-            float x0 = __uint_as_float(v[e]) + bb.x, x1 = __uint_as_float(v[e + 1]) + bb.y;
-            float x2 = __uint_as_float(v[e + 2]) + bb.z, x3 = __uint_as_float(v[e + 3]) + bb.w;
-            if (t.act == 1) { x0 = gelu_erf(x0); x1 = gelu_erf(x1); x2 = gelu_erf(x2); x3 = gelu_erf(x3); }
-            packed[2 * h2] = pack_half2(x0, x1);
-            packed[2 * h2 + 1] = pack_half2(x2, x3);
-          }
-          *reinterpret_cast<uint4*>(stg + (uint32_t)lane * kEpiPitch + (uint32_t)jj * 16u) =
-              make_uint4(packed[0], packed[1], packed[2], packed[3]);
-        }
-        __syncwarp();
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const int rr = i * 8 + (lane >> 2), ch = lane & 3;
-          const uint4 w = *reinterpret_cast<const uint4*>(stg + (uint32_t)rr * kEpiPitch + (uint32_t)ch * 16u);
-          const int grow = row_base + rr;
-          if (grow < t.T) *reinterpret_cast<uint4*>(t.Y + (size_t)grow * t.N + n0 + c0 + ch * 8) = w;
-        }
-        __syncwarp();
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[buf]);
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (MC) cluster_sync_all();   // no CTA leaves while its peer may still multicast into it or commit to its barriers
-  if (warp == kMmaWarp) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
-  }
-}
-
-// ---- tcgen05 linear layer, weights resident in shared memory, activations through a TMA tensor map ---------
-// For K <= 384 and N % 192 == 0.  A CTA owns ONE 192-column pass of the output for the whole launch: it
-// bulk-copies that pass of the pre-swizzled weight image (n_ks x 24 KB) into shared memory once and then
-// walks token tiles.  Per 128-token tile only the activations move: one thread issues a 2-D
-// cp.async.bulk.tensor (TMA tensor map over X[T, K], box 64 x 128, SWIZZLE_128B -- the layout the UMMA
-// A descriptor expects; rows past T are zero-filled by the hardware) per K slice.  That takes the L2 -> SM
-// traffic per tile from 288 KB (activations + a 256-column weight slice per tile) to 96 KB and frees the
-// eight loader warps: twelve epilogue warps (three per TMEM lane quarter, two 32-column chunks each) now
-// drain a 128 x 192 accumulator while the next tile's MMAs run into the other TMEM buffer.
-// Pass width 192, three activation stages.  (kResN = 128 -- 96 KB of resident weights, SIX stages, a whole token
-// tile of TMA loads in flight -- was measured and is slower: QKV 58.1 vs 61.5 us, but out-proj 24.7 vs 22.7 and
-// FFN-up 105.4 vs 90.2: the deeper prefetch does not pay for re-reading the activations 1.5x as often.)
-constexpr int kResEpiWarps = kResN == 128 ? 8 : 12;   // two 32-column chunks per warp either way
-constexpr int kResProdWarp = kResEpiWarps;
-constexpr int kResMmaWarp = kResEpiWarps + 1;
-constexpr int kResThreads = (kResEpiWarps + 2) * 32;
-constexpr int kResStages = kResN == 128 ? 6 : 3;
-constexpr int kResChunkStride = (kResEpiWarps / 4) * 32;   // columns between a warp's two chunks
-static_assert(kResN / 32 == 2 * (kResEpiWarps / 4), "two chunks per epilogue warp");
-constexpr uint32_t kResWSliceBytes = kResN * 128u;                    // one K slice of the pass: 24 KB
-constexpr uint32_t kResEpiBytes = kResEpiWarps * kEpiWarpBytes;
-
-__device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* tmap, int c0, int c1, uint64_t* bar) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(smem_dst)), "l"(tmap), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
-      : "memory");
-}
-
-__global__ void __launch_bounds__(kResThreads, 1) linear_wres_kernel(const __grid_constant__ CUtensorMap tmA, const LinArgs t) {
-  extern __shared__ unsigned char smem_dyn[];
-  unsigned char* base = smem_dyn + ((1024u - (smem_u32(smem_dyn) & 1023u)) & 1023u);
-  unsigned char* w_smem = base;                                               // [n_ks][192 x 128 B]
-  unsigned char* a_smem = w_smem + (size_t)t.n_ks * kResWSliceBytes;          // [kResStages][16 KB]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(a_smem + (size_t)kResStages * kABytes);
-  uint64_t* a_full = bars;                   // [kResStages]
-  uint64_t* a_empty = a_full + kResStages;   // [kResStages]
-  uint64_t* tmem_full = a_empty + kResStages;   // [2]
-  uint64_t* tmem_empty = tmem_full + 2;         // [2]
-  uint64_t* w_full = tmem_empty + 2;            // [1]
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(w_full + 1);
-  unsigned char* epi_stage = reinterpret_cast<unsigned char*>(bars) + kBarBytes;
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int m_tiles = (t.T + kTileM - 1) / kTileM;
-  // grid = n_pass * ctas_per_pass: CTA c serves pass c % n_pass and token tiles c / n_pass, + ctas_per_pass, ...
-  const int pass = (int)(blockIdx.x % (unsigned)t.n_pass);
-  const int first = (int)(blockIdx.x / (unsigned)t.n_pass), stride = (int)(gridDim.x / (unsigned)t.n_pass);
-  const int my_items = first < m_tiles ? (m_tiles - first + stride - 1) / stride : 0;
-
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < kResStages; ++i) {
-      mbar_init(&a_full[i], 1);
-      mbar_init(&a_empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], kResEpiWarps);
-    }
-    mbar_init(w_full, 1);
-    fence_barrier_init();
-  }
-  if (warp == kResMmaWarp) tmem_alloc(tmem_ptr, 512);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-
-  if (warp == kResProdWarp) {
+  if (warp == kLinProdWarp) {
     if (lane == 0 && my_items > 0) {
       asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
-      // the pass's weights: resident for the whole launch
-      const __half* wsrc = t.img + pass_offset_halves(t.N, t.K, pass, kResN);
-      mbar_arrive_expect_tx(w_full, (uint32_t)t.n_ks * kResWSliceBytes);
-      for (int ks = 0; ks < t.n_ks; ++ks)
-        bulk_g2s(w_smem + (size_t)ks * kResWSliceBytes, wsrc + (size_t)ks * kResN * kSliceK, kResWSliceBytes, w_full);
       int stage = 0;
       uint32_t phase = 0;
-      for (int it = 0; it < my_items; ++it) {
-        const int m_tile = first + it * stride;
+      for (int64_t it = 0; it < my_items; ++it) {
+        const int64_t item = first + it * stride;
+        const int m_tile = (int)(item / t.n_pass), pass = (int)(item % t.n_pass);
+        const int nb = (pass_rows(t.N, pass) + 15) / 16 * 16;
+        const uint32_t wbytes = (uint32_t)nb * 128u;
+        const __half* src = t.img + pass_offset_halves(t.K, pass);
         for (int ks = 0; ks < t.n_ks; ++ks) {
-          mbar_wait(&a_empty[stage], phase ^ 1u);
-          mbar_arrive_expect_tx(&a_full[stage], (uint32_t)kABytes);
-          tma_load_2d(a_smem + (size_t)stage * kABytes, &tmA, ks * kSliceK, m_tile * kTileM, &a_full[stage]);
-          if (++stage == kResStages) { stage = 0; phase ^= 1u; }
+          mbar_wait(&empty[stage], phase ^ 1u);
+          unsigned char* st = base + (size_t)stage * kLinStageBytes;
+          mbar_arrive_expect_tx(&full[stage], (uint32_t)kABytes + wbytes);
+          tma_load_2d(st, &tmA, ks * kSliceK, m_tile * kTileM, &full[stage]);
+          bulk_g2s(st + kABytes, src + (size_t)ks * nb * kSliceK, wbytes, &full[stage]);
+          if (++stage == t.stages) { stage = 0; phase ^= 1u; }
         }
       }
     }
-  } else if (warp == kResMmaWarp) {
-    if (lane == 0 && my_items > 0) {
-      const uint32_t idesc = make_idesc_f16(kTileM, kResN);
-      mbar_wait(w_full, 0u);
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int it = 0; it < my_items; ++it) {
-        const int buf = it & 1;
-        mbar_wait(&tmem_empty[buf], (uint32_t)(((it >> 1) & 1) ^ 1));
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(buf * kMaxN);
-        for (int ks = 0; ks < t.n_ks; ++ks) {
-          mbar_wait(&a_full[stage], phase);
-          tc_fence_after();
-          const uint64_t a_desc = make_kmajor_sw128_desc(smem_u32(a_smem + (size_t)stage * kABytes));
-          const uint64_t b_desc = make_kmajor_sw128_desc(smem_u32(w_smem + (size_t)ks * kResWSliceBytes));
-#pragma unroll
-          for (int k = 0; k < kSliceK / 16; ++k)
-            umma_f16(d_tmem, a_desc + (uint64_t)(2 * k), b_desc + (uint64_t)(2 * k), idesc, (ks | k) != 0 ? 1u : 0u);
-          umma_commit(&a_empty[stage]);
-          if (++stage == kResStages) { stage = 0; phase ^= 1u; }
+  } else if (warp < kLinConsumerWarps) {
+    const int wg = warp >> 2, wt = threadIdx.x & 127;
+    const int r_lo = (warp & 3) * 16 + (lane >> 2);   // rows r_lo and r_lo + 8 of this warpgroup's 64
+    const int c_lane = 2 * (lane & 3);
+    unsigned char* stg = epi + (size_t)wg * 64 * kEpiPitch;
+    int stage = 0;
+    uint32_t phase = 0;
+    float acc[64];
+    for (int64_t it = 0; it < my_items; ++it) {
+      const int64_t item = first + it * stride;
+      const int m_tile = (int)(item / t.n_pass), pass = (int)(item % t.n_pass);
+      const int nb = pass_rows(t.N, pass);
+      const int n0 = pass * kPassN;
+      int prev = -1;
+      for (int ks = 0; ks < t.n_ks; ++ks) {
+        mbar_wait(&full[stage], phase);
+        const uint32_t st_addr = smem_u32(base + (size_t)stage * kLinStageBytes);
+        wgmma_fence();
+        wgmma_slice(acc, make_kmajor_sw128_desc(st_addr + (uint32_t)wg * (64u * 128u)), make_kmajor_sw128_desc(st_addr + kABytes),
+                    ks > 0);
+        wgmma_commit();
+        if (prev >= 0) {
+          wgmma_wait<1>();
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&empty[prev]);
         }
-        umma_commit(&tmem_full[buf]);
+        prev = stage;
+        if (++stage == t.stages) { stage = 0; phase ^= 1u; }
       }
-    }
-  } else {
-    // epilogue: warp w drains TMEM lane quarter w % 4 (hardware rule); the three warps of a quarter take the
-    // 32-column chunks {i, i + 3} (i = w / 4).  Bias, activation, fp16, shared staging, 64-byte row stores.
-    // The CTA's pass and each warp's two chunks never change, so the 64 bias values a thread needs live in
-    // registers for the whole launch (ncu: with a bias load in front of every add, the epilogue warps spent a
-    // third of their samples stalled on those loads and set the pace of the kernel).
-    const int q = warp & 3, third = warp >> 2;
-    unsigned char* stg = epi_stage + (size_t)warp * kEpiWarpBytes;
-    const int n0 = pass * kResN;
-    float bias_r[2][32];
-#pragma unroll
-    for (int c = 0; c < 2; ++c) {
-      const float4* b4 = reinterpret_cast<const float4*>(t.bias + n0 + third * 32 + c * kResChunkStride);
-#pragma unroll
-      for (int e = 0; e < 8; ++e) {
-        const float4 bb = __ldg(b4 + e);
-        bias_r[c][4 * e] = bb.x; bias_r[c][4 * e + 1] = bb.y; bias_r[c][4 * e + 2] = bb.z; bias_r[c][4 * e + 3] = bb.w;
-      }
-    }
-    for (int it = 0; it < my_items; ++it) {
-      const int m_tile = first + it * stride;
-      const int buf = it & 1;
-      const int row_base = m_tile * kTileM + q * 32;
-      mbar_wait(&tmem_full[buf], (uint32_t)((it >> 1) & 1));
-      tc_fence_after();
-      const uint32_t taddr0 = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * kMaxN);
-#pragma unroll
-      for (int c = 0; c < 2; ++c) {
-        const int c0 = third * 32 + c * kResChunkStride;
-        uint32_t v[32];
-        tmem_ld32_async(taddr0 + (uint32_t)c0, v);
-        tmem_ld_wait(v);
-#pragma unroll
-        for (int jj = 0; jj < 4; ++jj) {
-          uint32_t packed[4];
-#pragma unroll
-          for (int h2 = 0; h2 < 2; ++h2) {
-            const int e = 8 * jj + 4 * h2;
-            float x0 = __uint_as_float(v[e]) + bias_r[c][e], x1 = __uint_as_float(v[e + 1]) + bias_r[c][e + 1];
-            float x2 = __uint_as_float(v[e + 2]) + bias_r[c][e + 2], x3 = __uint_as_float(v[e + 3]) + bias_r[c][e + 3];
-            if (t.act == 1) { x0 = gelu_erf(x0); x1 = gelu_erf(x1); x2 = gelu_erf(x2); x3 = gelu_erf(x3); }
-            packed[2 * h2] = pack_half2(x0, x1);
-            packed[2 * h2 + 1] = pack_half2(x2, x3);
-          }
-          *reinterpret_cast<uint4*>(stg + (uint32_t)lane * kEpiPitch + (uint32_t)jj * 16u) =
-              make_uint4(packed[0], packed[1], packed[2], packed[3]);
-        }
-        __syncwarp();
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const int rr = i * 8 + (lane >> 2), ch = lane & 3;
-          const uint4 w = *reinterpret_cast<const uint4*>(stg + (uint32_t)rr * kEpiPitch + (uint32_t)ch * 16u);
-          const int grow = row_base + rr;
-          if (grow < t.T) *reinterpret_cast<uint4*>(t.Y + (size_t)grow * t.N + n0 + c0 + ch * 8) = w;
-        }
-        __syncwarp();
-      }
-      tc_fence_before();
+      wgmma_wait<0>();
       __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[buf]);
+      if (lane == 0) mbar_arrive(&empty[prev]);
+      // epilogue: + bias -> activation -> fp16 -> shared staging (columns >= nb belong to no output: skipped)
+#pragma unroll
+      for (int c8 = 0; c8 < kPassN / 8; ++c8) {
+        if (8 * c8 >= nb) break;
+        const int c = 8 * c8 + c_lane;
+        const float2 bb = __ldg(reinterpret_cast<const float2*>(t.bias + n0 + c));
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float x0 = acc[4 * c8 + 2 * h] + bb.x, x1 = acc[4 * c8 + 2 * h + 1] + bb.y;
+          if (t.act == 1) { x0 = gelu_erf(x0); x1 = gelu_erf(x1); }
+          *reinterpret_cast<uint32_t*>(stg + (uint32_t)(r_lo + 8 * h) * kEpiPitch + (uint32_t)c * 2u) = pack_half2(x0, x1);
+        }
+      }
+      named_bar_sync(2 + wg, 128);
+      const int row_chunks = nb / 8;   // 16-byte chunks per row (nb is a multiple of 32)
+      const int row_base = m_tile * kTileM + wg * 64;
+      for (int idx = wt; idx < 64 * row_chunks; idx += 128) {
+        const int rr = idx / row_chunks, ch = idx - rr * row_chunks;
+        const int grow = row_base + rr;
+        if (grow < t.T)
+          *reinterpret_cast<uint4*>(t.Y + (size_t)grow * t.N + n0 + ch * 8) =
+              *reinterpret_cast<const uint4*>(stg + (uint32_t)rr * kEpiPitch + (uint32_t)ch * 16u);
+      }
+      named_bar_sync(2 + wg, 128);   // the staging buffer is free for the next item
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == kResMmaWarp) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
   }
 }
+// 16-byte asynchronous global -> shared copy (zero-fills when src_bytes == 0).
+__device__ __forceinline__ void cp_async_16(uint32_t dst_smem, const void* src, uint32_t src_bytes) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst_smem), "l"(src), "r"(src_bytes) : "memory");
+}
+
 
 // ---- embeddings + LayerNorm: one warp per token ----------------------------------------------------------
 __global__ void __launch_bounds__(256) embed_ln_kernel(const int32_t* __restrict__ ids, const int32_t* __restrict__ type_ids,
@@ -588,8 +260,8 @@ __global__ void __launch_bounds__(256) embed_ln_kernel(const int32_t* __restrict
 }
 
 // out = LayerNorm(x + res), one warp per token.  H % 128 == 0 (384 for MiniLM): a lane owns the columns
-// lane * 4 + 128 i, so every load / store instruction of the warp covers 256 contiguous bytes (8-byte pieces);
-// the first version moved 2 bytes per lane and instruction and ran at 3.5 TB/s.
+// lane * 4 + 128 i, so every load / store instruction of the warp covers 256 contiguous bytes (8-byte pieces)
+// rather than 2 bytes per lane and instruction.
 template <bool VEC>
 __global__ void __launch_bounds__(256) add_ln_kernel(const __half* __restrict__ xin, const __half* __restrict__ res,
                                                      const float* __restrict__ g, const float* __restrict__ bta, float eps,
@@ -886,9 +558,8 @@ __global__ void __launch_bounds__(1024) seq_order_kernel(const int32_t* __restri
 }
 
 // Two 16-query tiles per warp and key block: the K / V fragments are fetched from shared memory once and feed both
-// tiles' MMAs, and the two tiles' softmax chains (max -> ex2 -> sum -> pack) interleave.  ncu on the one-tile
-// kernel showed no saturated pipe (ex2 32 %, HMMA 30 %, issue 37 %) with three CTAs = 12 warps per SM: the
-// dependent chain of a single tile per warp, not a throughput limit, set the pace.
+// tiles' MMAs, and the two tiles' softmax chains (max -> ex2 -> sum -> pack) interleave: with one tile per warp and
+// three CTAs = 12 warps per SM, the dependent chain of that tile, not a pipe's throughput, sets the pace.
 //
 // Launch order: one CTA per (sequence, head), heads fastest, the sequences walked longest first (`order`, built once per call by
 // seq_order_kernel).  A CTA's work grows with L^2 and the lengths of a call spread over an order of magnitude; in
@@ -967,7 +638,7 @@ __global__ void __launch_bounds__(128, 3) attention2_kernel(const __half* __rest
     }
     // One block of NKK k-steps (16 keys each) starting at key kb: NKK = 4 for a full 64-key block, 1..3 for the tail of
     // the sequence.  NKK is a compile-time constant so that every loop unrolls without guards (run-time guards inside
-    // the unrolled body kept the compiler from interleaving the MMAs with the softmax: 134 -> 161 us per layer).
+    // the unrolled body keep the compiler from interleaving the MMAs with the softmax).
     auto block = [&](auto nkk_tag, int kb) {
       constexpr int NKK = decltype(nkk_tag)::value;
       constexpr int NJ = 2 * NKK;   // 8-key score tiles
@@ -1080,9 +751,8 @@ __global__ void __launch_bounds__(128, 3) attention2_kernel(const __half* __rest
 // (their [CLS] rows sit in shared memory as fp32) and its H/32 warps share the H pooler outputs; for one output
 // the lanes stride over the H inputs, so every Wp read is a coalesced 128-byte line shared by the CTA's
 // sequences, followed by one warp-shuffle reduction per sequence; the warps' partial logits meet in shared
-// memory and are summed in a fixed order.  (History: Wp row-per-lane, 32 lines per load instruction: 313 us per
-// launch; then one WARP per four sequences walking all H outputs one after the other: coalesced, but 16 CTAs of
-// serial work, 526 us per 256-sequence call = 9 % of the forward in the round-2 launch list.)
+// memory and are summed in a fixed order.  (Wp read row-per-lane touches 32 lines per load instruction; one warp per
+// four sequences walking all H outputs one after the other is coalesced but leaves a few CTAs with long serial work.)
 constexpr int kClsSeqs = 2;
 constexpr int kClsMaxWarps = 16;
 __global__ void __launch_bounds__(kClsMaxWarps * 32) cls_head_kernel(const __half* __restrict__ hidden, const int32_t* __restrict__ cu,
@@ -1142,15 +812,14 @@ using namespace rl;
 extern "C" size_t rl_xenc_linear_image_bytes(int N, int K) {
   const int n_ks = (K + kSliceK - 1) / kSliceK;
   const int n_pad = (N + 15) / 16 * 16;
-  const int pw = pass_width(N, K);
-  return (size_t)((n_pad + pw - 1) / pw) * pw * n_ks * kSliceK * sizeof(__half);
+  return (size_t)((n_pad + kPassN - 1) / kPassN) * kPassN * n_ks * kSliceK * sizeof(__half);
 }
 
 extern "C" int rl_xenc_pack_linear(const float* W, int N, int K, void* image, void* stream) {
   RL_REQUIRE(W && image && N > 0 && K > 0, RL_EINVAL, "rl_xenc_pack_linear: bad arguments");
   RL_REQUIRE(N % 16 == 0 && K % 8 == 0, RL_EUNSUPPORTED, "rl_xenc_pack_linear: N %% 16 and K %% 8 must be 0");
   RL_CUDA_CHECK(cudaMemsetAsync(image, 0, rl_xenc_linear_image_bytes(N, K), (cudaStream_t)stream));
-  pack_linear_kernel<<<1024, 256, 0, (cudaStream_t)stream>>>(W, N, K, pass_width(N, K), reinterpret_cast<__half*>(image));
+  pack_linear_kernel<<<1024, 256, 0, (cudaStream_t)stream>>>(W, N, K, reinterpret_cast<__half*>(image));
   RL_CUDA_CHECK(cudaGetLastError());
   return RL_OK;
 }
@@ -1170,11 +839,11 @@ static EncodeTiledFn encode_tiled_fn() {
   return fn;
 }
 
-static int launch_linear_resident(const __half* X, const void* img, const float* bias, __half* Y, int T, int N, int K, int act,
-                                  int sm_count, cudaStream_t stream) {
+static int launch_linear(const __half* X, const void* img, const float* bias, __half* Y, int T, int N, int K, int act,
+                         int sm_count, cudaStream_t stream) {
   EncodeTiledFn enc = encode_tiled_fn();
   RL_REQUIRE(enc != nullptr, RL_ECUDA, "cuTensorMapEncodeTiled is not available from this driver");
-  RL_REQUIRE((reinterpret_cast<uintptr_t>(X) & 15) == 0 && (K * 2) % 16 == 0, RL_EINVAL, "resident linear: X must be 16-byte aligned");
+  RL_REQUIRE((reinterpret_cast<uintptr_t>(X) & 15) == 0 && (K * 2) % 16 == 0, RL_EINVAL, "linear: X must be 16-byte aligned");
   CUtensorMap tm;
   const cuuint64_t gdim[2] = {(cuuint64_t)K, (cuuint64_t)T};          // innermost first
   const cuuint64_t gstr[1] = {(cuuint64_t)K * sizeof(__half)};        // bytes between token rows
@@ -1185,71 +854,18 @@ static int launch_linear_resident(const __half* X, const void* img, const float*
                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   RL_REQUIRE(r == CUDA_SUCCESS, RL_ECUDA, "cuTensorMapEncodeTiled failed (%d) for X[%d, %d]", (int)r, T, K);
   LinArgs t;
-  t.X = X; t.img = reinterpret_cast<const __half*>(img); t.bias = bias; t.Y = Y; t.T = T; t.N = N; t.K = K; t.act = act;
-  t.n_pass = N / kResN;
-  t.n_ks = K / kSliceK;
-  t.stages = kResStages;
-  t.cp_async = 0;
-  t.pw = kResN;
-  const size_t smem = (size_t)t.n_ks * kResWSliceBytes + (size_t)kResStages * kABytes + kBarBytes + kResEpiBytes + 1024;
-  RL_REQUIRE(smem <= 227 * 1024, RL_EUNSUPPORTED, "resident linear: %zu bytes of shared memory", smem);
-  RL_CUDA_CHECK(cudaFuncSetAttribute(linear_wres_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  const int m_tiles = (T + kTileM - 1) / kTileM;
-  int per_pass = sm_count / t.n_pass;
-  if (per_pass < 1) per_pass = 1;
-  if (per_pass > m_tiles) per_pass = m_tiles;
-  linear_wres_kernel<<<t.n_pass * per_pass, kResThreads, smem, stream>>>(tm, t);
-  RL_CUDA_CHECK(cudaGetLastError());
-  return RL_OK;
-}
-
-static int launch_linear(const __half* X, const void* img, const float* bias, __half* Y, int T, int N, int K, int act,
-                         int sm_count, cudaStream_t stream) {
-  // RL_XENC_RESIDENT=0 forces the streaming kernel (A/B switch; the image layout follows pass_width()).
-  const char* res_env = getenv("RL_XENC_RESIDENT");   // read per launch: tools/time_linear.py A/Bs it in one process
-  const bool resident_ok = res_env == nullptr || atoi(res_env) != 0;
-  if (use_resident(N, K)) {
-    if (resident_ok) return launch_linear_resident(X, img, bias, Y, T, N, K, act, sm_count, stream);
-  }
-  LinArgs t;
-  t.X = X; t.img = reinterpret_cast<const __half*>(img); t.bias = bias; t.Y = Y; t.T = T; t.N = N; t.K = K; t.act = act;
-  t.pw = pass_width(N, K);
-  t.n_pass = (N + t.pw - 1) / t.pw;
+  t.img = reinterpret_cast<const __half*>(img); t.bias = bias; t.Y = Y; t.T = T; t.N = N; t.K = K; t.act = act;
+  t.n_pass = (N + kPassN - 1) / kPassN;
   t.n_ks = (K + kSliceK - 1) / kSliceK;
-  // cp.async activation loader (every free smem stage in flight, no registers held) is the default: bit-identical
-  // outputs, 352 -> 309 us for the four GEMMs of a layer (profiles/r01_linear_loader_ab.json); RL_XENC_CPASYNC=0
-  // selects the register-ring loader.  Read per launch: tools/time_linear.py A/Bs it in one process.
-  const char* cpa = getenv("RL_XENC_CPASYNC");
-  t.cp_async = (cpa != nullptr && atoi(cpa) == 0) ? 0 : 1;
-  static_assert((2 * kMaxStages + 4) * 8 + 8 <= kBarBytes, "barrier block overflows its slot");
-  const uint32_t tail = kBarBytes + kEpiBytes;
-  int stages = (int)((kSmemBudget - 1024 - tail) / lin_stage_bytes());
+  const uint32_t tail = 2 * kMaxStages * 8 + kEpiBytes;   // barriers + epilogue staging
+  int stages = (int)((kSmemBudget - 1024 - tail) / kLinStageBytes);
   if (stages > kMaxStages) stages = kMaxStages;
   t.stages = stages;
-  const size_t smem = (size_t)stages * lin_stage_bytes() + tail + 1024;
-  // Cluster multicast of the weight slices (two token tiles per cluster).  Validated bit-identical, measured no
-  // gain on B200 (FFN-down 89.9 us vs 88.6 us without, tools/time_linear.py): at cluster size 2 L2 already merges
-  // the two CTAs' unicast requests for the same lines, so the multicast removes no traffic.  Opt-in: RL_XENC_MC=1.
-  const char* mc_env = getenv("RL_XENC_MC");
-  const bool mc = (mc_env != nullptr && atoi(mc_env) != 0) && t.cp_async && T > kTileM && sm_count >= 2 &&
-                  (((N + t.pw - 1) / t.pw == N / t.pw) && (t.pw * 128) % 32 == 0);
-  if (mc) {
-    RL_CUDA_CHECK(cudaFuncSetAttribute(linear_tcgen05_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    const int64_t units = (int64_t)(((T + kTileM - 1) / kTileM + 1) / 2) * t.n_pass;
-    const int clusters = (int)(units < sm_count / 2 ? units : sm_count / 2);
-    cudaLaunchConfig_t cfg{};
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    cfg.gridDim = dim3((unsigned)(2 * clusters)); cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = smem; cfg.stream = stream;
-    cfg.attrs = attr; cfg.numAttrs = 1;
-    RL_CUDA_CHECK(cudaLaunchKernelEx(&cfg, linear_tcgen05_kernel<true>, t));
-    return RL_OK;
-  }
-  RL_CUDA_CHECK(cudaFuncSetAttribute(linear_tcgen05_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  const size_t smem = (size_t)stages * kLinStageBytes + tail + 1024;
+  RL_CUDA_CHECK(cudaFuncSetAttribute(linear_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const int64_t items = (int64_t)((T + kTileM - 1) / kTileM) * t.n_pass;
   const int grid = (int)(items < sm_count ? items : sm_count);
-  linear_tcgen05_kernel<false><<<grid, kThreads, smem, stream>>>(t);
+  linear_wgmma_kernel<<<grid, kLinThreads, smem, stream>>>(tm, t);
   RL_CUDA_CHECK(cudaGetLastError());
   return RL_OK;
 }
@@ -1260,7 +876,7 @@ extern "C" int rl_xenc_linear(const void* X, const void* image, const float* bia
   RL_REQUIRE(N % 32 == 0 && K % 8 == 0, RL_EUNSUPPORTED, "rl_xenc_linear: N %% 32 and K %% 8 must be 0");
   RL_REQUIRE((reinterpret_cast<uintptr_t>(bias) & 15) == 0, RL_EINVAL, "rl_xenc_linear: bias must be 16-byte aligned");
   if (T == 0) return RL_OK;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   RL_CUDA_CHECK(cudaGetDevice(&dev));
   RL_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   return launch_linear(reinterpret_cast<const __half*>(X), image, bias, reinterpret_cast<__half*>(Y), T, N, K, act, sms,
@@ -1287,7 +903,7 @@ extern "C" int rl_xenc_score(const rl_xenc_weights* w, const int32_t* input_ids,
              "rl_xenc_score: hidden=%d heads=%d unsupported (head_dim must be 32, hidden <= 512)", H, nh);
   RL_REQUIRE(F % 32 == 0 && max_len > 0 && max_len <= w->max_pos, RL_EUNSUPPORTED, "rl_xenc_score: bad ffn / max_len");
   RL_REQUIRE(workspace && workspace_bytes >= rl_xenc_workspace_bytes(w, T), RL_ENOSPACE, "rl_xenc_score: workspace too small");
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   RL_CUDA_CHECK(cudaGetDevice(&dev));
   RL_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   __half* hidden = reinterpret_cast<__half*>(workspace);
@@ -1317,12 +933,11 @@ extern "C" int rl_xenc_score(const rl_xenc_weights* w, const int32_t* input_ids,
   const size_t att_smem = (size_t)((max_len + 63) / 64 * 64) * kAttPitch * 2 * sizeof(__half);
   RL_REQUIRE(att_smem <= 200 * 1024, RL_EUNSUPPORTED, "rl_xenc_score: max_len=%d too long for the attention kernel", max_len);
   // Two launches when the batch holds long sequences: keys <= kAttShort with a small allocation (occupancy), the rest
-  // with the full one.  (ncu, round 2: a single launch sized by the longest sequence ran 3 CTAs = 12 warps per SM.)
+  // with the full one (a single launch sized by the longest sequence holds every CTA to the largest allocation).
   constexpr int kAttShort = 256;
   const size_t att_smem_short = (size_t)kAttShort * kAttPitch * 2 * sizeof(__half);
-  // A/B switch for the Q loads / context stores.  Measured back to back on one B200 (262 k tokens per
-  // layer): 4-byte fragment pieces 0.744 ms, 16-byte rows + quad transpose 1.100 ms -- so pieces are
-  // the default and RL_XENC_ATT_QUAD=1 selects the transpose variant.
+  // Q loads / context stores of the one-tile attention kernel: 4-byte fragment pieces by default,
+  // RL_XENC_ATT_QUAD=1 selects 16-byte rows + a quad transpose.
   static const bool att_quad = []() { const char* e = getenv("RL_XENC_ATT_QUAD"); return e ? atoi(e) != 0 : false; }();
   RL_CUDA_CHECK(cudaFuncSetAttribute(attention_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)att_smem));
   RL_CUDA_CHECK(cudaFuncSetAttribute(attention_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)att_smem));
@@ -1340,9 +955,8 @@ extern "C" int rl_xenc_score(const rl_xenc_weights* w, const int32_t* input_ids,
       else if (att_quad) attention_kernel<true><<<dim3(P, nh), 128, smem, stream>>>(qkv, cu_seqlens, H, nh, scale, ctx, lo, hi);
       else attention_kernel<false><<<dim3(P, nh), 128, smem, stream>>>(qkv, cu_seqlens, H, nh, scale, ctx, lo, hi);
     };
-    // Measured (ncu launch list, 51 k tokens per call, mean 200): two bucketed launches 86 + 64 us vs 141 us for one
-    // launch -- the long sequences carry 40 % of the L^2 work and gain nothing, the split adds a tail.  Off
-    // unless RL_XENC_ATT_BUCKETS=1.
+    // Two launches bucketed by length (RL_XENC_ATT_BUCKETS=1) or one launch (the default): the long sequences carry
+    // most of the L^2 work either way, and the split adds a tail.
     static const bool buckets = []() { const char* e = getenv("RL_XENC_ATT_BUCKETS"); return e != nullptr && atoi(e) != 0; }();
     if (buckets && max_len > kAttShort) {
       attention(att_smem_short, 0, kAttShort);

@@ -42,6 +42,14 @@ def test_reference_arm_other_workloads(workload):
     assert d["impl"] == "reference" and d["value"] > 0 and workload in ("c2", "c3")
 
 
+@pytest.mark.parametrize("extra", [["--steps", "0"], ["--workload", "c5", "--gpus", "2", "--dump-outputs", "unused"]])
+def test_bad_argument_combinations_are_rejected(extra):
+    """Zero timed steps, and a c5 dump on several GPUs (each rank only holds its own pairs), stop at argument parsing."""
+    out = subprocess.run([sys.executable, str(ROOT / "bench.py"), "--impl", "reference", *extra], capture_output=True, text=True,
+                         timeout=120, check=False)
+    assert out.returncode == 2 and "error:" in out.stderr and not out.stdout.strip()
+
+
 def test_reference_arm_under_torchrun_only_rank0_prints():
     """N > 1: the driver launches the arm with torchrun; rank 0 alone runs and prints, the others exit 0 without work."""
     base = {"WORLD_SIZE": "2", "MASTER_ADDR": "127.0.0.1", "MASTER_PORT": "29655"}
@@ -68,3 +76,24 @@ def test_gpu_arm_line_carries_the_contract_keys():
     assert e["value"] > 0 and e["h2d_bytes_per_step"] > 0 and e["d2h_bytes_per_step"] > 0
     assert d["check"]["checked_queries"] >= 16 and d["check"]["identical_topk_sets"] == d["check"]["checked_queries"]
     assert {"sm_mhz", "sm_max_mhz", "reasons"} <= set(d["clocks"])
+
+
+@pytest.mark.gpu
+def test_gpu_arm_dump_outputs_are_reproducible(tmp_path):
+    """``--dump-outputs``: the last timed step's results as float32 / float64 .npy files, at most 64 MB in all, and the
+    same numbers from a second run with the same arguments (seeded inputs)."""
+    import numpy as np
+
+    dumps = []
+    for run in ("a", "b"):
+        out = tmp_path / run
+        subprocess.run([sys.executable, str(ROOT / "bench.py"), "--workload", "c2", "--steps", "2", "--warmup", "1",
+                        "--no-cpu-baseline", "--dump-outputs", str(out)], capture_output=True, text=True, timeout=600, check=True)
+        files = sorted(out.glob("*.npy"))
+        assert {f.stem for f in files} == {"hit_sim", "hit_chunk", "hit_count", "status"}
+        assert sum(f.stat().st_size for f in files) <= 64 << 20
+        arrays = {f.stem: np.load(f) for f in files}
+        assert all(a.dtype in (np.float32, np.float64) for a in arrays.values())
+        dumps.append(arrays)
+    for name, a in dumps[0].items():
+        assert np.array_equal(a, dumps[1][name]), name

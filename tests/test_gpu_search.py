@@ -395,7 +395,7 @@ def test_selection_larger_than_finalize_window_is_rejected(rl):
     Q = make_queries(E, 1, seed=94)
     with pytest.raises((RagliteB200Error, ValueError)):   # (k - 1) * 40 + 1 = 4361 rows would have to be ranked exactly
         rl.vector_search_batch(Q, num_results=110, config=rl.RAGLiteConfig(reranker=None), index=idx, exact_maxsim=True)
-    # ... 3961 fit the 4096-entry window (round 1 stopped at 3276)
+    # ... 3961 fit the 4096-entry window
     ids, sims, counts = rl.vector_search_batch(Q, num_results=100, config=rl.RAGLiteConfig(reranker=None), index=idx, exact_maxsim=True)
     check_exact_maxsim(E, off, Q[0], ids[0, :counts[0]], sims[0, :counts[0]], k=100)
 

@@ -1,4 +1,4 @@
-"""Compare the tcgen05 scan's approximate keys with the fp32 scan's, element by element."""
+"""Compare the tensor-core (wgmma) scan's approximate keys with the fp32 scan's, element by element."""
 import sys
 from pathlib import Path
 sys.path.insert(0, str(Path(__file__).resolve().parents[1])); sys.path.insert(0, str(Path(__file__).resolve().parents[1] / "tests"))

@@ -13,10 +13,13 @@ __global__ void __launch_bounds__(512) rd(const float4* __restrict__ p, size_t n
 }
 int main() {
   float* out; cudaMalloc(&out, 4);
-  for (size_t mb : {16, 32, 64, 96, 4096}) {
+  int sms = 0;
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
+  // 8 .. 32 MiB stay resident in an H100's 50 MB L2; 4 GiB streams from HBM
+  for (size_t mb : {8, 16, 32, 4096}) {
     size_t bytes = mb << 20; float4* p; cudaMalloc(&p, bytes); cudaMemset(p, 0, bytes);
-    int reps = mb <= 96 ? 200 : 4;
-    for (int grid : {148, 296, 592}) {
+    int reps = mb <= 32 ? 200 : 4;
+    for (int grid : {sms, 2 * sms, 4 * sms}) {
       cudaEvent_t a, b; cudaEventCreate(&a); cudaEventCreate(&b);
       rd<<<grid, 512>>>(p, bytes / 16, 2, out);
       cudaEventRecord(a); rd<<<grid, 512>>>(p, bytes / 16, reps, out); cudaEventRecord(b); cudaEventSynchronize(b);
