@@ -193,6 +193,10 @@ int rl_maxsim_release(const void* workspace);
 int rl_maxsim_copy_dump(const rl_scan_params* p, const void* workspace, float* dst, int64_t* n_sample_rows,
                         void* stream);
 
+/* Debug/test hook: copy the per-query error bound of the approximate key that the last call used
+ * (float32 [B], key units: |approximate key - exact key| <= eps[b] for every row) into dst (device memory). */
+int rl_maxsim_copy_eps(const rl_scan_params* p, const void* workspace, float* dst, void* stream);
+
 /* ---- Shard merge + GROUP BY chunk + top-k: _search.py:143-150 --------------------------------
  * hit_*[R,B,H] are the per-shard outputs of rl_maxsim_topk (all-gathered).  num_hits > 0: keep
  * the num_hits best vectors overall, group by chunk (max sim), order desc, limit k.  num_hits == 0:

@@ -27,14 +27,25 @@ def minilm_config(**over):  # noqa: ANN003, ANN201
     return BertConfig(**cfg)
 
 
-def seeded_model(seed: int = 0, **over):  # noqa: ANN003, ANN201
-    """Deterministic random weights (real ones cannot be downloaded here); scaled so that logits spread."""
+def seeded_model(seed: int = 0, *, perturb: bool = False, **over):  # noqa: ANN003, ANN201
+    """Deterministic random weights (real ones cannot be downloaded here); scaled so that logits spread.
+
+    The transformers init leaves every Linear bias at 0 and every LayerNorm at gamma = 1, beta = 0, so a forward
+    that dropped them would still match.  ``perturb`` draws them instead: biases (pooler and classifier included)
+    and LayerNorm betas from N(0, 0.1), LayerNorm gammas from 1 + N(0, 0.1)."""
     from transformers import BertForSequenceClassification
 
     torch.manual_seed(seed)
     model = BertForSequenceClassification(minilm_config(**over)).eval()
     with torch.no_grad():
         model.classifier.weight.mul_(8.0)
+        if perturb:
+            for m in model.modules():
+                if isinstance(m, torch.nn.Linear) and m.bias is not None:
+                    m.bias.normal_(0.0, 0.1)
+                elif isinstance(m, torch.nn.LayerNorm):
+                    m.weight.normal_(1.0, 0.1)
+                    m.bias.normal_(0.0, 0.1)
     return model
 
 

@@ -730,6 +730,14 @@ class CorpusIndex:
                   "rl_maxsim_copy_dump")
         return out
 
+    def debug_eps(self) -> torch.Tensor:
+        """Per-query error bound ``eps [B]`` of the approximate keys of the last scan, as the kernels computed it (test hook)."""
+        p = self.last_params
+        out = torch.empty(int(p.B), dtype=torch.float32, device=self.device)
+        with torch.cuda.device(self.device):
+            check(self.lib.rl_maxsim_copy_eps(C.byref(p), _ptr(self.last_ws), _ptr(out), _stream()), "rl_maxsim_copy_eps")
+        return out
+
     def kernel_times_ms(self) -> dict[str, float]:
         """Stage times of the last scan made with ``flags=RL_FLAG_TIME_KERNELS`` (synchronises)."""
         ms = (C.c_float * 5)()

@@ -427,6 +427,17 @@ extern "C" int rl_maxsim_copy_dump(const rl_scan_params* p, const void* workspac
   return RL_OK;
 }
 
+extern "C" int rl_maxsim_copy_eps(const rl_scan_params* p, const void* workspace, float* dst, void* stream) {
+  RL_REQUIRE(p && workspace && dst, RL_EINVAL, "rl_maxsim_copy_eps: null pointer");
+  Layout L;
+  int rc = make_layout(p, 132, &L);
+  if (rc != RL_OK) return rc;
+  if (p->B > 0)
+    RL_CUDA_CHECK(cudaMemcpyAsync(dst, static_cast<const unsigned char*>(workspace) + L.off_eps, (size_t)p->B * 4,
+                                  cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+  return RL_OK;
+}
+
 extern "C" int rl_topk_merge(const float* hit_sim, const int64_t* hit_chunk, const int32_t* hit_count, int R, int B,
                              int H, int num_hits, int k, float* out_sim, int64_t* out_chunk, int32_t* out_count,
                              void* stream) {

@@ -173,8 +173,8 @@ def test_large_clustered(rl):
 
 @pytest.mark.parametrize("metric", ["cosine", "dot", "l2"])
 def test_several_query_groups_per_tile(rl, metric):
-    """B > 256 (BASELINE configs[2] runs B = 1024): the scan walks every corpus tile once per group of 256
-    queries inside ONE launch; 600 queries = two full groups and a ragged third."""
+    """B > 128 (BASELINE configs[2] runs B = 1024): the scan walks every corpus tile once per group of 128
+    queries inside ONE launch; 600 queries = four full groups and a ragged fifth."""
     from synth_torch import gaussian_corpus_torch, host_blocks, queries_near_rows
 
     vecs, d, B, k = 4, 256, 600, 20

@@ -362,12 +362,13 @@ def test_fp16_storage_rejects_lossy_input(rl):
 
 @pytest.mark.parametrize("algo", ALGOS)
 def test_block_boundaries_and_batch_groups(rl, algo):
-    """Rows exactly on / one past a 128-row block edge; batches of 1, 256 and 257 (two query groups)."""
+    """Rows exactly on / one past a 128-row block edge; batches of 1, 257 (three query groups of 128) and 1025 (the
+    tensor-core scan's second launch: more than 8 groups)."""
     _algo_ok(rl, algo, 64)
     for n_rows in (128, 129, 256 * 3):
         E, off = make_corpus(n_rows, 1, 64, seed=n_rows)
         idx = rl.CorpusIndex(E, off)
-        for B in (1, 257):
+        for B in (1, 257, 1025):
             Q = make_queries(E, B, seed=B)
             ids, sims, counts = rl.vector_search_batch(Q, num_results=3, config=rl.RAGLiteConfig(reranker=None), index=idx, algo=algo)
             for b in (0, B - 1):
