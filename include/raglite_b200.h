@@ -242,10 +242,12 @@ int rl_rrf_fuse(const int64_t* ids, const double* weights, int B, int R, int L, 
 /* rl_span_collate: the ranking half of retrieve_chunk_spans (_search.py:323-360) for B lists of M retrieved chunk
  * indices (ranked[B, M], -1 padded).  Index tables (device): chunk_doc[c] = ordinal of the chunk's document in
  * ascending document_id order, chunk_pos[c] = Chunk.index, chunk_alive[c] (or NULL), and the lookup
- * (doc << 32 | pos) -> chunk as two arrays sorted by key.  Every retrieved chunk is joined by its neighbours at
- * the given position offsets inside its document (neighbors[n_neighbors], e.g. {-1, +1}), duplicates are dropped,
+ * (doc << 32 | pos) -> chunk as two arrays of n_chunks entries sorted by key (ranked indices outside [0, n_chunks) are
+ * skipped, so the lookup covers every chunk; deleted ones are turned away through chunk_alive).  Every retrieved
+ * chunk is joined by its neighbours at the given position offsets inside its document (neighbors[n_neighbors], e.g. {-1, +1}), duplicates are dropped,
  * members are ordered by (document, position) and cut into runs of consecutive positions; a run's score is the
- * sum of 1 / (rank + 1) over its retrieved members (float64), runs are ordered by descending score (stable).
+ * sum of 1 / (rank + 1) over its retrieved members (float64, compensated as Python's sum() is since 3.12), runs
+ * are ordered by descending score (stable).
  * Outputs, cap = M * (1 + n_neighbors) per query: out_member[B, cap] chunk indices in document order (-1 padded),
  * out_span_start / out_span_len[B, cap] (offsets into the member row, in final span order), out_span_score[B, cap],
  * out_n_span[B], out_n_member[B].  cap <= 4096. */
@@ -312,6 +314,11 @@ size_t rl_xenc_workspace_bytes(const rl_xenc_weights* w, int T);
 int rl_xenc_score(const rl_xenc_weights* w, const int32_t* input_ids, const int32_t* type_ids, const int32_t* pos_ids,
                   const int32_t* cu_seqlens, int P, int T, int max_len, float* out_logit, float* out_score,
                   void* workspace, size_t workspace_bytes, void* stream);
+/* Debug/test hook: the attention step of rl_xenc_score on its own.  qkv [T, 3*hidden] fp16 (Q | K | V), ctx [T, hidden]
+ * fp16, cu_seqlens [P+1] (device), max_len = longest sequence; head_dim 32.  Uses the RL_XENC_ATT* selection of
+ * rl_xenc_score.  workspace: >= 4*P bytes (the length-sorted order), 16-byte aligned. */
+int rl_xenc_attention(const void* qkv, const int32_t* cu_seqlens, int P, int T, int max_len, int hidden, int n_heads,
+                      void* ctx, void* workspace, size_t workspace_bytes, void* stream);
 
 #ifdef __cplusplus
 }

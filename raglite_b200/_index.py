@@ -564,7 +564,9 @@ class CorpusIndex:
         """Device tables ``rl_span_collate`` needs (built once per index change from the ``Chunk`` records):
         ``chunk_doc`` = ordinal of each chunk's document in ascending ``document_id`` order (the order
         ``retrieve_chunk_spans`` sorts by, ``_search.py:343``), ``chunk_pos`` = ``Chunk.index``, ``chunk_alive``, and the
-        lookup ``(doc << 32 | pos) -> chunk`` sorted by key."""
+        lookup ``(doc << 32 | pos) -> chunk`` sorted by key.  The lookup holds every chunk, deleted ones included: its
+        length is also the range the kernel accepts retrieved chunk indices from, and a deleted chunk is turned away
+        there through ``chunk_alive``.  Among equal keys the live chunk comes first, which is the one found."""
         if self.chunks is None:
             raise ValueError("The registered index holds no Chunk records (document ids / positions unknown)")
         with self._lock:
@@ -574,8 +576,7 @@ class CorpusIndex:
                 doc = np.fromiter((ordinal[c.document_id] for c in self.chunks), dtype=np.int32, count=len(self.chunks))
                 pos = np.fromiter((c.index for c in self.chunks), dtype=np.int32, count=len(self.chunks))
                 key = (doc.astype(np.uint64) << np.uint64(32)) | pos.astype(np.uint32).astype(np.uint64)
-                live = np.nonzero(self._chunk_alive)[0]
-                order = live[np.argsort(key[live], kind="stable")]
+                order = np.lexsort((~self._chunk_alive.astype(bool), key))   # by key, then live first
                 dev = self.device
                 self._span_tables = {
                     "chunk_doc": torch.from_numpy(doc).to(dev), "chunk_pos": torch.from_numpy(pos).to(dev),

@@ -10,7 +10,8 @@
 //                    order the runs by descending score (stable).
 //
 // One CTA per query; everything lives in shared memory (a few thousand entries).  Scores are float64, summed in
-// the reference's order, so they are the reference's Python floats bit for bit.
+// the reference's order and the way its Python code sums them (`+=` for RRF, compensated `sum()` for spans), so
+// they are the reference's Python floats bit for bit.
 #include "common.cuh"
 
 namespace rl {
@@ -151,10 +152,14 @@ __global__ void __launch_bounds__(kFuseThreads) span_collate_kernel(
   const int cap = M * (1 + n_nb);
   int npow2 = 1;
   while (npow2 < cap) npow2 <<= 1;
+  // Shared memory, npow2 entries per array: key | score | chunk_of | rel | tmpk (8 bytes each) | pay (4 bytes).  The
+  // 4-byte array comes last so that every 8-byte array starts on an 8-byte boundary for any npow2, 1 included.
   uint64_t* key = reinterpret_cast<uint64_t*>(fuse_smem);         // (doc << 32 | pos), later span sort keys
   double* score = reinterpret_cast<double*>(key + npow2);          // 1 / (rank + 1) of retrieved members, 0 for neighbours
-  uint32_t* pay = reinterpret_cast<uint32_t*>(score + npow2);      // slot in `ranked x (1 + n_nb)` -> chunk, later span index
-  int64_t* chunk_of = reinterpret_cast<int64_t*>(pay + npow2);     // [npow2] chunk per entry (by original slot)
+  int64_t* chunk_of = reinterpret_cast<int64_t*>(score + npow2);   // [npow2] chunk per entry (by original slot)
+  double* rel = reinterpret_cast<double*>(chunk_of + npow2);       // [npow2] relevance by unique index
+  uint64_t* tmpk = reinterpret_cast<uint64_t*>(rel + npow2);       // [npow2] scratch
+  uint32_t* pay = reinterpret_cast<uint32_t*>(tmpk + npow2);       // slot in `ranked x (1 + n_nb)` -> chunk, later span index
   __shared__ int n_span;
   const int b = blockIdx.x;
   // 1) entries: slot = i * (1 + n_nb) + o (o = 0: the retrieved chunk, o >= 1: its o-th neighbour offset)
@@ -199,7 +204,6 @@ __global__ void __launch_bounds__(kFuseThreads) span_collate_kernel(
   __syncthreads();
   const int nu = total_unique;
   // member list (unique chunks in document order) + per-member relevance, written to global / kept in registers via smem
-  double* rel = reinterpret_cast<double*>(chunk_of + npow2);       // [npow2] relevance by unique index
   int64_t* member = out_member + (size_t)b * cap;
   for (int e = threadIdx.x; e < npow2; e += blockDim.x) {
     const int u = head[e];
@@ -217,8 +221,7 @@ __global__ void __launch_bounds__(kFuseThreads) span_collate_kernel(
   uint64_t* ukey = key;   // reuse: first compact the unique keys
   __shared__ int dummy;
   (void)dummy;
-  // (unique keys, in order) -- gather through a second pass to avoid aliasing while reading `key`
-  uint64_t* tmpk = reinterpret_cast<uint64_t*>(rel + npow2);       // [npow2]
+  // (unique keys, in order) -- gather through a second pass (tmpk) to avoid aliasing while reading `key`
   for (int e = threadIdx.x; e < npow2; e += blockDim.x)
     if (head[e] >= 0) tmpk[head[e]] = key[e];
   __syncthreads();
@@ -228,17 +231,22 @@ __global__ void __launch_bounds__(kFuseThreads) span_collate_kernel(
   int32_t* s_len = out_span_len + (size_t)b * cap;
   double* s_score = out_span_score + (size_t)b * cap;
   if (threadIdx.x == 0) {   // sequential: the reference's groupby loop (a few thousand members at most)
+    // A run's score is the reference's sum() over its members, which Python (3.12 on) computes with Neumaier's
+    // compensated summation: a running sum plus a compensation term that is added once at the end.
+    auto py_sum = [](double acc, double comp) { return comp != 0.0 && isfinite(comp) ? acc + comp : acc; };
     int ns = 0, start = 0;
-    double acc = 0.0;
+    double acc = 0.0, comp = 0.0;
     for (int u = 0; u < nu; ++u) {
       const bool cont = u > 0 && (ukey[u] >> 32) == (ukey[u - 1] >> 32) && (uint32_t)ukey[u] == (uint32_t)ukey[u - 1] + 1u;
       if (u > 0 && !cont) {
-        s_start[ns] = start; s_len[ns] = u - start; s_score[ns] = acc; ++ns;
-        start = u; acc = 0.0;
+        s_start[ns] = start; s_len[ns] = u - start; s_score[ns] = py_sum(acc, comp); ++ns;
+        start = u; acc = 0.0; comp = 0.0;
       }
-      acc += rel[u];
+      const double x = rel[u], t = acc + x;
+      comp += fabs(acc) >= fabs(x) ? (acc - t) + x : (x - t) + acc;
+      acc = t;
     }
-    if (nu > 0) { s_start[ns] = start; s_len[ns] = nu - start; s_score[ns] = acc; ++ns; }
+    if (nu > 0) { s_start[ns] = start; s_len[ns] = nu - start; s_score[ns] = py_sum(acc, comp); ++ns; }
     n_span = ns;
   }
   __syncthreads();
@@ -299,7 +307,7 @@ extern "C" int rl_span_collate(const int64_t* ranked, int B, int M, const int32_
   RL_REQUIRE(cap <= kFuseMax, RL_EUNSUPPORTED, "rl_span_collate: M*(1+neighbors)=%lld exceeds %d", (long long)cap, kFuseMax);
   int npow2 = 1;
   while (npow2 < cap) npow2 <<= 1;
-  const size_t smem = (size_t)npow2 * (8 + 8 + 4 + 8 + 8 + 8);
+  const size_t smem = (size_t)npow2 * (8 + 8 + 8 + 8 + 8 + 4);   // key | score | chunk_of | rel | tmpk | pay
   RL_REQUIRE(smem <= 220 * 1024, RL_EUNSUPPORTED, "rl_span_collate: %zu bytes of shared memory", smem);
   RL_CUDA_CHECK(cudaFuncSetAttribute(span_collate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   span_collate_kernel<<<B, kFuseThreads, smem, (cudaStream_t)stream>>>(ranked, M, chunk_doc, chunk_pos, chunk_alive, sorted_key,

@@ -883,6 +883,97 @@ extern "C" int rl_xenc_linear(const void* X, const void* image, const float* bia
                        (cudaStream_t)stream);
 }
 
+// ---- attention step: variant selection and launches, shared by rl_xenc_score and the rl_xenc_attention test hook ----
+// Each variant switch is an A/B alternative read once per process from its environment variable.
+struct AttVariant {
+  bool lpt;           // RL_XENC_ATT_LPT (default on): walk the sequences longest first (0: arrival order, the A/B baseline)
+  bool stage_async;   // RL_XENC_ATT_CPASYNC (default on): K / V staging through cp.async with the first Q loads
+                      // overlapped (0: plain loads, the A/B baseline)
+  bool seq_fastest;   // RL_XENC_ATT_ORDER=1: sequences fastest in the CTA order of attention2_kernel (default: heads)
+  bool att2;          // RL_XENC_ATT2 (default on): attention2_kernel, two tiles per warp (0: attention_kernel)
+  bool quad;          // RL_XENC_ATT_QUAD=1: Q loads / context stores of attention_kernel as 16-byte rows + a quad
+                      // transpose (default: 4-byte fragment pieces)
+  bool buckets;       // RL_XENC_ATT_BUCKETS=1: two launches bucketed by length (default: one launch)
+};
+static const AttVariant& att_variant() {
+  static const AttVariant v = []() {
+    auto on = [](const char* name, bool dflt) { const char* e = getenv(name); return e == nullptr ? dflt : atoi(e) != 0; };
+    const char* order = getenv("RL_XENC_ATT_ORDER");
+    AttVariant r;
+    r.lpt = on("RL_XENC_ATT_LPT", true);
+    r.stage_async = on("RL_XENC_ATT_CPASYNC", true);
+    r.seq_fastest = order != nullptr && atoi(order) == 1;
+    r.att2 = on("RL_XENC_ATT2", true);
+    r.quad = on("RL_XENC_ATT_QUAD", false);
+    r.buckets = on("RL_XENC_ATT_BUCKETS", false);
+    return r;
+  }();
+  return v;
+}
+
+// Two launches when the batch holds long sequences (RL_XENC_ATT_BUCKETS=1): keys <= kAttShort with a small allocation
+// (occupancy), the rest with the full one (a single launch sized by the longest sequence holds every CTA to the largest
+// allocation).
+constexpr int kAttShort = 256;
+static size_t att_smem_bytes(int max_len) { return (size_t)((max_len + 63) / 64 * 64) * kAttPitch * 2 * sizeof(__half); }
+
+// Once per forward: the length-sorted sequence order (seq_order [P], when LPT is on) and the kernels' shared-memory limit.
+static int attention_setup(const int32_t* cu_seqlens, int P, int max_len, int32_t* seq_order, cudaStream_t stream) {
+  const AttVariant& v = att_variant();
+  const size_t att_smem = att_smem_bytes(max_len);
+  RL_REQUIRE(att_smem <= 200 * 1024, RL_EUNSUPPORTED, "max_len=%d too long for the attention kernel", max_len);
+  if (v.lpt) {
+    seq_order_kernel<<<1, 1024, 0, stream>>>(cu_seqlens, P, seq_order);
+    RL_CUDA_CHECK(cudaGetLastError());
+  }
+  RL_CUDA_CHECK(cudaFuncSetAttribute(attention_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)att_smem));
+  RL_CUDA_CHECK(cudaFuncSetAttribute(attention_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)att_smem));
+  RL_CUDA_CHECK(cudaFuncSetAttribute(attention2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)att_smem));
+  return RL_OK;
+}
+
+// Once per layer: ctx = softmax(Q K^T / sqrt(32)) V per sequence and head, from qkv [T, 3H] (Q | K | V).
+static int attention_launch(const __half* qkv, const int32_t* cu_seqlens, const int32_t* seq_order, int P, int max_len,
+                            int H, int nh, __half* ctx, cudaStream_t stream) {
+  const AttVariant& v = att_variant();
+  const size_t att_smem = att_smem_bytes(max_len), att_smem_short = att_smem_bytes(kAttShort);
+  const float scale = 1.4426950408889634f / sqrtf(32.f);  // softmax in the exp2 domain
+  auto attention = [&](size_t smem, int lo, int hi) {
+    if (v.att2 && lo == 0 && hi == max_len)
+      attention2_kernel<<<dim3((unsigned)P * (unsigned)nh), 128, smem, stream>>>(qkv, cu_seqlens, v.lpt ? seq_order : nullptr, H, nh, scale, ctx,
+                                                                                     P, v.seq_fastest ? 1 : 0, v.stage_async ? 1 : 0);
+    else if (v.quad) attention_kernel<true><<<dim3(P, nh), 128, smem, stream>>>(qkv, cu_seqlens, H, nh, scale, ctx, lo, hi);
+    else attention_kernel<false><<<dim3(P, nh), 128, smem, stream>>>(qkv, cu_seqlens, H, nh, scale, ctx, lo, hi);
+  };
+  // Two launches bucketed by length or one launch (the default): the long sequences carry most of the L^2 work either
+  // way, and the split adds a tail.
+  if (v.buckets && max_len > kAttShort) {
+    attention(att_smem_short, 0, kAttShort);
+    attention(att_smem, kAttShort, max_len);
+  } else {
+    attention(att_smem, 0, max_len);
+  }
+  RL_CUDA_CHECK(cudaGetLastError());
+  return RL_OK;
+}
+
+extern "C" int rl_xenc_attention(const void* qkv, const int32_t* cu_seqlens, int P, int T, int max_len, int hidden, int n_heads,
+                                 void* ctx, void* workspace, size_t workspace_bytes, void* stream_) {
+  RL_REQUIRE(qkv && cu_seqlens && ctx, RL_EINVAL, "rl_xenc_attention: null pointer");
+  if (P == 0 || T == 0) return RL_OK;
+  RL_REQUIRE(hidden % 32 == 0 && hidden <= 512 && n_heads > 0 && hidden / n_heads == 32, RL_EUNSUPPORTED,
+             "rl_xenc_attention: hidden=%d heads=%d unsupported (head_dim must be 32, hidden <= 512)", hidden, n_heads);
+  RL_REQUIRE(P > 0 && P <= T && max_len > 0, RL_EINVAL, "rl_xenc_attention: bad P=%d / T=%d / max_len=%d", P, T, max_len);
+  RL_REQUIRE(workspace && (reinterpret_cast<uintptr_t>(workspace) & 15) == 0 && workspace_bytes >= (size_t)P * sizeof(int32_t),
+             RL_ENOSPACE, "rl_xenc_attention: workspace must be 16-byte aligned and hold %d int32", P);
+  cudaStream_t stream = (cudaStream_t)stream_;
+  int32_t* seq_order = reinterpret_cast<int32_t*>(workspace);
+  const int rc = attention_setup(cu_seqlens, P, max_len, seq_order, stream);
+  if (rc != RL_OK) return rc;
+  return attention_launch(reinterpret_cast<const __half*>(qkv), cu_seqlens, seq_order, P, max_len, hidden, n_heads,
+                          reinterpret_cast<__half*>(ctx), stream);
+}
+
 extern "C" size_t rl_xenc_workspace_bytes(const rl_xenc_weights* w, int T) {
   if (w == nullptr || T < 0) return 0;
   const size_t H = (size_t)w->hidden, F = (size_t)w->ffn;
@@ -914,15 +1005,8 @@ extern "C" int rl_xenc_score(const rl_xenc_weights* w, const int32_t* input_ids,
   int32_t* seq_order = reinterpret_cast<int32_t*>(
       (reinterpret_cast<uintptr_t>(ffn + (size_t)T * F) + 15) & ~uintptr_t(15));   // [P] (P <= T)
   RL_REQUIRE(P <= T, RL_EINVAL, "rl_xenc_score: more sequences than tokens");
-  // Attention walks the sequences longest first (RL_XENC_ATT_LPT=0: in arrival order, the A/B baseline).
-  static const bool att_lpt = []() { const char* e = getenv("RL_XENC_ATT_LPT"); return e == nullptr || atoi(e) != 0; }();
-  // K / V staging through cp.async with the first Q loads overlapped (RL_XENC_ATT_CPASYNC=0: plain loads, the A/B baseline)
-  static const bool att_stage_async = []() { const char* e = getenv("RL_XENC_ATT_CPASYNC"); return e == nullptr || atoi(e) != 0; }();
-  static const bool att_seq_fastest = []() { const char* e = getenv("RL_XENC_ATT_ORDER"); return e != nullptr && atoi(e) == 1; }();
-  if (att_lpt) {
-    seq_order_kernel<<<1, 1024, 0, stream>>>(cu_seqlens, P, seq_order);
-    RL_CUDA_CHECK(cudaGetLastError());
-  }
+  int rc = attention_setup(cu_seqlens, P, max_len, seq_order, stream);
+  if (rc != RL_OK) return rc;
   const int tok_blocks = (T + 7) / 8;
   const bool ln_vec = H % 128 == 0;   // (LayerNorm gamma / beta come from torch allocations: 16-byte aligned)
   embed_ln_kernel<<<tok_blocks, 256, 0, stream>>>(input_ids, type_ids, pos_ids, reinterpret_cast<const __half*>(w->word_emb),
@@ -930,41 +1014,12 @@ extern "C" int rl_xenc_score(const rl_xenc_weights* w, const int32_t* input_ids,
                                                   reinterpret_cast<const __half*>(w->type_emb), w->emb_ln_g, w->emb_ln_b,
                                                   w->ln_eps, T, H, w->vocab, w->max_pos, w->type_vocab, hidden);
   RL_CUDA_CHECK(cudaGetLastError());
-  const size_t att_smem = (size_t)((max_len + 63) / 64 * 64) * kAttPitch * 2 * sizeof(__half);
-  RL_REQUIRE(att_smem <= 200 * 1024, RL_EUNSUPPORTED, "rl_xenc_score: max_len=%d too long for the attention kernel", max_len);
-  // Two launches when the batch holds long sequences: keys <= kAttShort with a small allocation (occupancy), the rest
-  // with the full one (a single launch sized by the longest sequence holds every CTA to the largest allocation).
-  constexpr int kAttShort = 256;
-  const size_t att_smem_short = (size_t)kAttShort * kAttPitch * 2 * sizeof(__half);
-  // Q loads / context stores of the one-tile attention kernel: 4-byte fragment pieces by default,
-  // RL_XENC_ATT_QUAD=1 selects 16-byte rows + a quad transpose.
-  static const bool att_quad = []() { const char* e = getenv("RL_XENC_ATT_QUAD"); return e ? atoi(e) != 0 : false; }();
-  RL_CUDA_CHECK(cudaFuncSetAttribute(attention_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)att_smem));
-  RL_CUDA_CHECK(cudaFuncSetAttribute(attention_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)att_smem));
-  RL_CUDA_CHECK(cudaFuncSetAttribute(attention2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)att_smem));
-  const float scale = 1.4426950408889634f / sqrtf(32.f);  // softmax in the exp2 domain
   for (int l = 0; l < w->n_layers; ++l) {
     const rl_xenc_layer& L = w->layers[l];
-    int rc = launch_linear(hidden, L.qkv_img, L.qkv_bias, qkv, T, 3 * H, H, 0, sms, stream);
+    rc = launch_linear(hidden, L.qkv_img, L.qkv_bias, qkv, T, 3 * H, H, 0, sms, stream);
     if (rc != RL_OK) return rc;
-    static const bool att2 = []() { const char* e = getenv("RL_XENC_ATT2"); return e == nullptr || atoi(e) != 0; }();
-    auto attention = [&](size_t smem, int lo, int hi) {
-      if (att2 && lo == 0 && hi == max_len)
-        attention2_kernel<<<dim3((unsigned)P * (unsigned)nh), 128, smem, stream>>>(qkv, cu_seqlens, att_lpt ? seq_order : nullptr, H, nh, scale, ctx,
-                                                                                       P, att_seq_fastest ? 1 : 0, att_stage_async ? 1 : 0);
-      else if (att_quad) attention_kernel<true><<<dim3(P, nh), 128, smem, stream>>>(qkv, cu_seqlens, H, nh, scale, ctx, lo, hi);
-      else attention_kernel<false><<<dim3(P, nh), 128, smem, stream>>>(qkv, cu_seqlens, H, nh, scale, ctx, lo, hi);
-    };
-    // Two launches bucketed by length (RL_XENC_ATT_BUCKETS=1) or one launch (the default): the long sequences carry
-    // most of the L^2 work either way, and the split adds a tail.
-    static const bool buckets = []() { const char* e = getenv("RL_XENC_ATT_BUCKETS"); return e != nullptr && atoi(e) != 0; }();
-    if (buckets && max_len > kAttShort) {
-      attention(att_smem_short, 0, kAttShort);
-      attention(att_smem, kAttShort, max_len);
-    } else {
-      attention(att_smem, 0, max_len);
-    }
-    RL_CUDA_CHECK(cudaGetLastError());
+    rc = attention_launch(qkv, cu_seqlens, seq_order, P, max_len, H, nh, ctx, stream);
+    if (rc != RL_OK) return rc;
     rc = launch_linear(ctx, L.o_img, L.o_bias, tmp, T, H, H, 0, sms, stream);
     if (rc != RL_OK) return rc;
     if (ln_vec) add_ln_kernel<true><<<tok_blocks, 256, 0, stream>>>(tmp, hidden, L.ln1_g, L.ln1_b, w->ln_eps, T, H, hidden);

@@ -59,6 +59,29 @@ def test_workspace_query_and_argument_validation_run_without_a_gpu():
     assert b"metric" in lib.rl_last_error()
 
 
+def test_attention_hook_refuses_what_rl_xenc_score_refuses():
+    """``rl_xenc_attention`` checks its arguments before any CUDA call (the pointers here are never dereferenced)."""
+    from raglite_b200 import _lib
+
+    lib = _lib.load()
+    ptr, ws = 4096, 8192                                        # placeholders: every call below is refused first
+
+    def call(*, qkv=ptr, P=4, T=100, max_len=64, hidden=384, heads=12, workspace=ws, ws_bytes=16):
+        return lib.rl_xenc_attention(qkv, ptr, P, T, max_len, hidden, heads, ptr, workspace, ws_bytes, None)
+
+    assert call(qkv=None) == -1
+    assert call(hidden=48, heads=1) == -4                       # hidden % 32
+    assert call(hidden=544, heads=17) == -4                     # hidden > 512
+    assert call(hidden=384, heads=6) == -4                      # head_dim 64
+    assert call(P=101) == -1                                    # more sequences than tokens
+    assert call(max_len=0) == -1
+    assert call(ws_bytes=15) == -3                              # 4 * P bytes
+    assert call(workspace=ws + 4) == -3                         # 16-byte alignment
+    assert call(workspace=None) == -3
+    assert call(max_len=1281, T=2000) == -4                     # K / V of 1344 keys exceed the shared memory
+    assert b"max_len=1281" in lib.rl_last_error()
+
+
 def test_config_mirrors_reference_fields():
     from raglite_b200 import RAGLiteConfig
 
