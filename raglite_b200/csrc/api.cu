@@ -134,7 +134,7 @@ int make_layout(const rl_scan_params* p, int sm_count, Layout* L) {
   L->off_hist = take(B * kHistBins * 4);
   L->off_histw = take(B * 4);
   L->off_cntall = take(B * 4);
-  L->off_qimg = take(algo == RL_ALGO_TCGEN05 ? wgmma_qimg_bytes(p->B, p->d) : 0);
+  L->off_qimg = take(algo == RL_ALGO_TCGEN05 ? wgmma_qimg_bytes(p) : 0);
   L->off_dump = take(B * (size_t)L->n_sample_rows * 4);
   L->off_cand = take(B * (size_t)L->cap * sizeof(Cand));
   L->total = off;

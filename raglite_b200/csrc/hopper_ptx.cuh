@@ -120,11 +120,34 @@ __device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t a_desc
       : "memory");
 }
 // One 64-wide K slice (four k16 steps) into the accumulator; `accumulate` = 0 starts a new sum.
-__device__ __forceinline__ void wgmma_slice(float (&d)[64], uint64_t a_desc, uint64_t b_desc, bool accumulate) {
+//   NACC = 64:  N = 128 queries, one m64n128k16 per k step.
+//   NACC = 128: N = 256 queries as two m64n128k16 per k step, on B rows 0..127 and 128..255 (16 KB further on:
+//   the 128B swizzle repeats every 8 rows, so the same descriptor form addresses the second half) into d[0..63] and
+//   d[64..127].  That is the m64n256k16 fragment layout (d[i] holds column 8 (i / 4) + 2 (t % 4) + i % 2).  A single
+//   m64n256k16 would need 154 registers at the instruction, over the 128 a 512-thread CTA starts with, and the
+//   compiler checks each instruction against that launch limit whatever setmaxnreg raises the budget to.
+template <int NACC>
+__device__ __forceinline__ void wgmma_slice(float (&d)[NACC], uint64_t a_desc, uint64_t b_desc, bool accumulate) {
+  static_assert(NACC == 64 || NACC == 128, "wgmma_slice: N is 128 or 256");
 #pragma unroll
-  for (int k = 0; k < 4; ++k)
-    wgmma_m64n128k16(d, a_desc + (uint64_t)(2 * k), b_desc + (uint64_t)(2 * k), (accumulate || k > 0) ? 1u : 0u);
+  for (int k = 0; k < 4; ++k) {
+    const uint32_t acc = (accumulate || k > 0) ? 1u : 0u;
+    float(&lo)[64] = *reinterpret_cast<float(*)[64]>(&d[0]);
+    wgmma_m64n128k16(lo, a_desc + (uint64_t)(2 * k), b_desc + (uint64_t)(2 * k), acc);
+    if constexpr (NACC == 128) {
+      float(&hi)[64] = *reinterpret_cast<float(*)[64]>(&d[64]);
+      wgmma_m64n128k16(hi, a_desc + (uint64_t)(2 * k), b_desc + (uint64_t)(2 * k + (128 * 128 >> 4)), acc);
+    }
+  }
 }
+
+// ---- per-warpgroup register budget ----------------------------------------------------------------
+// The whole warpgroup executes these.  dec hands registers back to the CTA's pool; inc blocks until the pool
+// holds enough.  Counts are multiples of 8 in [24, 256].
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 
 }  // namespace tc
 }  // namespace rl

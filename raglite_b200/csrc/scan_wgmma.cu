@@ -4,15 +4,16 @@
 // _search.py:69-79, _typing.py:123-134) with a coarse tensor-core pass whose survivors are
 // re-scored exactly in float64 by the finalize kernel (select_finalize.cu).
 //
-// One persistent CTA per SM (per SM and query group when B > 128) walks its tiles of 128 corpus rows:
+// One persistent CTA per SM (per SM and query group when B > N) walks its tiles of 128 corpus rows:
 //   * 8 loader warps stream the fp32 rows from HBM with coalesced 128-bit loads, scale them (cosine:
 //     1/|e|, dot/l2: a global power of two), round to fp16 and store them into a 128B-swizzled
 //     K-major shared-memory tile (the wgmma A operand); an fp16-stored corpus comes in through a
 //     TMA tensor map instead, with the swizzle applied by the copy engine,
 //   * lane 0 of the first loader warp bulk-copies (cp.async.bulk) the matching 64-wide K slice of the
-//     pre-swizzled fp16 query image (the wgmma B operand, N = 128 queries) into the same stage,
+//     pre-swizzled fp16 query image (the wgmma B operand, N = 256 queries for an fp32 corpus with B > 128 and
+//     d > 960, else 128) into the same stage,
 //   * two consumer warpgroups, 64 corpus rows each, issue wgmma.m64n128k16 (fp32 accumulate in
-//     registers) slice by slice, then turn their accumulators into keys and either dump them (sample
+//     registers; N = 256: two per k step) slice by slice, then turn their accumulators into keys and either dump them (sample
 //     tiles) or compare them with the per-query threshold; the few survivors are staged in shared
 //     memory together with a histogram of their keys, flushed in bulk (one global atomic per touched
 //     query / bin), and the global histogram is read back to tighten the thresholds while the scan is
@@ -37,7 +38,7 @@ using namespace tc;
 
 constexpr int kTileM = 128;           // corpus rows per tile (two warpgroups of M = 64)
 constexpr int kSliceK = 64;           // fp16 elements per K slice = one 128-byte swizzle row
-constexpr int kMaxQ = 128;            // queries per group (wgmma N)
+// Queries per group = wgmma N, the template parameter NQ: 256 or 128 (query_group_width()).
 constexpr int kNumConsumerWarps = 8;  // warps 0..7: warpgroup 0 takes rows 0..63 of a tile, warpgroup 1 rows 64..127
 constexpr int kNumConsumers = kNumConsumerWarps * 32;
 constexpr int kFirstLoaderWarp = 8;  // its lane 0 also brings the query slices (and, fp16 storage, the corpus tiles)
@@ -45,22 +46,41 @@ constexpr int kNumLoaderWarps = 8;
 // 512 threads: registers are allocated per four warps, so a 17th warp would cost a whole warpgroup's worth
 // and hold every thread to 96 registers.
 constexpr int kThreads = (kFirstLoaderWarp + kNumLoaderWarps) * 32;
+// NQ = 256: the 128 accumulators of a consumer thread do not fit the 128 registers every thread starts with, so the
+// loader warpgroups give registers back (setmaxnreg) and the consumer warpgroups take them: 2 x 72 + 2 x 184 = 4 x 128.
+constexpr int kLoaderRegs = 72;
+constexpr int kConsumerRegs = 184;
+static_assert(kLoaderRegs + kConsumerRegs == 2 * 65536 / kThreads, "the register split must use exactly the CTA's registers");
 constexpr int kMaxStages = 8;
 constexpr int kABytes = kTileM * 128;  // 16 KB per stage
 constexpr uint32_t kSmemBudget = 227 * 1024;
-constexpr int kPrefetchItems = 6;      // L2 prefetch distance in K-slice items (6 x 32 KB per SM)
+// L2 prefetch distance of the fp32 loaders in K-slice items (32 KB per SM each).  NQ = 256 prefetches nothing: measured
+// on an H100 80GB HBM3 at 400 W (c4shard, B = 256), distances of 2, 4, 6, 8 and 12 items made the scan 5, 10, 33, 52
+// and 79 % slower than none.
+template <int NQ>
+__host__ __device__ constexpr int prefetch_items() { return NQ == 128 ? 6 : 0; }
 constexpr int kListCap = 1024;         // staged hit records (12 KB)
 constexpr int kFlushFirst = 192;       // first flush early: it feeds the histogram that tightens the thresholds
 constexpr int kFlushAt = 512;          // later flushes: once this many hits are waiting (or at the end)
 constexpr int kRefreshEvery = 16;      // tiles between threshold refreshes from the global histogram
-constexpr int kMaxGroups = 8;          // query groups sharing one launch (B <= 1024 per launch)
+constexpr int kMaxBatchPerLaunch = 1024;   // query groups sharing one launch: 8 of 128 or 4 of 256
+
+// Query-group width (the qimg layout and the launch both follow it).  256 removes the duplicated fp32 -> fp16
+// conversion of B > 128: one CTA per lane converts each tile once for 256 queries.  It needs an fp32 corpus (fp16 rows
+// come in through TMA, unconverted) and long tiles: with 4 stages instead of 6, a tile of fewer than 16 K slices
+// cannot hide the 256-column epilogue.  Measured on an H100 80GB HBM3 at 400 W: 1.26x / 1.35x faster at d = 1024 (c4shard,
+// c3), 1.3x slower at d = 384 (c2), 1.5x slower with fp16 storage at d = 1024.
+inline int query_group_width(const rl_scan_params* p) {
+  const int n_ks = (p->d + kSliceK - 1) / kSliceK;
+  return (p->B > 128 && p->e_dtype != 1 && n_ks >= 16) ? 256 : 128;
+}
 
 struct TcArgs {
   ScanArgs a;
-  const __half* qimg;     // [groups][n_ks][kMaxQ][64] fp16, rows pre-swizzled
+  const __half* qimg;     // [groups][n_ks][NQ][64] fp16, rows pre-swizzled
   const float* q_scale;   // [B] key = acc * q_scale[b] (+ bias)
   const float* row_stats; // [4] max norm, max |element|, min norm, flags
-  int nq;                 // padded #queries of a full group (multiple of 16; kMaxQ when par_groups > 1)
+  int nq;                 // padded #queries of a full group (multiple of 16; NQ when par_groups > 1)
   int nq_last;            // padded #queries of the last group
   int par_groups;         // CTA c serves query group c % par_groups of the tiles of lane c / par_groups
   int n_ks;               // K slices
@@ -74,37 +94,39 @@ __device__ __forceinline__ float pow2_scale(float max_abs) {
 }
 
 struct SmemLayout {
-  unsigned char* stage_base;  // stages * kStageBytes
   uint64_t* full;             // [kMaxStages]
   uint64_t* empty;            // [kMaxStages]
-  float* thr;                 // [kMaxQ]
-  float* cs;                  // [kMaxQ]
-  float* thr0;                // [kMaxQ] threshold from the sample (histogram origin)
-  float* inv_w;               // [kMaxQ] 1 / bin width (bin width = 4 eps)
-  uint32_t* hist;             // [kMaxQ * kHistBins / 2] staged histogram, two 16-bit counters per word
-  int* cnt;                   // [kMaxQ] hits per query staged since the last flush
-  int* basev;                 // [kMaxQ] global slot base per query for the current flush
+  float* thr;                 // [NQ]
+  float* cs;                  // [NQ]
+  float* thr0;                // [NQ] threshold from the sample (histogram origin)
+  float* inv_w;               // [NQ] 1 / bin width (bin width = 4 eps)
+  uint32_t* hist;             // [NQ * kHistBins / 2] staged histogram, two 16-bit counters per word
+  int* cnt;                   // [NQ] hits per query staged since the last flush
+  int* basev;                 // [NQ] global slot base per query for the current flush
   int* list_n;                // [4] number of staged records
   uint32_t* list;             // [kListCap][3] {col | rank << 16, key bits, row}
+  unsigned char* stage_base;  // stages * stage_bytes<NQ>(), after the above (tail_bytes<NQ>())
 };
 
-// A stage: the corpus slice of a tile (A) and room for the query slice of a FULL group (B, kMaxQ rows of 128 bytes).
-// The wgmma always reads all kMaxQ rows of B; a group of nq < kMaxQ queries only copies nq rows, so rows nq..kMaxQ-1
+// A stage: the corpus slice of a tile (A) and room for the query slice of a FULL group (B, NQ rows of 128 bytes).
+// The wgmma always reads all NQ rows of B; a group of nq < NQ queries only copies nq rows, so rows nq..NQ-1
 // hold whatever an earlier slice left there.  They only feed accumulator columns >= nq, which the epilogue never reads,
 // and they lie inside the stage, so the MMA never reads another stage or the barriers.
-constexpr uint32_t kStageBytes = kABytes + kMaxQ * 128u;
-__host__ __device__ inline uint32_t tail_bytes() {
-  return 2 * kMaxStages * 8 + kMaxQ * (6u * 4u + (uint32_t)kHistBins * 2u) + 16 + kListCap * 12;
+template <int NQ>
+__host__ __device__ constexpr uint32_t stage_bytes() { return kABytes + NQ * 128u; }
+template <int NQ>
+__host__ __device__ constexpr uint32_t tail_bytes() {
+  return 2 * kMaxStages * 8 + NQ * (6u * 4u + (uint32_t)kHistBins * 2u) + 16 + kListCap * 12;
 }
 
 // EF16: the corpus is stored as fp16 (lossless for RAGLite data, whose embeddings are fp16-rounded,
 // reference _embed.py:140): the tensor map brings the rows into the swizzled tile without conversion, half the HBM bytes.
-template <int METRIC, bool EF16>
+template <int METRIC, bool EF16, int NQ>
 __global__ void __launch_bounds__(kThreads, 1) scan_wgmma_kernel(const __grid_constant__ CUtensorMap tmE, const TcArgs t) {
   extern __shared__ unsigned char smem_dyn[];
-  // Group-parallel mode (B > 128): the CTAs of a "lane" -- par_groups consecutive CTAs -- walk the SAME corpus
-  // tiles at the same time, one 128-query group each.  The first of them pulls a tile in from HBM, the others
-  // find it in L2 microseconds later, so HBM sees the corpus once.
+  // Group-parallel mode (B > NQ): the CTAs of a "lane" -- par_groups consecutive CTAs -- walk the SAME corpus tiles
+  // at the same time, one NQ-query group each.  The first of them pulls a tile in from HBM (and, NQ = 128, prefetches
+  // it into L2), the others find it in L2 microseconds later, so HBM sees the corpus once.
   const int P = t.par_groups > 1 ? t.par_groups : 1;
   const int pg = P > 1 ? (int)(blockIdx.x % (unsigned)P) : 0;
   ScanArgs a = t.a;
@@ -112,39 +134,46 @@ __global__ void __launch_bounds__(kThreads, 1) scan_wgmma_kernel(const __grid_co
   const __half* qimg_g = t.qimg;
   const int nq = (pg == P - 1) ? t.nq_last : t.nq;   // padded width of the group this CTA serves
   if (P > 1) {
-    const int q0p = pg * kMaxQ;
-    a.B = min(kMaxQ, t.a.B - q0p);
+    const int q0p = pg * NQ;
+    a.B = min(NQ, t.a.B - q0p);
     a.thr += q0p; a.cand_cnt += q0p; a.eps += q0p; a.hist_inv_w += q0p; a.q_inv_norm += q0p;
     if (a.cnt_all != nullptr) a.cnt_all += q0p;
     a.dump += (size_t)q0p * a.n_sample_rows;
     a.cand += (size_t)q0p * a.cap;
     a.ghist += (size_t)q0p * kHistBins;
     q_scale_g += q0p;
-    qimg_g += (size_t)pg * t.n_ks * kMaxQ * kSliceK;
+    qimg_g += (size_t)pg * t.n_ks * NQ * kSliceK;
   }
-  // 1024-byte alignment for the 128B-swizzled tiles.
-  unsigned char* base = smem_dyn + ((1024u - (smem_u32(smem_dyn) & 1023u)) & 1023u);
-  constexpr uint32_t sbytes = kStageBytes;
+  // The tail (barriers, per-query arrays, staged list) comes first, at fixed offsets: its addresses are constants,
+  // not registers the roles have to carry.  The stages follow, 1024-byte aligned for the 128B-swizzled tiles.
+  constexpr uint32_t sbytes = stage_bytes<NQ>();
   SmemLayout s;
-  s.stage_base = base;
-  s.full = reinterpret_cast<uint64_t*>(base + (size_t)t.stages * sbytes);
+  s.full = reinterpret_cast<uint64_t*>(smem_dyn);
   s.empty = s.full + kMaxStages;
   s.thr = reinterpret_cast<float*>(s.empty + kMaxStages);
-  s.cs = s.thr + kMaxQ;
-  s.thr0 = s.cs + kMaxQ;
-  s.inv_w = s.thr0 + kMaxQ;
-  s.hist = reinterpret_cast<uint32_t*>(s.inv_w + kMaxQ);
-  s.cnt = reinterpret_cast<int*>(s.hist + kMaxQ * kHistBins / 2);
-  s.basev = s.cnt + kMaxQ;
-  s.list_n = s.basev + kMaxQ;
+  s.cs = s.thr + NQ;
+  s.thr0 = s.cs + NQ;
+  s.inv_w = s.thr0 + NQ;
+  s.hist = reinterpret_cast<uint32_t*>(s.inv_w + NQ);
+  s.cnt = reinterpret_cast<int*>(s.hist + NQ * kHistBins / 2);
+  s.basev = s.cnt + NQ;
+  s.list_n = s.basev + NQ;
   s.list = reinterpret_cast<uint32_t*>(s.list_n + 4);
+  unsigned char* tail_end = smem_dyn + tail_bytes<NQ>();
+  s.stage_base = tail_end + ((1024u - (smem_u32(tail_end) & 1023u)) & 1023u);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int64_t n_tiles = a.n_mode_blocks;
-  const int64_t first = (int64_t)blockIdx.x / P;
-  const int64_t stride = (int64_t)gridDim.x / P;
+  // Tile counts and block indices stay below 2^24 (n_rows < 2^31), so they are computed in 32 bits: a 64-bit
+  // division is a subroutine call whose registers the loaders cannot spare at NQ = 256.
+  const uint32_t n_tiles = (uint32_t)a.n_mode_blocks;
+  const uint32_t first = blockIdx.x / (uint32_t)P;
+  const uint32_t stride = gridDim.x / (uint32_t)P;
   const int64_t my_tiles = first < n_tiles ? (n_tiles - first + stride - 1) / stride : 0;
-  auto ord_of = [&](int64_t tile) -> int64_t { return first + tile * stride; };
+  auto ord_of = [&](int64_t tile) -> uint32_t { return first + (uint32_t)tile * stride; };
+  auto block_of = [&](uint32_t ord) -> int64_t {   // mode_block_index() in 32 bits
+    const uint32_t S = (uint32_t)a.S;
+    return a.dump_mode ? ord * S : (S <= 1u ? ord : ord + ord / (S - 1u) + 1u);
+  };
   const uint32_t qbytes = (uint32_t)nq * 128u;   // one K slice of the group's queries
   const unsigned char* qsrc = reinterpret_cast<const unsigned char*>(qimg_g);
   const bool q_thread = threadIdx.x == kFirstLoaderWarp * 32;
@@ -162,26 +191,33 @@ __global__ void __launch_bounds__(kThreads, 1) scan_wgmma_kernel(const __grid_co
     }
     fence_barrier_init();
   }
-  for (int i = threadIdx.x; i < kMaxQ; i += blockDim.x) {
+  for (int i = threadIdx.x; i < NQ; i += blockDim.x) {
     s.thr[i] = (i < a.B && !a.dump_mode) ? a.thr[i] : __int_as_float(0x7f800000);  // +inf: never emit
     s.cs[i] = (i < a.B) ? q_scale_g[i] : 0.f;
     s.cnt[i] = 0;
     s.thr0[i] = s.thr[i];
     s.inv_w[i] = (i < a.B && !a.dump_mode) ? a.hist_inv_w[i] : 0.f;
   }
-  for (int i = threadIdx.x; i < kMaxQ * kHistBins / 2; i += blockDim.x) s.hist[i] = 0u;
+  for (int i = threadIdx.x; i < NQ * kHistBins / 2; i += blockDim.x) s.hist[i] = 0u;
   if (threadIdx.x == 0) { s.list_n[0] = 0; s.list_n[1] = 0; }
   __syncthreads();
   // Cosine on a corpus whose rows all have norm >= 0.5 and moderate magnitudes (the normal case:
   // embeddings are stored normalised): rows go to fp16 unscaled and the epilogue applies 1/|e|.
-  const bool cos_noscale = METRIC == RL_METRIC_COSINE &&
-                           (EF16 || (t.row_stats[2] > 0.f && t.row_stats[2] <= 2.f && t.row_stats[1] <= 1024.f &&
-                                     t.row_stats[3] == 0.f));   // (the host only allows fp16 storage when this holds)
+  // (a function of the row statistics that each role evaluates for itself: a value computed here and kept live
+  // into the roles would cost registers the NQ = 256 loaders do not have)
+  auto cos_noscale_of = [&]() -> bool {
+    return METRIC == RL_METRIC_COSINE &&
+           (EF16 || (t.row_stats[2] > 0.f && t.row_stats[2] <= 2.f && t.row_stats[1] <= 1024.f &&
+                     t.row_stats[3] == 0.f));   // (the host only allows fp16 storage when this holds)
+  };
 
   // fp32 loader fast path (uniform): whole K slices in pairs, no per-row scale in the loader
   const bool fast_f32 = !EF16 && a.d % kSliceK == 0 && (t.n_ks & 1) == 0 && a.ld * 64 < (int64_t(1) << 32) &&
-                        (METRIC != RL_METRIC_COSINE || cos_noscale);
+                        (METRIC != RL_METRIC_COSINE || cos_noscale_of());
+  // NQ = 256: each role sets its register budget first thing in its own branch (whole warpgroups: warps 0..7
+  // consume, warps 8..15 load), so that the compiler allocates the branch's code within that budget.
   if (EF16 && warp >= kFirstLoaderWarp) {
+    if constexpr (NQ == 256) setmaxnreg_dec<kLoaderRegs>();
     // ===== fp16 storage through the tensor map: one thread issues, per K slice, the TMA copy of the corpus tile (the
     // engine writes the 128B-swizzled layout itself) and the bulk copy of the query slice; the other loader warps idle.
     if (q_thread) {
@@ -191,7 +227,7 @@ __global__ void __launch_bounds__(kThreads, 1) scan_wgmma_kernel(const __grid_co
       // row0 of the current tile and of the next one, whose slices are prefetched into L2 one tile (n_ks slices =
       // 128 KB per SM at d = 1024) ahead
       int64_t tile = 0;
-      auto tile_row0 = [&](int64_t v) -> int { return v < my_tiles ? (int)(mode_block_index(a, ord_of(v)) * kTileM) : -1; };
+      auto tile_row0 = [&](int64_t v) -> int { return v < my_tiles ? (int)(block_of(ord_of(v)) * kTileM) : -1; };
       int row0 = tile_row0(0), row0_next = tile_row0(1);
       for (int64_t item = 0; item < total_items; ++item) {
         mbar_wait(&s.empty[stage], phase ^ 1u);
@@ -204,10 +240,11 @@ __global__ void __launch_bounds__(kThreads, 1) scan_wgmma_kernel(const __grid_co
       }
     }
   } else if (warp >= kFirstLoaderWarp && fast_f32) {
+    if constexpr (NQ == 256) setmaxnreg_dec<kLoaderRegs>();
     // ===== corpus loaders, fp32 storage, fast path (d % 128 == 0, no per-row scale) =====
-    // Same data movement as the generic loader below -- HBM fp32 -> registers (two K-slice items = 64 KB per SM in
-    // flight) -> cvt.rn.f16x2 -> 128B-swizzled smem tile, L2 prefetch ahead -- with the bookkeeping cut down: an
-    // iteration handles the PAIR of items (ks, ks + 1): one cursor step, row pointers with a 32-bit pitch shared by
+    // Same data movement as the generic loader below -- HBM fp32 -> registers -> cvt.rn.f16x2 -> 128B-swizzled smem
+    // tile; NQ = 128: two K-slice items (64 KB per SM) in flight and an L2 prefetch ahead, NQ = 256: one item and no
+    // prefetch -- with the bookkeeping cut down: an iteration handles the PAIR of items (ks, ks + 1): one cursor step, row pointers with a 32-bit pitch shared by
     // both items through a +256 B immediate, smem / barrier addresses kept incrementally.
     const int lt = threadIdx.x - kFirstLoaderWarp * 32;  // 0..255
     const int c4 = lt & 15;                              // float4 column within the 64-wide K slice
@@ -219,7 +256,8 @@ __global__ void __launch_bounds__(kThreads, 1) scan_wgmma_kernel(const __grid_co
     uint32_t sw_off = (uint32_t)r0 * 128u + ((((uint32_t)c4 >> 1) ^ ((uint32_t)r0 & 7u)) << 4) + (((uint32_t)c4 & 1u) << 3);
     // opaque moves: keep these in registers instead of re-deriving them from %tid / the parameter bank per item
     asm volatile("" : "+r"(n_ks), "+r"(n_stages), "+r"(pitch16), "+r"(sw_off));
-    const int64_t total_items = my_tiles * (int64_t)n_ks;
+    // (32 bits: an item is 32 KB of a corpus that fits in device memory)
+    const uint32_t total_items = (uint32_t)my_tiles * n_ks;
 
     struct Cursor { int64_t tile; uint32_t ks; int rows; const unsigned char* ptr; };
     // Load cursor: this thread's row r0 / column c4 of the NEXT pair of items to load.
@@ -227,7 +265,7 @@ __global__ void __launch_bounds__(kThreads, 1) scan_wgmma_kernel(const __grid_co
     auto ld_set_tile = [&]() {
       ld.rows = 0;
       if (ld.tile < my_tiles) {
-        const int64_t blk = mode_block_index(a, ord_of(ld.tile));
+        const int64_t blk = block_of(ord_of(ld.tile));
         const int64_t rem = a.n_rows - blk * kTileM;
         ld.rows = rem < kTileM ? (int)rem : kTileM;
         ld.ptr = reinterpret_cast<const unsigned char*>(a.E + (size_t)(blk * kTileM + r0) * a.ld + c4 * 4);
@@ -238,7 +276,7 @@ __global__ void __launch_bounds__(kThreads, 1) scan_wgmma_kernel(const __grid_co
     auto pf_set_tile = [&]() {
       pf.rows = 0;
       if (pg == 0 && t.pf_pairs > 0 && pf.tile < my_tiles) {
-        const int64_t blk = mode_block_index(a, ord_of(pf.tile));
+        const int64_t blk = block_of(ord_of(pf.tile));
         const int64_t rem = a.n_rows - blk * kTileM;
         pf.rows = rem < kTileM ? (int)rem : kTileM;
         pf.ptr = reinterpret_cast<const unsigned char*>(a.E + (size_t)(blk * kTileM + (lt >> 1)) * a.ld + (lt & 1) * 32);
@@ -291,22 +329,40 @@ __global__ void __launch_bounds__(kThreads, 1) scan_wgmma_kernel(const __grid_co
     ld_set_tile();
     pf_set_tile();
     for (int i = 0; i < t.pf_pairs + 1; ++i) pf_pair();   // the load cursor starts one pair ahead of the stores
-    issue(ringA, ld.rows, ld.ptr);
-    issue(ringB, ld.rows, ld.ptr + 256);
-    for (int64_t item = 0; item < total_items; item += 2) {
-      // advance the load cursor to the next pair (possibly the first pair of the next tile)
-      ld.ptr += 512;
-      ld.ks += 2;
-      if (ld.ks == n_ks) { ld.ks = 0; ++ld.tile; ld_set_tile(); }
-      const int rows = ld.rows;
-      const unsigned char* src = ld.ptr;
-      store(ringA);
-      issue(ringA, rows, src);
-      store(ringB);
-      issue(ringB, rows, src + 256);
-      pf_pair();
+    if constexpr (NQ == 128) {
+      issue(ringA, ld.rows, ld.ptr);
+      issue(ringB, ld.rows, ld.ptr + 256);
+      for (uint32_t item = 0; item < total_items; item += 2) {
+        // advance the load cursor to the next pair (possibly the first pair of the next tile)
+        ld.ptr += 512;
+        ld.ks += 2;
+        if (ld.ks == n_ks) { ld.ks = 0; ++ld.tile; ld_set_tile(); }
+        const int rows = ld.rows;
+        const unsigned char* src = ld.ptr;
+        store(ringA);
+        issue(ringA, rows, src);
+        store(ringB);
+        issue(ringB, rows, src + 256);
+        pf_pair();
+      }
+    } else {
+      // kLoaderRegs registers hold one item (32 KB per SM in flight)
+      issue(ringA, ld.rows, ld.ptr);
+      for (uint32_t item = 0; item < total_items; item += 2) {
+        const int rows = ld.rows;             // the pair being stored
+        const unsigned char* src = ld.ptr;
+        ld.ptr += 512;
+        ld.ks += 2;
+        if (ld.ks == n_ks) { ld.ks = 0; ++ld.tile; ld_set_tile(); }
+        store(ringA);
+        issue(ringA, rows, src + 256);
+        store(ringA);
+        issue(ringA, ld.rows, ld.ptr);
+        if constexpr (prefetch_items<NQ>() > 0) pf_pair();
+      }
     }
   } else if (warp >= kFirstLoaderWarp) {
+    if constexpr (NQ == 256) setmaxnreg_dec<kLoaderRegs>();
     // ===== corpus loaders: HBM fp32 -> registers -> fp16 -> swizzled smem (wgmma A operand) =====
     const int lt = threadIdx.x - kFirstLoaderWarp * 32;  // 0..255
     const int c4 = lt & 15;                              // float4 column within the 64-wide K slice
@@ -314,13 +370,14 @@ __global__ void __launch_bounds__(kThreads, 1) scan_wgmma_kernel(const __grid_co
     const float gscale = (METRIC == RL_METRIC_COSINE) ? 1.f : pow2_scale(t.row_stats[1]);
     // Rows are converted without a multiply when no scaling is needed (normalised corpora: the
     // cosine 1/|e| then moves to the epilogue; dot/l2: the global scale is 1).
-    const bool noscale = (METRIC == RL_METRIC_COSINE) ? cos_noscale : (gscale == 1.f);
-    const int64_t total_items = my_tiles * t.n_ks;
-    float4 ring[2][8];
+    const bool noscale = (METRIC == RL_METRIC_COSINE) ? cos_noscale_of() : (gscale == 1.f);
+    const uint32_t total_items = (uint32_t)my_tiles * (uint32_t)t.n_ks;   // (32 bits, as in the fast path)
+    constexpr int kInFlight = NQ == 128 ? 2 : 1;   // items held in registers (NQ = 256: kLoaderRegs has room for one)
+    float4 ring[kInFlight][8];
     float rs[8];
 
-    // Incremental cursors (no integer divisions or multiplies on the hot path).  `ld_*` runs two items
-    // ahead of `st_*`; `pf_*` runs kPrefetchItems ahead of `ld_*` and only touches L2.
+    // Incremental cursors (no integer divisions or multiplies on the hot path).  `ld_*` runs kInFlight items
+    // ahead of `st_*`; `pf_*` runs prefetch_items<NQ>() ahead of `ld_*` and only touches L2.
     const size_t pitch16_bytes = (size_t)a.ld * 16 * sizeof(float);   // between this thread's consecutive rows
     const size_t slice_bytes = kSliceK * sizeof(float);
     int64_t ld_tile = 0;
@@ -328,7 +385,7 @@ __global__ void __launch_bounds__(kThreads, 1) scan_wgmma_kernel(const __grid_co
     const unsigned char* ld_ptr = nullptr;                 // row r0 of the tile, column c4*4 + ld_ks*64
     auto ld_set_tile = [&]() {
       if (ld_tile < my_tiles) {
-        const int64_t blk = mode_block_index(a, ord_of(ld_tile));
+        const int64_t blk = block_of(ord_of(ld_tile));
         const int64_t rem = a.n_rows - blk * kTileM;
         ld_rows = rem < kTileM ? (int)rem : kTileM;
         ld_ptr = reinterpret_cast<const unsigned char*>(a.E + (size_t)(blk * kTileM + r0) * a.ld + c4 * 4);
@@ -342,7 +399,7 @@ __global__ void __launch_bounds__(kThreads, 1) scan_wgmma_kernel(const __grid_co
     const unsigned char* pf_ptr = nullptr;
     auto pf_set_tile = [&]() {   // only the first group's CTA pulls a tile from HBM
       if (pg == 0 && pf_tile < my_tiles) {
-        const int64_t blk = mode_block_index(a, ord_of(pf_tile));
+        const int64_t blk = block_of(ord_of(pf_tile));
         const int64_t rem = a.n_rows - blk * kTileM;
         pf_rows = rem < kTileM ? (int)rem : kTileM;
         pf_ptr = reinterpret_cast<const unsigned char*>(a.E + (size_t)(blk * kTileM + (lt >> 1)) * a.ld + (lt & 1) * 32);
@@ -362,6 +419,7 @@ __global__ void __launch_bounds__(kThreads, 1) scan_wgmma_kernel(const __grid_co
     };
     auto issue_item = [&](float4 (&buf)[8]) {
       const bool col_ok = ld_ks * kSliceK + c4 * 4 < a.d;
+      const int rows_left = ld_rows - r0;   // (one register for the eight row predicates below)
       const unsigned char* p = ld_ptr;
       if (col_ok && ld_rows == kTileM) {   // full tile: no per-row predicates
 #pragma unroll
@@ -372,7 +430,7 @@ __global__ void __launch_bounds__(kThreads, 1) scan_wgmma_kernel(const __grid_co
       } else {
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
-          if (col_ok && r0 + 16 * i < ld_rows) buf[i] = ldg_stream(reinterpret_cast<const float*>(p));
+          if (col_ok && 16 * i < rows_left) buf[i] = ldg_stream(reinterpret_cast<const float*>(p));
           else buf[i] = make_float4(0.f, 0.f, 0.f, 0.f);
           p += pitch16_bytes;
         }
@@ -383,7 +441,7 @@ __global__ void __launch_bounds__(kThreads, 1) scan_wgmma_kernel(const __grid_co
         ++ld_tile;
         ld_set_tile();
       }
-      prefetch_item();
+      if constexpr (prefetch_items<NQ>() > 0) prefetch_item();
     };
 
     int64_t st_tile = 0;
@@ -395,18 +453,18 @@ __global__ void __launch_bounds__(kThreads, 1) scan_wgmma_kernel(const __grid_co
 #pragma unroll
       for (int i = 0; i < 8; ++i) rs[i] = (METRIC == RL_METRIC_COSINE) ? 0.f : gscale;
       if (METRIC == RL_METRIC_COSINE && !noscale && tile < my_tiles) {
-        const int64_t blk = mode_block_index(a, ord_of(tile));
+        const int64_t row0 = block_of(ord_of(tile)) * kTileM + r0;
+        const int64_t rows_left = a.n_rows - row0;
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
-          const int64_t row = blk * kTileM + r0 + 16 * i;
-          if (row < a.n_rows) rs[i] = __ldg(a.inv_norm + row);
+          if (16 * i < rows_left) rs[i] = __ldg(a.inv_norm + row0 + 16 * i);
         }
       }
     };
     // Per-thread constant part of the swizzled store offset: row r = r0 + 16 i has r & 7 == r0 & 7.
     const uint32_t sw_off = (uint32_t)r0 * 128u + ((((uint32_t)c4 >> 1) ^ ((uint32_t)r0 & 7u)) << 4) + (((uint32_t)c4 & 1u) << 3);
-    // Convert + store one item, then refill its register slots with the loads of the item two
-    // ahead: two stage-loads (64 KB per SM) stay in flight.
+    // Convert + store one item, then refill its register slots with the loads of the item kInFlight
+    // ahead: kInFlight stage-loads (32 KB per SM each) stay in flight.
     auto process = [&](float4 (&buf)[8]) {
       mbar_wait(&s.empty[stage], phase ^ 1u);
       if (q_thread) put_query(stage, st_ks);
@@ -445,15 +503,17 @@ __global__ void __launch_bounds__(kThreads, 1) scan_wgmma_kernel(const __grid_co
     fetch_scales(0);
     ld_set_tile();
     pf_set_tile();
-    for (int i = 0; i < kPrefetchItems; ++i) prefetch_item();
-    issue_item(ring[0]);
-    issue_item(ring[1]);
-    for (int64_t item = 0; item < total_items; item += 2) {
+    for (int i = 0; i < prefetch_items<NQ>(); ++i) prefetch_item();
+    for (int i = 0; i < kInFlight; ++i) issue_item(ring[i]);
+    for (uint32_t item = 0; item < total_items; item += kInFlight) {
       process(ring[0]);
-      if (item + 1 < total_items) process(ring[1]);
+      if constexpr (kInFlight == 2) {
+        if (item + 1 < total_items) process(ring[1]);
+      }
     }
   } else {
     // ===== consumer warpgroups (warps 0..7): wgmma over the K slices, then the epilogue from registers =====
+    if constexpr (NQ == 256) setmaxnreg_inc<kConsumerRegs>();
     const int wg = warp >> 2;                      // rows wg * 64 .. wg * 64 + 63 of the tile
     const int r_lo = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // this thread's rows: r_lo and r_lo + 8
     const int c_lane = 2 * (lane & 3);            // this thread's columns: 8 c8 + c_lane + {0, 1}
@@ -461,7 +521,8 @@ __global__ void __launch_bounds__(kThreads, 1) scan_wgmma_kernel(const __grid_co
     bool flushed_once = false;
     int stage = 0;
     uint32_t phase = 0;
-    float acc[64];
+    float acc[NQ / 2];
+    const bool cos_noscale = cos_noscale_of();
     for (int64_t tile = 0; tile < my_tiles; ++tile) {
       // ---- MMAs: one stage per K slice; a stage is released once the wgmma of the next slice is in flight ----
       int prev = -1;
@@ -487,7 +548,7 @@ __global__ void __launch_bounds__(kThreads, 1) scan_wgmma_kernel(const __grid_co
 
       // ---- epilogue: accumulators -> keys -> dump / threshold + staged emit ----
       const int64_t ord = ord_of(tile);
-      const int64_t blk = mode_block_index(a, ord);
+      const int64_t blk = block_of(ord);
       int r_in[2];
       int64_t row[2];
       bool valid[2], masked_alive[2];
@@ -512,7 +573,7 @@ __global__ void __launch_bounds__(kThreads, 1) scan_wgmma_kernel(const __grid_co
       };
       if (a.dump_mode) {
 #pragma unroll
-        for (int c8 = 0; c8 < kMaxQ / 8; ++c8) {
+        for (int c8 = 0; c8 < NQ / 8; ++c8) {
 #pragma unroll
           for (int e = 0; e < 4; ++e) {
             const int h = e >> 1, col = 8 * c8 + c_lane + (e & 1);
@@ -524,7 +585,7 @@ __global__ void __launch_bounds__(kThreads, 1) scan_wgmma_kernel(const __grid_co
         }
       } else {
 #pragma unroll
-        for (int c8 = 0; c8 < kMaxQ / 8; ++c8) {
+        for (int c8 = 0; c8 < NQ / 8; ++c8) {
           if (8 * c8 >= nq) break;
           const int c = 8 * c8 + c_lane;
           const float2 th = *reinterpret_cast<const float2*>(s.thr + c);
@@ -568,14 +629,14 @@ __global__ void __launch_bounds__(kThreads, 1) scan_wgmma_kernel(const __grid_co
             s.list[e * 3 + 0] = (uint32_t)col | ((uint32_t)atomicAdd(&s.cnt[col], 1) << 16);
           }
           named_bar_sync(1, kNumConsumers);
-          for (int col = et; col < kMaxQ; col += kNumConsumers) {
+          for (int col = et; col < NQ; col += kNumConsumers) {
             const int c = s.cnt[col];
             if (c > 0) {
               s.basev[col] = atomicAdd(a.cand_cnt + col, c);
               s.cnt[col] = 0;
             }
           }
-          for (int w = et; w < kMaxQ * kHistBins / 2; w += kNumConsumers) {
+          for (int w = et; w < NQ * kHistBins / 2; w += kNumConsumers) {
             const uint32_t h = s.hist[w];
             if (h != 0u) {
               if (h & 0xFFFFu) atomicAdd(a.ghist + 2 * w, (int)(h & 0xFFFFu));
@@ -628,11 +689,11 @@ __global__ void __launch_bounds__(kThreads, 1) scan_wgmma_kernel(const __grid_co
 __global__ void __launch_bounds__(128) query_image_kernel(const float* __restrict__ Q, int B, int d, int metric,
                                                           const float* __restrict__ q_inv_norm,
                                                           const float* __restrict__ row_stats, float* __restrict__ q_scale,
-                                                          __half* __restrict__ qimg, int n_ks, int rows_scaled) {
+                                                          __half* __restrict__ qimg, int n_ks, int rows_scaled, int gw) {
   __shared__ float red[4];
   const int b = blockIdx.x;
-  const int group = b / kMaxQ, n = b % kMaxQ;
-  const int nq = min(kMaxQ, (B - group * kMaxQ + 15) / 16 * 16);
+  const int group = b / gw, n = b % gw;   // gw: query-group width (the scan's NQ)
+  const int nq = min(gw, (B - group * gw + 15) / 16 * 16);
   const float* q = Q + (size_t)b * d;
   float scale;
   if (metric == RL_METRIC_COSINE) {
@@ -651,7 +712,7 @@ __global__ void __launch_bounds__(128) query_image_kernel(const float* __restric
     const float rs_e = rows_scaled ? pow2_scale(row_stats[1]) : 1.f;
     if (threadIdx.x == 0) q_scale[b] = (metric == RL_METRIC_L2 ? 2.f : 1.f) / (scale * rs_e);
   }
-  __half* img = qimg + (size_t)group * n_ks * kMaxQ * kSliceK;  // groups are laid out with the full kMaxQ-row pitch
+  __half* img = qimg + (size_t)group * n_ks * gw * kSliceK;  // groups are laid out with the full gw-row pitch
   for (int c = threadIdx.x; c < n_ks * kSliceK; c += blockDim.x) {
     const int ks = c / kSliceK, e = c % kSliceK;
     const float v = c < d ? q[c] * scale : 0.f;
@@ -699,45 +760,41 @@ bool wgmma_scan_supported(const rl_scan_params* p) {
   return true;
 }
 
-size_t wgmma_qimg_bytes(int B, int d) {
-  const int n_ks = (d + kSliceK - 1) / kSliceK;
-  const int groups = (B + kMaxQ - 1) / kMaxQ;
-  return (size_t)groups * n_ks * kMaxQ * kSliceK * sizeof(__half);
+size_t wgmma_qimg_bytes(const rl_scan_params* p) {
+  const int n_ks = (p->d + kSliceK - 1) / kSliceK;
+  const int gw = query_group_width(p);
+  const int groups = (p->B + gw - 1) / gw;
+  return (size_t)groups * n_ks * gw * kSliceK * sizeof(__half);
 }
 
 int wgmma_prepare_queries(const rl_scan_params* p, const float* q_inv_norm, float* q_scale, void* qimg, cudaStream_t stream) {
   const int n_ks = (p->d + kSliceK - 1) / kSliceK;
-  RL_CUDA_CHECK(cudaMemsetAsync(qimg, 0, wgmma_qimg_bytes(p->B, p->d), stream));
+  RL_CUDA_CHECK(cudaMemsetAsync(qimg, 0, wgmma_qimg_bytes(p), stream));
   query_image_kernel<<<p->B, 128, 0, stream>>>(p->Q, p->B, p->d, p->metric, q_inv_norm, p->row_stats, q_scale,
-                                                 reinterpret_cast<__half*>(qimg), n_ks, p->e_dtype == 1 ? 0 : 1);
+                                                 reinterpret_cast<__half*>(qimg), n_ks, p->e_dtype == 1 ? 0 : 1,
+                                                 query_group_width(p));
   RL_CUDA_CHECK(cudaGetLastError());
   return RL_OK;
 }
 
-int launch_scan_wgmma(const ScanArgs& a_in, const rl_scan_params* p, const float* q_scale, const void* qimg, int sm_count,
-                      cudaStream_t stream) {
-  if (a_in.n_mode_blocks == 0 || a_in.B == 0) return RL_OK;
-  RL_REQUIRE(p->row_stats != nullptr, RL_EINVAL, "tensor-core scan needs row_stats");
+namespace {
+
+template <int NQ>
+int launch_scan_groups(const ScanArgs& a_in, const rl_scan_params* p, const float* q_scale, const void* qimg, int sm_count,
+                       const CUtensorMap& tmE, cudaStream_t stream) {
   const int n_ks = (p->d + kSliceK - 1) / kSliceK;
-  const int groups = (a_in.B + kMaxQ - 1) / kMaxQ;
-  // Up to kMaxGroups groups of 128 queries share one launch, one group per CTA, so that HBM sees the corpus once
-  // per launch; every group needs a CTA of its own in each lane.
+  const int groups = (a_in.B + NQ - 1) / NQ;
+  // Up to kMaxBatchPerLaunch / NQ groups of NQ queries share one launch, one group per CTA, so that HBM sees the
+  // corpus once per launch; every group needs a CTA of its own in each lane.
   int max_groups = sm_count / 2;
-  if (max_groups > kMaxGroups) max_groups = kMaxGroups;
+  if (max_groups > kMaxBatchPerLaunch / NQ) max_groups = kMaxBatchPerLaunch / NQ;
   if (max_groups < 1) max_groups = 1;
-  // fp16 storage: the corpus tiles go HBM -> shared memory through a tensor map (TMA writes the swizzled tile,
-  // no loader warps, no registers in between).  wgmma_scan_supported() and make_layout() already guarantee the
-  // alignment, pitch and row count the tensor map needs.
-  CUtensorMap tmE;
-  memset(&tmE, 0, sizeof(tmE));
-  RL_REQUIRE(p->e_dtype != 1 || make_corpus_tensor_map(&tmE, p->E, p->n_rows, p->ld, p->d), RL_EUNSUPPORTED,
-             "fp16 storage: no TMA tensor map for the corpus (cuTensorMapEncodeTiled unavailable or failed)");
   for (int g0 = 0; g0 < groups; g0 += max_groups) {
     TcArgs t;
     t.a = a_in;
-    const int q0 = g0 * kMaxQ;
+    const int q0 = g0 * NQ;
     const int ng = groups - g0 < max_groups ? groups - g0 : max_groups;
-    const int nb = a_in.B - q0 < ng * kMaxQ ? a_in.B - q0 : ng * kMaxQ;
+    const int nb = a_in.B - q0 < ng * NQ ? a_in.B - q0 : ng * NQ;
     t.a.B = nb;
     t.a.thr = a_in.thr + q0;
     t.a.dump = a_in.dump + (size_t)q0 * a_in.n_sample_rows;
@@ -748,21 +805,21 @@ int launch_scan_wgmma(const ScanArgs& a_in, const rl_scan_params* p, const float
     t.a.hist_inv_w = a_in.hist_inv_w + q0;
     t.a.q_inv_norm = a_in.q_inv_norm + q0;
     t.a.cnt_all = a_in.cnt_all ? a_in.cnt_all + q0 : nullptr;
-    t.qimg = reinterpret_cast<const __half*>(qimg) + (size_t)g0 * n_ks * kMaxQ * kSliceK;
+    t.qimg = reinterpret_cast<const __half*>(qimg) + (size_t)g0 * n_ks * NQ * kSliceK;
     t.q_scale = q_scale + q0;
     t.row_stats = p->row_stats;
     t.par_groups = ng;
-    const int last_b = nb - (ng - 1) * kMaxQ;              // queries of the last group
+    const int last_b = nb - (ng - 1) * NQ;                 // queries of the last group
     t.nq_last = (last_b + 15) / 16 * 16;
-    t.nq = ng > 1 ? kMaxQ : t.nq_last;                     // a full group (the only group when ng == 1)
+    t.nq = ng > 1 ? NQ : t.nq_last;                        // a full group (the only group when ng == 1)
     t.n_ks = n_ks;
-    t.pf_pairs = kPrefetchItems / 2;
-    const uint32_t avail = kSmemBudget - 1024 - tail_bytes();
-    int stages = (int)(avail / kStageBytes);
+    t.pf_pairs = prefetch_items<NQ>() / 2;
+    const uint32_t avail = kSmemBudget - 1024 - tail_bytes<NQ>();
+    int stages = (int)(avail / stage_bytes<NQ>());
     if (stages > kMaxStages) stages = kMaxStages;
     RL_REQUIRE(stages >= 2, RL_EUNSUPPORTED, "tensor-core scan: not enough shared memory for 2 stages");
     t.stages = stages;
-    const size_t smem = (size_t)stages * kStageBytes + tail_bytes() + 1024;
+    const size_t smem = (size_t)stages * stage_bytes<NQ>() + tail_bytes<NQ>() + 1024;
     auto launch = [&](auto kernel) -> int {
       RL_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
       const int lanes = sm_count / t.par_groups;
@@ -771,14 +828,41 @@ int launch_scan_wgmma(const ScanArgs& a_in, const rl_scan_params* p, const float
       RL_CUDA_CHECK(cudaGetLastError());
       return RL_OK;
     };
-    const bool f16 = p->e_dtype == 1;
     int rc;
-    if (p->metric == RL_METRIC_COSINE) rc = f16 ? launch(scan_wgmma_kernel<RL_METRIC_COSINE, true>) : launch(scan_wgmma_kernel<RL_METRIC_COSINE, false>);
-    else if (p->metric == RL_METRIC_DOT) rc = f16 ? launch(scan_wgmma_kernel<RL_METRIC_DOT, true>) : launch(scan_wgmma_kernel<RL_METRIC_DOT, false>);
-    else rc = f16 ? launch(scan_wgmma_kernel<RL_METRIC_L2, true>) : launch(scan_wgmma_kernel<RL_METRIC_L2, false>);
+    if (p->e_dtype == 1) {
+      if constexpr (NQ == 128) {   // (fp16 storage always runs groups of 128)
+        if (p->metric == RL_METRIC_COSINE) rc = launch(scan_wgmma_kernel<RL_METRIC_COSINE, true, NQ>);
+        else if (p->metric == RL_METRIC_DOT) rc = launch(scan_wgmma_kernel<RL_METRIC_DOT, true, NQ>);
+        else rc = launch(scan_wgmma_kernel<RL_METRIC_L2, true, NQ>);
+      } else {
+        RL_REQUIRE(false, RL_EUNSUPPORTED, "tensor-core scan: fp16 storage runs query groups of 128");
+      }
+    } else {
+      if (p->metric == RL_METRIC_COSINE) rc = launch(scan_wgmma_kernel<RL_METRIC_COSINE, false, NQ>);
+      else if (p->metric == RL_METRIC_DOT) rc = launch(scan_wgmma_kernel<RL_METRIC_DOT, false, NQ>);
+      else rc = launch(scan_wgmma_kernel<RL_METRIC_L2, false, NQ>);
+    }
     if (rc != RL_OK) return rc;
   }
   return RL_OK;
+}
+
+}  // namespace
+
+int launch_scan_wgmma(const ScanArgs& a_in, const rl_scan_params* p, const float* q_scale, const void* qimg, int sm_count,
+                      cudaStream_t stream) {
+  if (a_in.n_mode_blocks == 0 || a_in.B == 0) return RL_OK;
+  RL_REQUIRE(p->row_stats != nullptr, RL_EINVAL, "tensor-core scan needs row_stats");
+  // fp16 storage: the corpus tiles go HBM -> shared memory through a tensor map (TMA writes the swizzled tile,
+  // no loader warps, no registers in between).  wgmma_scan_supported() and make_layout() already guarantee the
+  // alignment, pitch and row count the tensor map needs.
+  CUtensorMap tmE;
+  memset(&tmE, 0, sizeof(tmE));
+  RL_REQUIRE(p->e_dtype != 1 || make_corpus_tensor_map(&tmE, p->E, p->n_rows, p->ld, p->d), RL_EUNSUPPORTED,
+             "fp16 storage: no TMA tensor map for the corpus (cuTensorMapEncodeTiled unavailable or failed)");
+  // the group width must match the query image wgmma_prepare_queries() built
+  if (query_group_width(p) == 256) return launch_scan_groups<256>(a_in, p, q_scale, qimg, sm_count, tmE, stream);
+  return launch_scan_groups<128>(a_in, p, q_scale, qimg, sm_count, tmE, stream);
 }
 
 }  // namespace rl

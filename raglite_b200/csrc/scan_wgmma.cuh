@@ -5,7 +5,7 @@
 namespace rl {
 
 bool wgmma_scan_supported(const rl_scan_params* p);
-size_t wgmma_qimg_bytes(int B, int d);
+size_t wgmma_qimg_bytes(const rl_scan_params* p);
 // Builds the fp16, pre-swizzled shared-memory image of the (scaled) query batch.
 int wgmma_prepare_queries(const rl_scan_params* p, const float* q_inv_norm, float* q_scale, void* qimg,
                           cudaStream_t stream);
