@@ -319,6 +319,18 @@ int rl_xenc_score(const rl_xenc_weights* w, const int32_t* input_ids, const int3
  * rl_xenc_score.  workspace: >= 4*P bytes (the length-sorted order), 16-byte aligned. */
 int rl_xenc_attention(const void* qkv, const int32_t* cu_seqlens, int P, int T, int max_len, int hidden, int n_heads,
                       void* ctx, void* workspace, size_t workspace_bytes, void* stream);
+/* Token encoder (BERT / XLM-RoBERTa, e.g. bge-m3): the embeddings and layers of rl_xenc_score without its head.
+ * out_hidden [T, H] float32 = the last layer's output LayerNorm for every token.  pooler_* and cls_* may be null.
+ * head_dim (hidden / n_heads) 32 or 64, hidden % 32 == 0 and <= 1024, ffn % 32 == 0, n_layers >= 1,
+ * 0 < max_len <= min(512, max_pos), P <= T; workspace >= rl_xenc_workspace_bytes(w, T), 16-byte aligned.  Anything
+ * else is refused with RL_EUNSUPPORTED / RL_EINVAL / RL_ENOSPACE before any CUDA call. */
+int rl_xenc_encode(const rl_xenc_weights* w, const int32_t* input_ids, const int32_t* type_ids, const int32_t* pos_ids,
+                   const int32_t* cu_seqlens, int P, int T, int max_len, float* out_hidden, void* workspace,
+                   size_t workspace_bytes, void* stream);
+/* Debug/test hook: the attention step of rl_xenc_encode on its own (arguments as rl_xenc_attention; head_dim 32 or 64,
+ * hidden <= 1024, max_len <= 512). */
+int rl_xenc_encode_attention(const void* qkv, const int32_t* cu_seqlens, int P, int T, int max_len, int hidden, int n_heads,
+                             void* ctx, void* workspace, size_t workspace_bytes, void* stream);
 
 #ifdef __cplusplus
 }

@@ -2,11 +2,12 @@
 
 Drop-in surface (reference ``raglite/__init__.py`` names for this path): ``RAGLiteConfig``,
 ``vector_search``, ``rerank_chunks``, ``embed_strings``; plus the device-resident ``CorpusIndex`` /
-``ShardedIndex`` that replace the database for this path and the batched ``vector_search_batch``.
+``ShardedIndex`` that replace the database for this path and the batched ``vector_search_batch``; and
+``TokenEmbedderEngine``, the embedding model's encoder on the GPU behind ``embed_strings`` / ``embed_queries``.
 """
 
 from ._config import RAGLiteConfig
-from ._embed import embed_strings, register_token_embedder
+from ._embed import embed_queries, embed_strings, register_token_embedder
 from ._index import Chunk, CorpusIndex, get_index, merge_hits, register_index, unregister_index
 from ._query_adapter import update_query_adapter
 from ._search import (
@@ -25,16 +26,19 @@ from ._search import (
     vector_search_batch,
     vector_search_batch_async,
 )
+from ._xenc import TokenEmbedderEngine
 
 __all__ = [
     "Chunk",
     "ChunkSpan",
     "CorpusIndex",
     "RAGLiteConfig",
+    "TokenEmbedderEngine",
     "collate_spans_device",
     "hybrid_search",
     "register_keyword_search",
     "rrf_fuse_device",
+    "embed_queries",
     "embed_strings",
     "get_index",
     "merge_hits",

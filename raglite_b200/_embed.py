@@ -2,9 +2,11 @@
 
 Mirrors ``raglite/_embed.py``: ``embed_strings`` dispatches on the embedder string (``:193-200``);
 the late-chunking path (``:16-141``) counts tokens with the sentinel trick, cuts the document into
-preamble+content segments, asks the token embedder (llama.cpp in the reference -- out of scope here,
-any object with ``n_ctx() / n_batch / tokenize / detokenize / embed``) for per-token embeddings, and
-then pools.  The pool itself -- largest-remainder split, per-sentence mean, L2 normalise, fp16 cast
+preamble+content segments, asks the token embedder (llama.cpp in the reference; here any object with
+``n_ctx() / n_batch / tokenize / detokenize / embed``, e.g. ``TokenEmbedderEngine``, which runs the encoder
+on the GPU) for per-token embeddings, and then pools.  An embedder that also offers the packed device path
+(``token_ids_for_embedding`` + ``embed_token_ids``, as ``TokenEmbedderEngine`` does) runs every segment
+of a call in one packed forward, and the pool reads its output where it lies on the device.  The pool itself -- largest-remainder split, per-sentence mean, L2 normalise, fp16 cast
 (``:122-140``) -- is what this package accelerates: sizes are computed on the host with the same
 NumPy calls as the reference, the arithmetic runs in ``rl_segment_mean_pool``.
 """
@@ -119,25 +121,48 @@ def segment_mean_pool(X: torch.Tensor, row_begin: np.ndarray, row_end: np.ndarra
     return out
 
 
+def _device_path(model: Any) -> bool:
+    """Whether the embedder runs packed forwards whose token rows stay on the device."""
+    return hasattr(model, "embed_token_ids") and hasattr(model, "token_ids_for_embedding")
+
+
 def pool_segments(  # noqa: PLR0913
-    segment_embeddings: Sequence[np.ndarray | torch.Tensor], num_tokens: np.ndarray,
+    segment_embeddings: Sequence[np.ndarray | torch.Tensor] | torch.Tensor, num_tokens: np.ndarray,
     segments: Sequence[tuple[int, int, int]], *, normalize: bool = True, device: Any | None = None,
+    row_offsets: np.ndarray | None = None,
 ) -> torch.Tensor:
     """Pool all segments of a document in ONE kernel launch: stack the token matrices, list the
-    content sentences' row ranges (preamble sentences are skipped, ``_embed.py:133``)."""
-    device = torch.device(device if device is not None else "cuda")
-    mats = [torch.as_tensor(np.asarray(x, dtype=np.float32) if not isinstance(x, torch.Tensor) else x)
-            for x in segment_embeddings]
-    X = torch.cat([m.to(device=device, dtype=torch.float32, non_blocking=True) for m in mats], dim=0)
+    content sentences' row ranges (preamble sentences are skipped, ``_embed.py:133``).  With ``row_offsets``
+    (``[n_segments + 1]``), ``segment_embeddings`` is already the packed float32 ``[T, d]`` device matrix and
+    segment i owns its rows ``row_offsets[i] : row_offsets[i + 1]``."""
+    if row_offsets is None:
+        device = torch.device(device if device is not None else "cuda")
+        mats = [torch.as_tensor(np.asarray(x, dtype=np.float32) if not isinstance(x, torch.Tensor) else x)
+                for x in segment_embeddings]
+        X = torch.cat([m.to(device=device, dtype=torch.float32, non_blocking=True) for m in mats], dim=0)
+        rows = [int(m.shape[0]) for m in mats]
+    else:
+        X = segment_embeddings
+        rows = np.diff(np.asarray(row_offsets)).tolist()
     begins, ends = [], []
     base = 0
-    for m, (s, c, e) in zip(mats, segments, strict=True):
-        sizes = largest_remainder_sizes(int(m.shape[0]), np.asarray(num_tokens[s:e]))
+    for n, (s, c, e) in zip(rows, segments, strict=True):
+        sizes = largest_remainder_sizes(n, np.asarray(num_tokens[s:e]))
         cuts = np.concatenate([[0], np.cumsum(sizes)]) + base
         begins.append(cuts[c - s : -1])
         ends.append(cuts[c - s + 1 :])
-        base += int(m.shape[0])
+        base += n
     return segment_mean_pool(X.contiguous(), np.concatenate(begins), np.concatenate(ends), normalize=1 if normalize else 0)
+
+
+def _pool_planned(model: Any, texts: list[str], num_tokens: np.ndarray, segments: list[tuple[int, int, int]], *,
+                  normalize: bool) -> torch.Tensor:
+    """Embed the planned segments (``texts[i]`` is the text of ``segments[i]``) and pool them."""
+    if _device_path(model):
+        X, offs = model.embed_token_ids(model.token_ids_for_embedding(texts))
+        return pool_segments(X, num_tokens, segments, normalize=normalize, row_offsets=offs)
+    seg_emb = [np.asarray(model.embed(t), dtype=np.float32) for t in texts]
+    return pool_segments(seg_emb, num_tokens, segments, normalize=normalize)
 
 
 def embed_strings_with_late_chunking(sentences: list[str], *, config: RAGLiteConfig | None = None) -> FloatMatrix:
@@ -147,9 +172,8 @@ def embed_strings_with_late_chunking(sentences: list[str], *, config: RAGLiteCon
     model = _token_embedder(config)
     num_tokens = count_tokens(sentences, model)
     segments = plan_segments(num_tokens, model.n_ctx(), model.n_batch)
-    seg_emb = [np.asarray(model.embed("".join(sentences[s:e])), dtype=np.float32) for (s, _, e) in segments]
-    out = pool_segments(seg_emb, num_tokens, segments, normalize=config.embedder_normalize)
-    return out.cpu().numpy()
+    texts = ["".join(sentences[s:e]) for (s, _, e) in segments]
+    return _pool_planned(model, texts, num_tokens, segments, normalize=config.embedder_normalize).cpu().numpy()
 
 
 def embed_strings_without_late_chunking(strings: list[str], *, config: RAGLiteConfig | None = None) -> FloatMatrix:
@@ -157,6 +181,9 @@ def embed_strings_without_late_chunking(strings: list[str], *, config: RAGLiteCo
     (LiteLLM) are outside the accelerated path."""
     config = config or RAGLiteConfig()
     model = _token_embedder(config)
+    if _device_path(model):
+        X, offs = model.embed_token_ids(model.token_ids_for_embedding(list(strings)))
+        return segment_mean_pool(X, offs[:-1], offs[1:], normalize=2 if config.embedder_normalize else 0).cpu().numpy()
     outs = []
     for i in range(0, len(strings), 96):  # batch size 96 (_embed.py:173)
         mats = [np.asarray(m, dtype=np.float32) for m in model.embed(list(strings[i : i + 96]))]
@@ -164,6 +191,32 @@ def embed_strings_without_late_chunking(strings: list[str], *, config: RAGLiteCo
         cuts = np.concatenate([[0], np.cumsum([len(m) for m in mats])])
         outs.append(segment_mean_pool(X, cuts[:-1], cuts[1:], normalize=2 if config.embedder_normalize else 0))
     return torch.cat(outs, dim=0).cpu().numpy()
+
+
+def embed_queries(queries: Sequence[str], *, config: RAGLiteConfig | None = None) -> FloatMatrix:
+    """fp16 ``[B, d]`` embeddings of a batch of query strings; row b equals ``embed_strings([queries[b]])[0]`` bit for
+    bit.  Each query is planned as a one-sentence document, exactly as ``embed_strings`` plans it, and all of their
+    segments run in one packed forward and one pool launch, ready for ``vector_search_batch(...,
+    queries_are_fp16=True)``.  An embedder without the device path embeds the queries one by one."""
+    config = config or RAGLiteConfig()
+    queries = list(queries)
+    model = _token_embedder(config)
+    if not queries or not _device_path(model):
+        rows = [embed_strings([q], config=config)[0] for q in queries]
+        return np.stack(rows) if rows else np.zeros((0, model.n_embd()), dtype=np.float16)
+    if embedding_type(config=config) != "late_chunking":
+        return embed_strings_without_late_chunking(queries, config=config)
+    texts, all_tokens, all_segments = [], [], []
+    base = 0
+    for q in queries:
+        num_tokens = count_tokens([q], model)
+        for s, c, e in plan_segments(num_tokens, model.n_ctx(), model.n_batch):
+            texts.append(q)   # ("".join of the query's single sentence)
+            all_segments.append((s + base, c + base, e + base))
+        all_tokens.append(num_tokens)
+        base += len(num_tokens)
+    return _pool_planned(model, texts, np.concatenate(all_tokens), all_segments,
+                         normalize=config.embedder_normalize).cpu().numpy()
 
 
 def embedding_type(*, config: RAGLiteConfig | None = None) -> str:

@@ -25,7 +25,7 @@ EXPORTS = [
     "rl_version", "rl_last_error", "rl_device_info", "rl_row_stats", "rl_row_stats_f16", "rl_chunk_row_map", "rl_adapter_apply",
     "rl_maxsim_workspace_bytes", "rl_maxsim_topk", "rl_maxsim_count_at_least", "rl_maxsim_unfiltered_bound", "rl_maxsim_stats", "rl_maxsim_kernel_times", "rl_maxsim_release", "rl_maxsim_copy_dump", "rl_maxsim_copy_eps", "rl_topk_merge", "rl_topk_merge_packed", "rl_hits_packed_bytes", "rl_row_mask", "rl_rrf_fuse", "rl_span_collate", "rl_best_vectors", "rl_adapter_targets",
     "rl_segment_mean_pool", "rl_xenc_linear_image_bytes", "rl_xenc_pack_linear", "rl_xenc_linear",
-    "rl_xenc_workspace_bytes", "rl_xenc_score", "rl_xenc_attention",
+    "rl_xenc_workspace_bytes", "rl_xenc_score", "rl_xenc_attention", "rl_xenc_encode", "rl_xenc_encode_attention",
 ]
 
 
@@ -106,6 +106,8 @@ def _declare(lib: C.CDLL) -> None:
     lib.rl_xenc_workspace_bytes.restype = C.c_size_t
     lib.rl_xenc_score.argtypes = [C.POINTER(XencWeights), vp, vp, vp, vp, i32, i32, i32, vp, vp, vp, C.c_size_t, vp]
     lib.rl_xenc_attention.argtypes = [vp, vp, i32, i32, i32, i32, i32, vp, vp, C.c_size_t, vp]
+    lib.rl_xenc_encode.argtypes = [C.POINTER(XencWeights), vp, vp, vp, vp, i32, i32, i32, vp, vp, C.c_size_t, vp]
+    lib.rl_xenc_encode_attention.argtypes = [vp, vp, i32, i32, i32, i32, i32, vp, vp, C.c_size_t, vp]
     for name in EXPORTS:
         if name not in ("rl_last_error", "rl_maxsim_workspace_bytes", "rl_xenc_linear_image_bytes", "rl_xenc_workspace_bytes",
                         "rl_hits_packed_bytes"):

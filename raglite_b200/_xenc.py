@@ -5,6 +5,10 @@ FlashRankRanker: tokenise (query, passage) pairs, run ms-marco-MiniLM-L-12-v2 (B
 12 heads, FFN=1536) with onnxruntime, sigmoid the logit, sort.  Here the forward runs in
 ``rl_xenc_score`` (hand-written CUDA: wgmma linear layers with fused bias/GELU, attention,
 LayerNorm, pooler+classifier) on packed variable-length batches -- no padding tokens are computed.
+
+``TokenEmbedderEngine`` runs the same encoder without the head (``rl_xenc_encode``: head_dim 32 or 64, H <= 1024) and
+returns per-token hidden states: the embedding model behind ``embed_strings`` (bge-m3 by default), which the reference
+runs in llama.cpp.
 """
 
 from __future__ import annotations
@@ -55,42 +59,41 @@ def random_minilm_state_dict(seed: int = 0, *, n_layers: int = 12, hidden: int =
     return sd
 
 
-class CrossEncoderEngine:
-    """Device-resident packed weights + tokenizer + batching."""
+def _pack_inputs(h: np.ndarray, ids: Sequence[np.ndarray], type_ids: Sequence[np.ndarray] | None, lens: np.ndarray,
+                 pos_offset: int) -> int:
+    """Lay one packed call out in the int32 array ``h``: ids [T] | type ids [T] | position ids [T] | cu_seqlens [P + 1].
+    Position ids run ``pos_offset + i`` per sequence (0 for BERT; ``padding_idx + 1`` for XLM-RoBERTa, whose table
+    keeps rows for the padding index and below); type ids are 0 when ``type_ids`` is None.  Returns T."""
+    P, T = len(ids), int(lens.sum())
+    if T:
+        np.concatenate(ids, out=h[:T], casting="unsafe")
+    if type_ids is None:
+        h[T:2 * T] = 0
+    elif T:
+        np.concatenate(type_ids, out=h[T:2 * T], casting="unsafe")
+    cu = h[3 * T:3 * T + P + 1]
+    cu[0] = 0
+    np.cumsum(lens, out=cu[1:])
+    h[2 * T:3 * T] = np.arange(T, dtype=np.int32) - np.repeat(cu[:-1], lens) + pos_offset
+    return T
+
+
+class _EncoderEngine:
+    """Device-resident packed encoder weights (embeddings + layers), the workspace and the pinned double-buffered call
+    pipeline: what the cross-encoder and the token embedder share."""
 
     def __init__(self, state_dict: dict[str, torch.Tensor], *, n_layers: int, hidden: int, n_heads: int, ffn: int,
-                 max_pos: int, ln_eps: float = 1e-12, tokenizer: Any | None = None, max_length: int = 512,
-                 device: Any | None = None, max_tokens_per_call: int = 1 << 18) -> None:
+                 max_pos: int, ln_eps: float, device: Any | None, max_tokens_per_call: int, pos_offset: int = 0) -> None:
         if not torch.cuda.is_available():
             raise RuntimeError("raglite_b200 needs a CUDA device (there is no CPU fallback)")
         self.lib = _lib.load()
         self.device = torch.device(device if device is not None else f"cuda:{torch.cuda.current_device()}")
-        self.tokenizer = tokenizer
-        self.max_length = min(max_length, max_pos)
         self.max_tokens_per_call = max_tokens_per_call
         self.hidden, self.n_layers = hidden, n_layers
+        self.pos_offset = pos_offset
         self._keep: list[torch.Tensor] = []
-        sd = {k.removeprefix("bert."): v for k, v in state_dict.items()}
-
-        def f32(name: str) -> torch.Tensor:
-            t = sd[name].detach().to(device=self.device, dtype=torch.float32).contiguous()
-            self._keep.append(t)
-            return t
-
-        def f16(name: str) -> torch.Tensor:
-            t = sd[name].detach().to(device=self.device, dtype=torch.float16).contiguous()
-            self._keep.append(t)
-            return t
-
-        def packed(weight: torch.Tensor) -> torch.Tensor:
-            W = weight.detach().to(device=self.device, dtype=torch.float32).contiguous()
-            N, K = W.shape
-            img = torch.empty(int(self.lib.rl_xenc_linear_image_bytes(N, K)), dtype=torch.uint8, device=self.device)
-            with torch.cuda.device(self.device):
-                check(self.lib.rl_xenc_pack_linear(W.data_ptr(), N, K, img.data_ptr(), _stream()), "rl_xenc_pack_linear")
-                torch.cuda.current_stream().synchronize()
-            self._keep.append(img)
-            return img
+        sd = {k.removeprefix("bert.").removeprefix("roberta."): v for k, v in state_dict.items()}
+        self._sd = sd
 
         self._layers = (XencLayer * n_layers)()
         for l in range(n_layers):
@@ -100,33 +103,127 @@ class CrossEncoderEngine:
             qkv_b = qkv_b.detach().to(device=self.device, dtype=torch.float32).contiguous()
             self._keep.append(qkv_b)
             L = self._layers[l]
-            L.qkv_img, L.qkv_bias = packed(qkv_w).data_ptr(), qkv_b.data_ptr()
-            L.o_img, L.o_bias = packed(sd[pre + "attention.output.dense.weight"]).data_ptr(), f32(pre + "attention.output.dense.bias").data_ptr()
-            L.ln1_g, L.ln1_b = f32(pre + "attention.output.LayerNorm.weight").data_ptr(), f32(pre + "attention.output.LayerNorm.bias").data_ptr()
-            L.up_img, L.up_bias = packed(sd[pre + "intermediate.dense.weight"]).data_ptr(), f32(pre + "intermediate.dense.bias").data_ptr()
-            L.down_img, L.down_bias = packed(sd[pre + "output.dense.weight"]).data_ptr(), f32(pre + "output.dense.bias").data_ptr()
-            L.ln2_g, L.ln2_b = f32(pre + "output.LayerNorm.weight").data_ptr(), f32(pre + "output.LayerNorm.bias").data_ptr()
+            L.qkv_img, L.qkv_bias = self._packed(qkv_w).data_ptr(), qkv_b.data_ptr()
+            L.o_img, L.o_bias = self._packed(sd[pre + "attention.output.dense.weight"]).data_ptr(), self._f32(pre + "attention.output.dense.bias").data_ptr()
+            L.ln1_g, L.ln1_b = self._f32(pre + "attention.output.LayerNorm.weight").data_ptr(), self._f32(pre + "attention.output.LayerNorm.bias").data_ptr()
+            L.up_img, L.up_bias = self._packed(sd[pre + "intermediate.dense.weight"]).data_ptr(), self._f32(pre + "intermediate.dense.bias").data_ptr()
+            L.down_img, L.down_bias = self._packed(sd[pre + "output.dense.weight"]).data_ptr(), self._f32(pre + "output.dense.bias").data_ptr()
+            L.ln2_g, L.ln2_b = self._f32(pre + "output.LayerNorm.weight").data_ptr(), self._f32(pre + "output.LayerNorm.bias").data_ptr()
         w = XencWeights()
         w.n_layers, w.hidden, w.n_heads, w.ffn = n_layers, hidden, n_heads, ffn
         w.vocab, w.max_pos = int(sd["embeddings.word_embeddings.weight"].shape[0]), max_pos
         w.type_vocab, w.ln_eps = int(sd["embeddings.token_type_embeddings.weight"].shape[0]), ln_eps
-        w.word_emb = f16("embeddings.word_embeddings.weight").data_ptr()
-        w.pos_emb = f16("embeddings.position_embeddings.weight").data_ptr()
-        w.type_emb = f16("embeddings.token_type_embeddings.weight").data_ptr()
-        w.emb_ln_g, w.emb_ln_b = f32("embeddings.LayerNorm.weight").data_ptr(), f32("embeddings.LayerNorm.bias").data_ptr()
+        w.word_emb = self._f16("embeddings.word_embeddings.weight").data_ptr()
+        w.pos_emb = self._f16("embeddings.position_embeddings.weight").data_ptr()
+        w.type_emb = self._f16("embeddings.token_type_embeddings.weight").data_ptr()
+        w.emb_ln_g, w.emb_ln_b = self._f32("embeddings.LayerNorm.weight").data_ptr(), self._f32("embeddings.LayerNorm.bias").data_ptr()
         w.layers = C.cast(self._layers, C.POINTER(XencLayer))
-        w.pooler_w, w.pooler_b = f32("pooler.dense.weight").data_ptr(), f32("pooler.dense.bias").data_ptr()
+        self.weights = w
+        self._ws: torch.Tensor | None = None
+        self._host_bufs: dict[str, torch.Tensor] = {}   # pinned staging (double-buffered inputs / outputs)
+        self._dev_bufs: dict[int, torch.Tensor] = {}
+        self._lock = threading.RLock()   # reference callers rerank from thread pools (_rag.py:317)
+
+    def _f32(self, name: str) -> torch.Tensor:
+        t = self._sd[name].detach().to(device=self.device, dtype=torch.float32).contiguous()
+        self._keep.append(t)
+        return t
+
+    def _f16(self, name: str) -> torch.Tensor:
+        t = self._sd[name].detach().to(device=self.device, dtype=torch.float16).contiguous()
+        self._keep.append(t)
+        return t
+
+    def _packed(self, weight: torch.Tensor) -> torch.Tensor:
+        W = weight.detach().to(device=self.device, dtype=torch.float32).contiguous()
+        N, K = W.shape
+        img = torch.empty(int(self.lib.rl_xenc_linear_image_bytes(N, K)), dtype=torch.uint8, device=self.device)
+        with torch.cuda.device(self.device):
+            check(self.lib.rl_xenc_pack_linear(W.data_ptr(), N, K, img.data_ptr(), _stream()), "rl_xenc_pack_linear")
+            torch.cuda.current_stream().synchronize()
+        self._keep.append(img)
+        return img
+
+    def _pipelined(self, lens: np.ndarray, launch: Any, collect: Any) -> None:
+        """Cut the sequences into calls of at most ``max_tokens_per_call`` tokens and pipeline them: while the GPU runs
+        call *i*, the host packs call *i+1* into the other half of a pinned double buffer and enqueues its upload and
+        kernels; call *i* is only waited for (``collect(lo, hi, item)``) once the next call is in the queue.  A pinned
+        half is refilled two calls later, after its call was collected.  ``launch(lo, hi, slot)`` returns ``item``."""
+        P = len(lens)
+        cuts = [0]
+        tok = 0
+        for i in range(P):
+            if i > cuts[-1] and tok + lens[i] > self.max_tokens_per_call:
+                cuts.append(i)
+                tok = 0
+            tok += int(lens[i])
+        cuts.append(P)
+        with self._lock, torch.cuda.device(self.device):
+            pending: tuple[int, int, Any] | None = None
+            for c in range(len(cuts) - 1):
+                lo, hi = cuts[c], cuts[c + 1]
+                if hi == lo:
+                    continue
+                item = launch(lo, hi, c & 1)
+                if pending is not None:
+                    collect(*pending)
+                pending = (lo, hi, item)
+            if pending is not None:
+                collect(*pending)
+
+    def _pinned(self, name: str, n: int, dtype: torch.dtype) -> torch.Tensor:
+        buf = self._host_bufs.get(name)
+        if buf is None or buf.numel() < n:
+            buf = torch.empty(max(n, 1024), dtype=dtype, pin_memory=True)
+            self._host_bufs[name] = buf
+        return buf
+
+    def _upload_packed(self, ids: Sequence[np.ndarray], type_ids: Sequence[np.ndarray] | None, lens: np.ndarray, *, slot: int
+                       ) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]:
+        """Pack one call into pinned buffer ``slot`` and enqueue its upload; returns the device ids, type ids, position
+        ids and cu_seqlens, and makes sure the workspace holds the call.  Caller holds the lock."""
+        P, T = len(ids), int(lens.sum())
+        n_in = 3 * T + P + 1
+        host_in = self._pinned(f"in{slot}", n_in, torch.int32)
+        h = host_in.numpy()
+        _pack_inputs(h, ids, type_ids, lens, self.pos_offset)
+        # A tokenizer that does not match the weights would index past the embedding tables.
+        w = self.weights
+        if T and (int(h[:T].min()) < 0 or int(h[:T].max()) >= w.vocab):
+            raise ValueError(f"token id outside the model's vocabulary [0, {w.vocab}) -- tokenizer / weights mismatch?")
+        if T and (int(h[T:2 * T].min()) < 0 or int(h[T:2 * T].max()) >= w.type_vocab):
+            raise ValueError(f"token type id outside [0, {w.type_vocab})")
+        if P and int(lens.max()) + self.pos_offset > w.max_pos:
+            raise ValueError(f"sequence longer than the model's {w.max_pos - self.pos_offset} positions")
+        dev = self._dev_bufs.get(slot)
+        if dev is None or dev.numel() < n_in:
+            dev = torch.empty(max(n_in, 1024), dtype=torch.int32, device=self.device)
+            self._dev_bufs[slot] = dev
+        dev[:n_in].copy_(host_in[:n_in], non_blocking=True)
+        need = int(self.lib.rl_xenc_workspace_bytes(C.byref(self.weights), T))
+        if self._ws is None or self._ws.numel() < need:
+            self._ws = torch.empty(need, dtype=torch.uint8, device=self.device)
+        return dev[:T], dev[T:2 * T], dev[2 * T:3 * T], dev[3 * T:n_in]
+
+
+class CrossEncoderEngine(_EncoderEngine):
+    """Device-resident packed weights + tokenizer + batching."""
+
+    def __init__(self, state_dict: dict[str, torch.Tensor], *, n_layers: int, hidden: int, n_heads: int, ffn: int,
+                 max_pos: int, ln_eps: float = 1e-12, tokenizer: Any | None = None, max_length: int = 512,
+                 device: Any | None = None, max_tokens_per_call: int = 1 << 18) -> None:
+        super().__init__(state_dict, n_layers=n_layers, hidden=hidden, n_heads=n_heads, ffn=ffn, max_pos=max_pos,
+                         ln_eps=ln_eps, device=device, max_tokens_per_call=max_tokens_per_call)
+        self.tokenizer = tokenizer
+        self.max_length = min(max_length, max_pos)
+        w = self.weights
+        w.pooler_w, w.pooler_b = self._f32("pooler.dense.weight").data_ptr(), self._f32("pooler.dense.bias").data_ptr()
         cls_w = state_dict["classifier.weight"].detach().to(device=self.device, dtype=torch.float32).reshape(-1).contiguous()
         if cls_w.numel() != hidden:
             raise ValueError("only single-logit classifiers (num_labels == 1) are supported")
         cls_b = state_dict["classifier.bias"].detach().to(device=self.device, dtype=torch.float32).contiguous()
         self._keep += [cls_w, cls_b]
         w.cls_w, w.cls_b = cls_w.data_ptr(), cls_b.data_ptr()
-        self.weights = w
-        self._ws: torch.Tensor | None = None
-        self._host_bufs: dict[str, torch.Tensor] = {}   # pinned staging (double-buffered inputs / outputs)
-        self._dev_bufs: dict[int, torch.Tensor] = {}
-        self._lock = threading.RLock()   # reference callers rerank from thread pools (_rag.py:317)
 
     # ---- constructors ------------------------------------------------------------------------------
     @classmethod
@@ -164,75 +261,28 @@ class CrossEncoderEngine:
         lens = np.fromiter((len(x) for x in ids), dtype=np.int64, count=P)
         if P and lens.max() > self.max_length:
             raise ValueError("sequence longer than max_length")
-        cuts = [0]
-        tok = 0
-        for i in range(P):
-            if i > cuts[-1] and tok + lens[i] > self.max_tokens_per_call:
-                cuts.append(i)
-                tok = 0
-            tok += int(lens[i])
-        cuts.append(P)
-        with self._lock, torch.cuda.device(self.device):
-            pending: tuple[int, int, torch.Tensor, torch.cuda.Event] | None = None
-            for c in range(len(cuts) - 1):
-                lo, hi = cuts[c], cuts[c + 1]
-                if hi == lo:
-                    continue
-                item = self._launch_packed(ids[lo:hi], type_ids[lo:hi], lens[lo:hi], slot=c & 1)
-                if pending is not None:
-                    self._collect(pending, logits, scores)
-                pending = (lo, hi, *item)
-            if pending is not None:
-                self._collect(pending, logits, scores)
+
+        def launch(lo: int, hi: int, slot: int) -> tuple[torch.Tensor, torch.cuda.Event]:
+            return self._launch_packed(ids[lo:hi], type_ids[lo:hi], lens[lo:hi], slot=slot)
+
+        def collect(lo: int, hi: int, item: tuple[torch.Tensor, torch.cuda.Event]) -> None:
+            host, ev = item
+            ev.synchronize()
+            res = host.numpy()[: 2 * (hi - lo)].reshape(2, hi - lo)
+            logits[lo:hi], scores[lo:hi] = res[0], res[1]
+
+        self._pipelined(lens, launch, collect)
         return logits, scores
-
-    def _collect(self, pending: tuple[int, int, torch.Tensor, torch.cuda.Event], logits: np.ndarray, scores: np.ndarray) -> None:
-        lo, hi, host, ev = pending
-        ev.synchronize()
-        res = host.numpy()[: 2 * (hi - lo)].reshape(2, hi - lo)
-        logits[lo:hi], scores[lo:hi] = res[0], res[1]
-
-    def _pinned(self, name: str, n: int, dtype: torch.dtype) -> torch.Tensor:
-        buf = self._host_bufs.get(name)
-        if buf is None or buf.numel() < n:
-            buf = torch.empty(max(n, 1024), dtype=dtype, pin_memory=True)
-            self._host_bufs[name] = buf
-        return buf
 
     def _launch_packed(self, ids: Sequence[np.ndarray], type_ids: Sequence[np.ndarray], lens: np.ndarray, *, slot: int
                        ) -> tuple[torch.Tensor, torch.cuda.Event]:
         """Pack one call into pinned buffer ``slot``, enqueue upload + forward + download; returns the pinned
         result buffer and the event that marks it complete.  Caller holds the lock."""
-        P, T = len(ids), int(lens.sum())
-        n_in = 3 * T + P + 1
-        host_in = self._pinned(f"in{slot}", n_in, torch.int32)
-        h = host_in.numpy()
-        np.concatenate(ids, out=h[:T], casting="unsafe")
-        np.concatenate(type_ids, out=h[T:2 * T], casting="unsafe")
-        cu = h[3 * T:3 * T + P + 1]
-        cu[0] = 0
-        np.cumsum(lens, out=cu[1:])
-        h[2 * T:3 * T] = np.arange(T, dtype=np.int32) - np.repeat(cu[:-1], lens)      # position ids 0..len-1 per pair
-        # A tokenizer that does not match the weights would index past the embedding tables.
-        w = self.weights
-        if T and (int(h[:T].min()) < 0 or int(h[:T].max()) >= w.vocab):
-            raise ValueError(f"token id outside the model's vocabulary [0, {w.vocab}) -- tokenizer / weights mismatch?")
-        if T and (int(h[T:2 * T].min()) < 0 or int(h[T:2 * T].max()) >= w.type_vocab):
-            raise ValueError(f"token type id outside [0, {w.type_vocab})")
-        if P and int(lens.max()) > w.max_pos:
-            raise ValueError(f"sequence longer than the model's {w.max_pos} positions")
-        dev = self._dev_bufs.get(slot)
-        if dev is None or dev.numel() < n_in:
-            dev = torch.empty(max(n_in, 1024), dtype=torch.int32, device=self.device)
-            self._dev_bufs[slot] = dev
-        dev[:n_in].copy_(host_in[:n_in], non_blocking=True)
-        d_ids, d_types, d_pos, d_cu = dev[:T], dev[T:2 * T], dev[2 * T:3 * T], dev[3 * T:n_in]
+        P = len(ids)
+        d_ids, d_types, d_pos, d_cu = self._upload_packed(ids, type_ids, lens, slot=slot)
         out = torch.empty((2, P), dtype=torch.float32, device=self.device)
-        need = int(self.lib.rl_xenc_workspace_bytes(C.byref(self.weights), T))
-        if self._ws is None or self._ws.numel() < need:
-            self._ws = torch.empty(need, dtype=torch.uint8, device=self.device)
         check(self.lib.rl_xenc_score(C.byref(self.weights), d_ids.data_ptr(), d_types.data_ptr(), d_pos.data_ptr(),
-                                     d_cu.data_ptr(), P, T, int(lens.max()), out[0].data_ptr(), out[1].data_ptr(),
+                                     d_cu.data_ptr(), P, len(d_ids), int(lens.max()), out[0].data_ptr(), out[1].data_ptr(),
                                      self._ws.data_ptr(), self._ws.numel(), _stream()), "rl_xenc_score")
         host_out = self._pinned(f"out{slot}", 2 * P, torch.float32)
         host_out[: 2 * P].copy_(out.reshape(-1), non_blocking=True)
@@ -261,3 +311,156 @@ class CrossEncoderEngine:
     def score_pairs(self, queries: Sequence[str], docs: Sequence[str]) -> list[float]:
         ids, types = self.encode_pairs(queries, docs)
         return [float(s) for s in self.score_tokens(ids, types)[1]]
+
+
+# ---- token embedder (late-chunking ingest, string queries) -------------------------------------------------------------
+# Tokens per forward call of TokenEmbedderEngine: 65,536 tokens take about 1.34 GB of workspace and 0.27 GB of fp32
+# output at bge-m3's shape (H = 1024, FFN = 4096: ~20 KB of workspace per token); the cross-encoder's 2^18 would take
+# 5.4 GB + 1.1 GB.  A call of 2^16 tokens is already ~130 tokens per SM per linear layer pass.
+EMBED_TOKENS_PER_CALL = 1 << 16
+
+
+class EmbedderTokenizer:
+    """The llama-like tokenizer side of ``TokenEmbedderEngine`` (host only): ``n_ctx() / n_batch / tokenize /
+    detokenize`` as ``raglite_b200._embed`` calls them, over a ``tokenizers.Tokenizer`` (or a transformers fast
+    tokenizer, whose backend is used).  ``token_ids_for_embedding`` adds the tokenizer's special tokens
+    (``<s> ... </s>`` / ``[CLS] ... [SEP]``) and truncates to ``n_batch`` tokens, as llama-cpp-python's
+    ``embed(truncate=True)`` does."""
+
+    def __init__(self, tokenizer: Any, n_ctx: int) -> None:
+        from tokenizers import Tokenizer
+
+        tok = getattr(tokenizer, "backend_tokenizer", tokenizer)
+        self.tokenizer = Tokenizer.from_str(tok.to_str())   # a private copy: truncation / padding are turned off here
+        self.tokenizer.no_truncation()
+        self.tokenizer.no_padding()
+        self._n_ctx = int(n_ctx)
+        self.n_batch = int(n_ctx)
+
+    def n_ctx(self) -> int:
+        return self._n_ctx
+
+    def tokenize(self, text: bytes, add_bos: bool = False, special: bool = False) -> list[int]:  # noqa: ARG002
+        """Token ids of ``text`` without special tokens (``add_bos`` / ``special`` only mirror llama.cpp's signature)."""
+        return list(self.tokenizer.encode(text.decode(), add_special_tokens=False).ids)
+
+    def detokenize(self, tokens: Sequence[int]) -> bytes:
+        return self.tokenizer.decode([int(t) for t in tokens], skip_special_tokens=False).encode()
+
+    def token_ids_for_embedding(self, texts: Sequence[str]) -> list[np.ndarray]:
+        enc = self.tokenizer.encode_batch(list(texts), add_special_tokens=True)
+        return [np.asarray(e.ids[: self.n_batch], dtype=np.int32) for e in enc]
+
+
+def _position_offset(config: Any) -> int:
+    """First position id of a sequence: XLM-RoBERTa counts from ``padding_idx + 1`` (its table keeps rows for the
+    padding index and below), BERT from 0."""
+    if config.model_type in ("xlm-roberta", "roberta"):
+        return int(config.pad_token_id) + 1
+    if config.model_type == "bert":
+        return 0
+    raise ValueError(f"unsupported encoder model type {config.model_type!r} (BERT or XLM-RoBERTa)")
+
+
+class TokenEmbedderEngine(_EncoderEngine):
+    """Per-token embeddings of a BERT / XLM-RoBERTa encoder (bge-m3: XLM-RoBERTa, 24 layers, H = 1024, 16 heads x 64,
+    FFN 4096) on the GPU: the forward runs in ``rl_xenc_encode`` and returns the last layer's LayerNorm output of every
+    token in float32.  It implements the llama-like protocol of ``raglite_b200._embed`` (``n_ctx() / n_batch /
+    n_embd() / tokenize / detokenize / embed``) plus ``embed_token_ids``, a packed forward whose output stays on the
+    device, which ``embed_strings`` uses to pool without a host round trip.  Register it with
+    ``register_token_embedder(config.embedder, TokenEmbedderEngine.from_pretrained(local_dir))``."""
+
+    def __init__(self, state_dict: dict[str, torch.Tensor], *, n_layers: int, hidden: int, n_heads: int, ffn: int,
+                 max_pos: int, ln_eps: float = 1e-5, pos_offset: int = 0, tokenizer: Any | None = None, n_ctx: int = 512,
+                 device: Any | None = None, max_tokens_per_call: int = EMBED_TOKENS_PER_CALL) -> None:
+        super().__init__(state_dict, n_layers=n_layers, hidden=hidden, n_heads=n_heads, ffn=ffn, max_pos=max_pos,
+                         ln_eps=ln_eps, device=device, max_tokens_per_call=max_tokens_per_call, pos_offset=pos_offset)
+        n_ctx = min(int(n_ctx), max_pos - pos_offset, 512)
+        self.tok = EmbedderTokenizer(tokenizer, n_ctx) if tokenizer is not None else None
+        self._n_ctx = n_ctx
+        self.n_batch = n_ctx
+
+    # ---- constructors ------------------------------------------------------------------------------
+    @classmethod
+    def from_hf(cls, model: Any, tokenizer: Any | None = None, **kw: Any) -> "TokenEmbedderEngine":
+        """From a ``transformers`` ``XLMRobertaModel`` or ``BertModel`` (or a model that wraps one under
+        ``roberta.`` / ``bert.``) and its tokenizer."""
+        c = model.config
+        if getattr(c, "hidden_act", "gelu") != "gelu":
+            raise ValueError(f"hidden_act={c.hidden_act!r}: the encoder's FFN computes GELU(erf) only")
+        return cls(model.state_dict(), n_layers=c.num_hidden_layers, hidden=c.hidden_size, n_heads=c.num_attention_heads,
+                   ffn=c.intermediate_size, max_pos=c.max_position_embeddings, ln_eps=c.layer_norm_eps,
+                   pos_offset=_position_offset(c), tokenizer=tokenizer, **kw)
+
+    @classmethod
+    def from_pretrained(cls, path: Path | str, n_ctx: int = 512, **kw: Any) -> "TokenEmbedderEngine":
+        """Load HF weights + ``tokenizer.json`` from a local directory (e.g. ``BAAI/bge-m3``); no network access is
+        attempted."""
+        path = Path(path)
+        if not (path / "config.json").exists():
+            raise FileNotFoundError(f"No embedder weights at {path} (expected an HF model directory)")
+        from tokenizers import Tokenizer
+        from transformers import AutoModel
+
+        model = AutoModel.from_pretrained(path, local_files_only=True)
+        if not (path / "tokenizer.json").exists():
+            raise FileNotFoundError(f"No tokenizer.json in {path}")
+        return cls.from_hf(model, Tokenizer.from_file(str(path / "tokenizer.json")), n_ctx=n_ctx, **kw)
+
+    # ---- llama-like protocol -----------------------------------------------------------------------
+    def _tokenizer(self) -> EmbedderTokenizer:
+        if self.tok is None:
+            raise ValueError("this engine was built without a tokenizer; use embed_token_ids")
+        return self.tok
+
+    def n_ctx(self) -> int:
+        return self._n_ctx
+
+    def n_embd(self) -> int:
+        return self.hidden
+
+    def tokenize(self, text: bytes, add_bos: bool = False, special: bool = False) -> list[int]:
+        return self._tokenizer().tokenize(text, add_bos=add_bos, special=special)
+
+    def detokenize(self, tokens: Sequence[int]) -> bytes:
+        return self._tokenizer().detokenize(tokens)
+
+    def token_ids_for_embedding(self, texts: Sequence[str]) -> list[np.ndarray]:
+        return self._tokenizer().token_ids_for_embedding(texts)
+
+    def embed(self, text: str | Sequence[str]) -> np.ndarray | list[np.ndarray]:
+        """float32 ``[tokens, H]`` per text, special tokens included, truncated to ``n_batch`` tokens."""
+        texts = [text] if isinstance(text, str) else list(text)
+        X, offs = self.embed_token_ids(self.token_ids_for_embedding(texts))
+        host = X.cpu().numpy()
+        rows = [host[offs[i]:offs[i + 1]] for i in range(len(texts))]
+        return rows[0] if isinstance(text, str) else rows
+
+    # ---- device path -------------------------------------------------------------------------------
+    def embed_token_ids(self, ids: Sequence[np.ndarray]) -> tuple[torch.Tensor, np.ndarray]:
+        """One packed forward over token-id sequences (1 to ``n_ctx`` tokens each), in calls of at most
+        ``max_tokens_per_call`` tokens: float32 hidden states ``[T_total, H]`` on the device and the row offsets
+        ``[P + 1]`` of the sequences in it."""
+        P = len(ids)
+        lens = np.fromiter((len(x) for x in ids), dtype=np.int64, count=P)
+        if P and (lens.min() < 1 or lens.max() > self._n_ctx):
+            raise ValueError(f"every sequence needs 1 to {self._n_ctx} tokens")
+        offs = np.zeros(P + 1, dtype=np.int64)
+        np.cumsum(lens, out=offs[1:])
+        out = torch.empty((int(offs[-1]), self.hidden), dtype=torch.float32, device=self.device)
+
+        def launch(lo: int, hi: int, slot: int) -> torch.cuda.Event:
+            d_ids, d_types, d_pos, d_cu = self._upload_packed(ids[lo:hi], None, lens[lo:hi], slot=slot)
+            check(self.lib.rl_xenc_encode(C.byref(self.weights), d_ids.data_ptr(), d_types.data_ptr(), d_pos.data_ptr(),
+                                          d_cu.data_ptr(), hi - lo, len(d_ids), int(lens[lo:hi].max()),
+                                          out[int(offs[lo]):].data_ptr(), self._ws.data_ptr(), self._ws.numel(), _stream()),
+                  "rl_xenc_encode")
+            ev = torch.cuda.Event()
+            ev.record()
+            return ev
+
+        def collect(lo: int, hi: int, ev: torch.cuda.Event) -> None:   # noqa: ARG001  (the pinned half is free again)
+            ev.synchronize()
+
+        self._pipelined(lens, launch, collect)
+        return out, offs

@@ -223,6 +223,8 @@ __device__ __forceinline__ void cp_async_16(uint32_t dst_smem, const void* src, 
 
 
 // ---- embeddings + LayerNorm: one warp per token ----------------------------------------------------------
+// NC columns per lane: H <= 32 NC (16 for the cross-encoder's H <= 512, 32 for H <= 1024).
+template <int NC>
 __global__ void __launch_bounds__(256) embed_ln_kernel(const int32_t* __restrict__ ids, const int32_t* __restrict__ type_ids,
                                                        const int32_t* __restrict__ pos_ids, const __half* __restrict__ word,
                                                        const __half* __restrict__ pos, const __half* __restrict__ type,
@@ -236,10 +238,10 @@ __global__ void __launch_bounds__(256) embed_ln_kernel(const int32_t* __restrict
   const __half* w = word + (size_t)min(max(ids[tok], 0), vocab - 1) * H;
   const __half* p = pos + (size_t)min(max(pos_ids[tok], 0), max_pos - 1) * H;
   const __half* ty = type + (size_t)min(max(type_ids[tok], 0), type_vocab - 1) * H;
-  float x[16];  // H <= 512
+  float x[NC];  // H <= 32 NC
   float s = 0.f;
 #pragma unroll
-  for (int i = 0; i < 16; ++i) {
+  for (int i = 0; i < NC; ++i) {
     const int c = lane + 32 * i;
     x[i] = c < H ? __half2float(w[c]) + __half2float(p[c]) + __half2float(ty[c]) : 0.f;
     s += x[i];
@@ -247,35 +249,50 @@ __global__ void __launch_bounds__(256) embed_ln_kernel(const int32_t* __restrict
   const float mean = warp_sum_f(s) / (float)H;
   float var = 0.f;
 #pragma unroll
-  for (int i = 0; i < 16; ++i) {
+  for (int i = 0; i < NC; ++i) {
     const int c = lane + 32 * i;
     if (c < H) var += (x[i] - mean) * (x[i] - mean);
   }
   const float rstd = rsqrtf(warp_sum_f(var) / (float)H + eps);
 #pragma unroll
-  for (int i = 0; i < 16; ++i) {
+  for (int i = 0; i < NC; ++i) {
     const int c = lane + 32 * i;
     if (c < H) out[(size_t)tok * H + c] = __float2half_rn((x[i] - mean) * rstd * g[c] + bta[c]);
   }
 }
 
+// Four consecutive LayerNorm outputs: fp16 rows (8 bytes) inside the encoder, fp32 rows (16 bytes) for the last
+// layer of rl_xenc_encode.
+__device__ __forceinline__ void store4(__half* row, int piece, float a, float b, float c, float d) {
+  uint2 o;
+  o.x = pack_half2(a, b);
+  o.y = pack_half2(c, d);
+  reinterpret_cast<uint2*>(row)[piece] = o;
+}
+__device__ __forceinline__ void store4(float* row, int piece, float a, float b, float c, float d) {
+  reinterpret_cast<float4*>(row)[piece] = make_float4(a, b, c, d);
+}
+__device__ __forceinline__ void store1(__half* p, float a) { *p = __float2half_rn(a); }
+__device__ __forceinline__ void store1(float* p, float a) { *p = a; }
+
 // out = LayerNorm(x + res), one warp per token.  H % 128 == 0 (384 for MiniLM): a lane owns the columns
 // lane * 4 + 128 i, so every load / store instruction of the warp covers 256 contiguous bytes (8-byte pieces)
-// rather than 2 bytes per lane and instruction.
-template <bool VEC>
+// rather than 2 bytes per lane and instruction.  NC columns per lane: H <= 32 NC.  OutT: __half, or float for
+// the fp32 rows rl_xenc_encode returns.
+template <bool VEC, int NC = 16, typename OutT = __half>
 __global__ void __launch_bounds__(256) add_ln_kernel(const __half* __restrict__ xin, const __half* __restrict__ res,
                                                      const float* __restrict__ g, const float* __restrict__ bta, float eps,
-                                                     int T, int H, __half* __restrict__ out) {
+                                                     int T, int H, OutT* __restrict__ out) {
   const int lane = threadIdx.x & 31;
   const int tok = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (tok >= T) return;
-  float x[16];   // H <= 512
+  float x[NC];   // H <= 32 NC
   float s = 0.f;
   if (VEC) {
     const uint2* xi = reinterpret_cast<const uint2*>(xin + (size_t)tok * H);
     const uint2* ri = reinterpret_cast<const uint2*>(res + (size_t)tok * H);
 #pragma unroll
-    for (int i = 0; i < 4; ++i) {
+    for (int i = 0; i < NC / 4; ++i) {
       if (i * 128 < H) {
         const uint2 a = __ldg(xi + lane + 32 * i), r = __ldg(ri + lane + 32 * i);
         const float2 a0 = __half22float2(*reinterpret_cast<const __half2*>(&a.x)), a1 = __half22float2(*reinterpret_cast<const __half2*>(&a.y));
@@ -288,7 +305,7 @@ __global__ void __launch_bounds__(256) add_ln_kernel(const __half* __restrict__ 
     }
   } else {
 #pragma unroll
-    for (int i = 0; i < 16; ++i) {
+    for (int i = 0; i < NC; ++i) {
       const int c = lane + 32 * i;
       x[i] = c < H ? __half2float(xin[(size_t)tok * H + c]) + __half2float(res[(size_t)tok * H + c]) : 0.f;
       s += x[i];
@@ -297,29 +314,28 @@ __global__ void __launch_bounds__(256) add_ln_kernel(const __half* __restrict__ 
   const float mean = warp_sum_f(s) / (float)H;
   float var = 0.f;
 #pragma unroll
-  for (int i = 0; i < 16; ++i) {
+  for (int i = 0; i < NC; ++i) {
     const int c = VEC ? (i >> 2) * 128 : lane + 32 * i;   // (VEC: all four values of a piece are in or out together)
     if (c < H) var += (x[i] - mean) * (x[i] - mean);
   }
   const float rstd = rsqrtf(warp_sum_f(var) / (float)H + eps);
   if (VEC) {
-    uint2* oo = reinterpret_cast<uint2*>(out + (size_t)tok * H);
+    OutT* oo = out + (size_t)tok * H;
 #pragma unroll
-    for (int i = 0; i < 4; ++i) {
+    for (int i = 0; i < NC / 4; ++i) {
       if (i * 128 < H) {
         const float4 gg = __ldg(reinterpret_cast<const float4*>(g) + lane + 32 * i);
         const float4 bb = __ldg(reinterpret_cast<const float4*>(bta) + lane + 32 * i);
-        uint2 o;
-        o.x = pack_half2((x[4 * i] - mean) * rstd * gg.x + bb.x, (x[4 * i + 1] - mean) * rstd * gg.y + bb.y);
-        o.y = pack_half2((x[4 * i + 2] - mean) * rstd * gg.z + bb.z, (x[4 * i + 3] - mean) * rstd * gg.w + bb.w);
-        oo[lane + 32 * i] = o;
+        store4(oo, lane + 32 * i, (x[4 * i] - mean) * rstd * gg.x + bb.x,
+               (x[4 * i + 1] - mean) * rstd * gg.y + bb.y, (x[4 * i + 2] - mean) * rstd * gg.z + bb.z,
+               (x[4 * i + 3] - mean) * rstd * gg.w + bb.w);
       }
     }
   } else {
 #pragma unroll
-    for (int i = 0; i < 16; ++i) {
+    for (int i = 0; i < NC; ++i) {
       const int c = lane + 32 * i;
-      if (c < H) out[(size_t)tok * H + c] = __float2half_rn((x[i] - mean) * rstd * g[c] + bta[c]);
+      if (c < H) store1(out + (size_t)tok * H + c, (x[i] - mean) * rstd * g[c] + bta[c]);
     }
   }
 }
@@ -746,6 +762,153 @@ __global__ void __launch_bounds__(128, 3) attention2_kernel(const __half* __rest
   }
 }
 
+// ---- attention at head_dim 64 (the encoder of rl_xenc_encode) ----------------------------------------------
+// One CTA per (sequence, head, 64-query block); each of its four warps owns 16 queries.  K / V of the head stream through
+// shared memory in 64-key blocks, double-buffered with cp.async (zero-filled past the sequence), so a CTA holds 36 KB
+// whatever the length and several CTAs share an SM; the whole head of a 512-token sequence resident (the design of
+// attention2_kernel) would take about 147 KB at this width.  S = Q K^T and O += P V on m16n8k16 (fp16 in, fp32
+// accumulate), online softmax in the exp2 domain as in attention_kernel.  CTAs walk the sequences longest first
+// (seq_order_kernel), heads and then query blocks fastest.
+constexpr int kAtt64Dim = 64;
+constexpr int kAtt64Keys = 64;                 // keys per streamed block
+constexpr int kAtt64Queries = 64;              // queries per CTA
+constexpr int kAtt64Pitch = kAtt64Dim + 8;     // halves per staged row: 144 bytes, conflict-free ldmatrix
+constexpr int kAtt64Threads = 128;
+
+__global__ void __launch_bounds__(kAtt64Threads, 3) attention64_kernel(const __half* __restrict__ qkv, const int32_t* __restrict__ cu,
+                                                                       const int32_t* __restrict__ order, int H, int n_heads,
+                                                                       int n_qb, float scale_log2e, __half* __restrict__ ctx) {
+  __shared__ __align__(16) __half Ks[2][kAtt64Keys * kAtt64Pitch];
+  __shared__ __align__(16) __half Vs[2][kAtt64Keys * kAtt64Pitch];
+  const int qb = (int)(blockIdx.x % (unsigned)n_qb);
+  const int sh = (int)(blockIdx.x / (unsigned)n_qb);
+  const int head = sh % n_heads, seq = order[sh / n_heads];
+  const int t0 = cu[seq], L = cu[seq + 1] - t0;
+  if (qb * kAtt64Queries >= L) return;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const size_t ld = (size_t)3 * H;
+  const __half* kg = qkv + (size_t)t0 * ld + H + head * kAtt64Dim;   // key j of the head: kg + j * ld; its value: + H
+  auto load_kv = [&](int kb, int st) {   // keys [kb, kb + 64): 64 rows x 8 pieces of 16 bytes, for K and V
+#pragma unroll
+    for (int idx = threadIdx.x; idx < kAtt64Keys * 8; idx += kAtt64Threads) {
+      const int j = idx >> 3, c = idx & 7;
+      const bool ok = kb + j < L;
+      const __half* src = kg + (size_t)(ok ? kb + j : L - 1) * ld + c * 8;   // (clamped: a zero-fill copy reads nothing)
+      cp_async_16(smem_u32(&Ks[st][j * kAtt64Pitch + c * 8]), src, ok ? 16u : 0u);
+      cp_async_16(smem_u32(&Vs[st][j * kAtt64Pitch + c * 8]), src + H, ok ? 16u : 0u);
+    }
+    asm volatile("cp.async.commit_group;" ::: "memory");
+  };
+  load_kv(0, 0);
+  const int r = lane >> 2, cp = (lane & 3) * 2;
+  const int q0 = qb * kAtt64Queries + warp * 16 + r, q1 = q0 + 8;
+  const bool active = qb * kAtt64Queries + warp * 16 < L;   // warp-uniform: this warp has at least one query
+  // A fragments of S = Q K^T, four 16-wide k-steps over the head's 64 columns (rows >= L read as zero)
+  uint32_t a[4][4];
+#pragma unroll
+  for (int ks = 0; ks < 4; ++ks) {
+    const __half* p0 = qkv + (size_t)(t0 + q0) * ld + head * kAtt64Dim + ks * 16 + cp;
+    const __half* p1 = qkv + (size_t)(t0 + q1) * ld + head * kAtt64Dim + ks * 16 + cp;
+    a[ks][0] = q0 < L ? __ldg(reinterpret_cast<const uint32_t*>(p0)) : 0u;
+    a[ks][1] = q1 < L ? __ldg(reinterpret_cast<const uint32_t*>(p1)) : 0u;
+    a[ks][2] = q0 < L ? __ldg(reinterpret_cast<const uint32_t*>(p0 + 8)) : 0u;
+    a[ks][3] = q1 < L ? __ldg(reinterpret_cast<const uint32_t*>(p1 + 8)) : 0u;
+  }
+  float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
+  float O[8][4];
+#pragma unroll
+  for (int i = 0; i < 8; ++i)
+#pragma unroll
+    for (int e = 0; e < 4; ++e) O[i][e] = 0.f;
+  const int n_kb = (L + kAtt64Keys - 1) / kAtt64Keys;
+  for (int b = 0; b < n_kb; ++b) {
+    const int kb = b * kAtt64Keys, st = b & 1;
+    if (b + 1 < n_kb) {   // the next block travels while this one is computed
+      load_kv(kb + kAtt64Keys, st ^ 1);
+      asm volatile("cp.async.wait_group 1;" ::: "memory");
+    } else {
+      asm volatile("cp.async.wait_group 0;" ::: "memory");
+    }
+    __syncthreads();
+    if (active) {
+      const __half* Kb = Ks[st];
+      const __half* Vb = Vs[st];
+      float S[8][4];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+#pragma unroll
+        for (int e = 0; e < 4; ++e) S[j][e] = 0.f;
+#pragma unroll
+        for (int kp = 0; kp < 2; ++kp) {   // columns [32 kp, 32 kp + 32): k-steps 2 kp and 2 kp + 1
+          uint32_t bf[4];
+          ldsm_x4(bf, Kb + (j * 8 + (lane & 7)) * kAtt64Pitch + kp * 32 + (lane >> 3) * 8);
+          mma16816(S[j], a[2 * kp], bf[0], bf[1]);
+          mma16816(S[j], a[2 * kp + 1], bf[2], bf[3]);
+        }
+      }
+      if (kb + kAtt64Keys > L) {   // only the last key block holds padding keys
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+#pragma unroll
+          for (int e = 0; e < 4; ++e)
+            if (kb + j * 8 + cp + (e & 1) >= L) S[j][e] = -INFINITY;
+      }
+      float mx0 = -INFINITY, mx1 = -INFINITY;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        mx0 = fmaxf(mx0, fmaxf(S[j][0], S[j][1]));
+        mx1 = fmaxf(mx1, fmaxf(S[j][2], S[j][3]));
+      }
+      mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 1));
+      mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
+      mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1));
+      mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
+      // finite: every key block holds a valid key (scale > 0, so max commutes with the scaling)
+      const float mn0 = fmaxf(m0, mx0 * scale_log2e), mn1 = fmaxf(m1, mx1 * scale_log2e);
+      const float c0 = ex2_approx(m0 - mn0), c1 = ex2_approx(m1 - mn1);
+      l0 *= c0; l1 *= c1;
+#pragma unroll
+      for (int i = 0; i < 8; ++i) { O[i][0] *= c0; O[i][1] *= c0; O[i][2] *= c1; O[i][3] *= c1; }
+#pragma unroll
+      for (int j = 0; j < 8; ++j)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const float pexp = ex2_approx(fmaf(S[j][e], scale_log2e, e < 2 ? -mn0 : -mn1));   // -inf -> 0
+          S[j][e] = pexp;
+          if (e < 2) l0 += pexp; else l1 += pexp;
+        }
+      m0 = mn0; m1 = mn1;
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) {
+        uint32_t pa[4];
+        pa[0] = pack_half2(S[2 * kk][0], S[2 * kk][1]);
+        pa[1] = pack_half2(S[2 * kk][2], S[2 * kk][3]);
+        pa[2] = pack_half2(S[2 * kk + 1][0], S[2 * kk + 1][1]);
+        pa[3] = pack_half2(S[2 * kk + 1][2], S[2 * kk + 1][3]);
+#pragma unroll
+        for (int dn2 = 0; dn2 < 4; ++dn2) {
+          uint32_t vb[4];
+          ldsm_x4_trans(vb, Vb + (kk * 16 + (lane & 7) + ((lane >> 3) & 1) * 8) * kAtt64Pitch + (dn2 * 2 + (lane >> 4)) * 8);
+          mma16816(O[dn2 * 2], pa, vb[0], vb[1]);
+          mma16816(O[dn2 * 2 + 1], pa, vb[2], vb[3]);
+        }
+      }
+    }
+    __syncthreads();   // stage st is refilled by the next iteration's load
+  }
+  if (!active) return;
+  l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
+  l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
+  l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
+  l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+  const float inv0 = 1.f / l0, inv1 = 1.f / l1;
+#pragma unroll
+  for (int dn = 0; dn < 8; ++dn) {
+    if (q0 < L) *reinterpret_cast<uint32_t*>(ctx + (size_t)(t0 + q0) * H + head * kAtt64Dim + dn * 8 + cp) = pack_half2(O[dn][0] * inv0, O[dn][1] * inv0);
+    if (q1 < L) *reinterpret_cast<uint32_t*>(ctx + (size_t)(t0 + q1) * H + head * kAtt64Dim + dn * 8 + cp) = pack_half2(O[dn][2] * inv1, O[dn][3] * inv1);
+  }
+}
+
 // ---- pooler + classifier ----------------------------------------------------------------------------------
 // logit[s] = Wc . tanh(Wp h_s + bp) + bc with h_s the [CLS] row of sequence s.  A CTA owns kClsSeqs sequences
 // (their [CLS] rows sit in shared memory as fp32) and its H/32 warps share the H pooler outputs; for one output
@@ -982,6 +1145,103 @@ extern "C" size_t rl_xenc_workspace_bytes(const rl_xenc_weights* w, int T) {
   return ((size_t)T * (H + 3 * H + H + H + F) * sizeof(__half) + (size_t)T * sizeof(int32_t) + 4096);
 }
 
+// ---- attention at head_dim 64: setup and launches, shared by rl_xenc_encode and the rl_xenc_encode_attention hook ----
+static int attention64_setup(const int32_t* cu_seqlens, int P, int32_t* seq_order, cudaStream_t stream) {
+  seq_order_kernel<<<1, 1024, 0, stream>>>(cu_seqlens, P, seq_order);
+  RL_CUDA_CHECK(cudaGetLastError());
+  return RL_OK;
+}
+
+static int attention64_launch(const __half* qkv, const int32_t* cu_seqlens, const int32_t* seq_order, int P, int max_len,
+                              int H, int nh, __half* ctx, cudaStream_t stream) {
+  const int n_qb = (max_len + kAtt64Queries - 1) / kAtt64Queries;
+  const float scale = 1.4426950408889634f / sqrtf((float)kAtt64Dim);  // softmax in the exp2 domain
+  attention64_kernel<<<dim3((unsigned)P * (unsigned)nh * (unsigned)n_qb), kAtt64Threads, 0, stream>>>(
+      qkv, cu_seqlens, seq_order, H, nh, n_qb, scale, ctx);
+  RL_CUDA_CHECK(cudaGetLastError());
+  return RL_OK;
+}
+
+// The attention step of an encoder forward by head_dim: 32 takes the cross-encoder's kernels (and their RL_XENC_ATT*
+// selection), 64 attention64_kernel.
+static int encoder_attention_setup(int head_dim, const int32_t* cu_seqlens, int P, int max_len, int32_t* seq_order,
+                                   cudaStream_t stream) {
+  return head_dim == 64 ? attention64_setup(cu_seqlens, P, seq_order, stream)
+                        : attention_setup(cu_seqlens, P, max_len, seq_order, stream);
+}
+static int encoder_attention_launch(int head_dim, const __half* qkv, const int32_t* cu_seqlens, const int32_t* seq_order, int P,
+                                    int max_len, int H, int nh, __half* ctx, cudaStream_t stream) {
+  return head_dim == 64 ? attention64_launch(qkv, cu_seqlens, seq_order, P, max_len, H, nh, ctx, stream)
+                        : attention_launch(qkv, cu_seqlens, seq_order, P, max_len, H, nh, ctx, stream);
+}
+
+// LayerNorm launches by width: 16 columns per lane up to H = 512 (the cross-encoder's instantiations), 32 up to 1024.
+static void launch_embed_ln(const rl_xenc_weights* w, const int32_t* ids, const int32_t* type_ids, const int32_t* pos_ids, int T,
+                            __half* out, cudaStream_t stream) {
+  const int H = w->hidden, blocks = (T + 7) / 8;
+  const __half* word = reinterpret_cast<const __half*>(w->word_emb);
+  const __half* pos = reinterpret_cast<const __half*>(w->pos_emb);
+  const __half* type = reinterpret_cast<const __half*>(w->type_emb);
+  if (H <= 512)
+    embed_ln_kernel<16><<<blocks, 256, 0, stream>>>(ids, type_ids, pos_ids, word, pos, type, w->emb_ln_g, w->emb_ln_b, w->ln_eps,
+                                                    T, H, w->vocab, w->max_pos, w->type_vocab, out);
+  else
+    embed_ln_kernel<32><<<blocks, 256, 0, stream>>>(ids, type_ids, pos_ids, word, pos, type, w->emb_ln_g, w->emb_ln_b, w->ln_eps,
+                                                    T, H, w->vocab, w->max_pos, w->type_vocab, out);
+}
+template <typename OutT>
+static void launch_add_ln(const __half* x, const __half* res, const float* g, const float* b, float eps, int T, int H, OutT* out,
+                          cudaStream_t stream) {
+  const int blocks = (T + 7) / 8;
+  const bool vec = H % 128 == 0;   // (LayerNorm gamma / beta come from torch allocations: 16-byte aligned)
+  if (H <= 512) {
+    if (vec) add_ln_kernel<true, 16, OutT><<<blocks, 256, 0, stream>>>(x, res, g, b, eps, T, H, out);
+    else add_ln_kernel<false, 16, OutT><<<blocks, 256, 0, stream>>>(x, res, g, b, eps, T, H, out);
+  } else {
+    if (vec) add_ln_kernel<true, 32, OutT><<<blocks, 256, 0, stream>>>(x, res, g, b, eps, T, H, out);
+    else add_ln_kernel<false, 32, OutT><<<blocks, 256, 0, stream>>>(x, res, g, b, eps, T, H, out);
+  }
+}
+
+// Embeddings and every encoder layer of a packed batch, shared by rl_xenc_score and rl_xenc_encode (arguments checked by
+// the caller).  The last layer's output LayerNorm writes fp16 rows into the workspace's hidden buffer or, when out_f32 is
+// set, fp32 rows to out_f32 [T, H].
+static int encoder_forward(const rl_xenc_weights* w, const int32_t* input_ids, const int32_t* type_ids, const int32_t* pos_ids,
+                           const int32_t* cu_seqlens, int P, int T, int max_len, void* workspace, float* out_f32, int sms,
+                           cudaStream_t stream) {
+  const int H = w->hidden, F = w->ffn, nh = w->n_heads, head_dim = H / nh;
+  __half* hidden = reinterpret_cast<__half*>(workspace);
+  __half* qkv = hidden + (size_t)T * H;
+  __half* ctx = qkv + (size_t)T * 3 * H;
+  __half* tmp = ctx + (size_t)T * H;
+  __half* ffn = tmp + (size_t)T * H;
+  int32_t* seq_order = reinterpret_cast<int32_t*>(
+      (reinterpret_cast<uintptr_t>(ffn + (size_t)T * F) + 15) & ~uintptr_t(15));   // [P] (P <= T)
+  int rc = encoder_attention_setup(head_dim, cu_seqlens, P, max_len, seq_order, stream);
+  if (rc != RL_OK) return rc;
+  launch_embed_ln(w, input_ids, type_ids, pos_ids, T, hidden, stream);
+  RL_CUDA_CHECK(cudaGetLastError());
+  for (int l = 0; l < w->n_layers; ++l) {
+    const rl_xenc_layer& L = w->layers[l];
+    rc = launch_linear(hidden, L.qkv_img, L.qkv_bias, qkv, T, 3 * H, H, 0, sms, stream);
+    if (rc != RL_OK) return rc;
+    rc = encoder_attention_launch(head_dim, qkv, cu_seqlens, seq_order, P, max_len, H, nh, ctx, stream);
+    if (rc != RL_OK) return rc;
+    rc = launch_linear(ctx, L.o_img, L.o_bias, tmp, T, H, H, 0, sms, stream);
+    if (rc != RL_OK) return rc;
+    launch_add_ln(tmp, hidden, L.ln1_g, L.ln1_b, w->ln_eps, T, H, hidden, stream);
+    RL_CUDA_CHECK(cudaGetLastError());
+    rc = launch_linear(hidden, L.up_img, L.up_bias, ffn, T, F, H, 1, sms, stream);
+    if (rc != RL_OK) return rc;
+    rc = launch_linear(ffn, L.down_img, L.down_bias, tmp, T, H, F, 0, sms, stream);
+    if (rc != RL_OK) return rc;
+    if (out_f32 != nullptr && l == w->n_layers - 1) launch_add_ln(tmp, hidden, L.ln2_g, L.ln2_b, w->ln_eps, T, H, out_f32, stream);
+    else launch_add_ln(tmp, hidden, L.ln2_g, L.ln2_b, w->ln_eps, T, H, hidden, stream);
+    RL_CUDA_CHECK(cudaGetLastError());
+  }
+  return RL_OK;
+}
+
 extern "C" int rl_xenc_score(const rl_xenc_weights* w, const int32_t* input_ids, const int32_t* type_ids,
                              const int32_t* pos_ids, const int32_t* cu_seqlens, int P, int T, int max_len,
                              float* out_logit, float* out_score, void* workspace, size_t workspace_bytes, void* stream_) {
@@ -997,45 +1257,60 @@ extern "C" int rl_xenc_score(const rl_xenc_weights* w, const int32_t* input_ids,
   int dev = 0, sms = 132;
   RL_CUDA_CHECK(cudaGetDevice(&dev));
   RL_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  __half* hidden = reinterpret_cast<__half*>(workspace);
-  __half* qkv = hidden + (size_t)T * H;
-  __half* ctx = qkv + (size_t)T * 3 * H;
-  __half* tmp = ctx + (size_t)T * H;
-  __half* ffn = tmp + (size_t)T * H;
-  int32_t* seq_order = reinterpret_cast<int32_t*>(
-      (reinterpret_cast<uintptr_t>(ffn + (size_t)T * F) + 15) & ~uintptr_t(15));   // [P] (P <= T)
   RL_REQUIRE(P <= T, RL_EINVAL, "rl_xenc_score: more sequences than tokens");
-  int rc = attention_setup(cu_seqlens, P, max_len, seq_order, stream);
+  const int rc = encoder_forward(w, input_ids, type_ids, pos_ids, cu_seqlens, P, T, max_len, workspace, nullptr, sms, stream);
   if (rc != RL_OK) return rc;
-  const int tok_blocks = (T + 7) / 8;
-  const bool ln_vec = H % 128 == 0;   // (LayerNorm gamma / beta come from torch allocations: 16-byte aligned)
-  embed_ln_kernel<<<tok_blocks, 256, 0, stream>>>(input_ids, type_ids, pos_ids, reinterpret_cast<const __half*>(w->word_emb),
-                                                  reinterpret_cast<const __half*>(w->pos_emb),
-                                                  reinterpret_cast<const __half*>(w->type_emb), w->emb_ln_g, w->emb_ln_b,
-                                                  w->ln_eps, T, H, w->vocab, w->max_pos, w->type_vocab, hidden);
-  RL_CUDA_CHECK(cudaGetLastError());
-  for (int l = 0; l < w->n_layers; ++l) {
-    const rl_xenc_layer& L = w->layers[l];
-    rc = launch_linear(hidden, L.qkv_img, L.qkv_bias, qkv, T, 3 * H, H, 0, sms, stream);
-    if (rc != RL_OK) return rc;
-    rc = attention_launch(qkv, cu_seqlens, seq_order, P, max_len, H, nh, ctx, stream);
-    if (rc != RL_OK) return rc;
-    rc = launch_linear(ctx, L.o_img, L.o_bias, tmp, T, H, H, 0, sms, stream);
-    if (rc != RL_OK) return rc;
-    if (ln_vec) add_ln_kernel<true><<<tok_blocks, 256, 0, stream>>>(tmp, hidden, L.ln1_g, L.ln1_b, w->ln_eps, T, H, hidden);
-    else add_ln_kernel<false><<<tok_blocks, 256, 0, stream>>>(tmp, hidden, L.ln1_g, L.ln1_b, w->ln_eps, T, H, hidden);
-    RL_CUDA_CHECK(cudaGetLastError());
-    rc = launch_linear(hidden, L.up_img, L.up_bias, ffn, T, F, H, 1, sms, stream);
-    if (rc != RL_OK) return rc;
-    rc = launch_linear(ffn, L.down_img, L.down_bias, tmp, T, H, F, 0, sms, stream);
-    if (rc != RL_OK) return rc;
-    if (ln_vec) add_ln_kernel<true><<<tok_blocks, 256, 0, stream>>>(tmp, hidden, L.ln2_g, L.ln2_b, w->ln_eps, T, H, hidden);
-    else add_ln_kernel<false><<<tok_blocks, 256, 0, stream>>>(tmp, hidden, L.ln2_g, L.ln2_b, w->ln_eps, T, H, hidden);
-    RL_CUDA_CHECK(cudaGetLastError());
-  }
   const int cls_warps = H / 32 < kClsMaxWarps ? H / 32 : kClsMaxWarps;
   cls_head_kernel<<<(P + kClsSeqs - 1) / kClsSeqs, cls_warps * 32, ((size_t)kClsSeqs * H + kClsMaxWarps * kClsSeqs) * sizeof(float), stream>>>(
-      hidden, cu_seqlens, w->pooler_w, w->pooler_b, w->cls_w, w->cls_b, P, H, out_logit, out_score);
+      reinterpret_cast<const __half*>(workspace), cu_seqlens, w->pooler_w, w->pooler_b, w->cls_w, w->cls_b, P, H, out_logit, out_score);
   RL_CUDA_CHECK(cudaGetLastError());
   return RL_OK;
+}
+
+// Shapes the encoder path takes: head_dim 32 or 64, H <= 1024 (LayerNorm at 32 columns per lane), up to 512 tokens.
+constexpr int kEncodeMaxHidden = 1024;
+constexpr int kEncodeMaxLen = 512;
+
+extern "C" int rl_xenc_encode(const rl_xenc_weights* w, const int32_t* input_ids, const int32_t* type_ids,
+                              const int32_t* pos_ids, const int32_t* cu_seqlens, int P, int T, int max_len, float* out_hidden,
+                              void* workspace, size_t workspace_bytes, void* stream_) {
+  RL_REQUIRE(w && w->layers && input_ids && type_ids && pos_ids && cu_seqlens && out_hidden, RL_EINVAL,
+             "rl_xenc_encode: null pointer");
+  if (P == 0 || T == 0) return RL_OK;
+  const int H = w->hidden, F = w->ffn, nh = w->n_heads;
+  RL_REQUIRE(H % 32 == 0 && H <= kEncodeMaxHidden && nh > 0 && H % nh == 0 && (H / nh == 32 || H / nh == 64), RL_EUNSUPPORTED,
+             "rl_xenc_encode: hidden=%d heads=%d unsupported (head_dim 32 or 64, hidden %% 32 == 0, hidden <= %d)", H, nh,
+             kEncodeMaxHidden);
+  RL_REQUIRE(F % 32 == 0 && w->n_layers > 0, RL_EUNSUPPORTED, "rl_xenc_encode: ffn %% 32 and n_layers > 0 required");
+  RL_REQUIRE(max_len > 0 && max_len <= kEncodeMaxLen && max_len <= w->max_pos, RL_EUNSUPPORTED,
+             "rl_xenc_encode: max_len=%d unsupported (at most min(%d, max_pos=%d))", max_len, kEncodeMaxLen, w->max_pos);
+  RL_REQUIRE(P <= T, RL_EINVAL, "rl_xenc_encode: more sequences (%d) than tokens (%d)", P, T);
+  RL_REQUIRE(workspace && (reinterpret_cast<uintptr_t>(workspace) & 15) == 0 && workspace_bytes >= rl_xenc_workspace_bytes(w, T),
+             RL_ENOSPACE, "rl_xenc_encode: workspace must be 16-byte aligned and hold rl_xenc_workspace_bytes(w, T) bytes");
+  int dev = 0, sms = 132;
+  RL_CUDA_CHECK(cudaGetDevice(&dev));
+  RL_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  return encoder_forward(w, input_ids, type_ids, pos_ids, cu_seqlens, P, T, max_len, workspace, out_hidden, sms,
+                         (cudaStream_t)stream_);
+}
+
+extern "C" int rl_xenc_encode_attention(const void* qkv, const int32_t* cu_seqlens, int P, int T, int max_len, int hidden,
+                                        int n_heads, void* ctx, void* workspace, size_t workspace_bytes, void* stream_) {
+  RL_REQUIRE(qkv && cu_seqlens && ctx, RL_EINVAL, "rl_xenc_encode_attention: null pointer");
+  if (P == 0 || T == 0) return RL_OK;
+  RL_REQUIRE(hidden % 32 == 0 && hidden <= kEncodeMaxHidden && n_heads > 0 && hidden % n_heads == 0 &&
+                 (hidden / n_heads == 32 || hidden / n_heads == 64),
+             RL_EUNSUPPORTED, "rl_xenc_encode_attention: hidden=%d heads=%d unsupported (head_dim 32 or 64, hidden <= %d)",
+             hidden, n_heads, kEncodeMaxHidden);
+  RL_REQUIRE(P > 0 && P <= T && max_len > 0, RL_EINVAL, "rl_xenc_encode_attention: bad P=%d / T=%d / max_len=%d", P, T, max_len);
+  RL_REQUIRE(max_len <= kEncodeMaxLen, RL_EUNSUPPORTED, "rl_xenc_encode_attention: max_len=%d > %d", max_len, kEncodeMaxLen);
+  RL_REQUIRE(workspace && (reinterpret_cast<uintptr_t>(workspace) & 15) == 0 && workspace_bytes >= (size_t)P * sizeof(int32_t),
+             RL_ENOSPACE, "rl_xenc_encode_attention: workspace must be 16-byte aligned and hold %d int32", P);
+  cudaStream_t stream = (cudaStream_t)stream_;
+  const int head_dim = hidden / n_heads;
+  int32_t* seq_order = reinterpret_cast<int32_t*>(workspace);
+  const int rc = encoder_attention_setup(head_dim, cu_seqlens, P, max_len, seq_order, stream);
+  if (rc != RL_OK) return rc;
+  return encoder_attention_launch(head_dim, reinterpret_cast<const __half*>(qkv), cu_seqlens, seq_order, P, max_len, hidden,
+                                  n_heads, reinterpret_cast<__half*>(ctx), stream);
 }
