@@ -315,8 +315,8 @@ int rl_xenc_score(const rl_xenc_weights* w, const int32_t* input_ids, const int3
                   const int32_t* cu_seqlens, int P, int T, int max_len, float* out_logit, float* out_score,
                   void* workspace, size_t workspace_bytes, void* stream);
 /* Debug/test hook: the attention step of rl_xenc_score on its own.  qkv [T, 3*hidden] fp16 (Q | K | V), ctx [T, hidden]
- * fp16, cu_seqlens [P+1] (device), max_len = longest sequence; head_dim 32.  Uses the RL_XENC_ATT* selection of
- * rl_xenc_score.  workspace: >= 4*P bytes (the length-sorted order), 16-byte aligned. */
+ * fp16, cu_seqlens [P+1] (device), max_len = longest sequence; head_dim 32.  workspace: >= 4*P bytes (the
+ * length-sorted order), 16-byte aligned. */
 int rl_xenc_attention(const void* qkv, const int32_t* cu_seqlens, int P, int T, int max_len, int hidden, int n_heads,
                       void* ctx, void* workspace, size_t workspace_bytes, void* stream);
 /* Token encoder (BERT / XLM-RoBERTa, e.g. bge-m3): the embeddings and layers of rl_xenc_score without its head.

@@ -7,15 +7,14 @@
 //                        sliced by 64), X through a TMA tensor map into 128B-swizzled smem, W as a
 //                        pre-swizzled fp16 image fetched with cp.async.bulk, fp32 accumulate in
 //                        registers, bias / GELU(erf) fused in the epilogue
-//   attention_kernel     softmax(Q K^T / sqrt(dh)) V per (sequence, head), fp32 math
+//   attention2_kernel    softmax(Q K^T / sqrt(dh)) V per (sequence, head) at head_dim 32, fp32 math
+//                        (attention64_kernel: head_dim 64, the token encoder of rl_xenc_encode)
 //   add_ln_kernel        LayerNorm(x + residual)
 //   cls_head_kernel      pooler (dense + tanh on [CLS]) -> classifier -> logit, sigmoid score
 #include <cuda.h>
 #include <cuda_fp16.h>
 
 #include <type_traits>
-
-#include <mutex>
 
 #include "common.cuh"
 #include "hopper_ptx.cuh"
@@ -342,9 +341,10 @@ __global__ void __launch_bounds__(256) add_ln_kernel(const __half* __restrict__ 
 
 // ---- attention: one block per (sequence, head), flash-style on mma.sync tensor cores ---------------------
 // qkv [T, 3H] (Q | K | V), ctx [T, H].  head_dim must be 32 (MiniLM-L12-H384: 12 heads x 32).
-// K and V of the head sit in shared memory (80-byte row pitch: conflict-free ldmatrix); each warp
-// owns 16-query blocks: S = Q K^T with m16n8k16 (fp16 in, fp32 acc), online softmax in the exp2
-// domain, O += P V with P re-packed from the S accumulators as the A operand.
+// K and V of the head sit in shared memory (80-byte row pitch: conflict-free ldmatrix): S = Q K^T with
+// m16n8k16 (fp16 in, fp32 acc), online softmax in the exp2 domain, O += P V with P re-packed from the S
+// accumulators as the A operand.  The running maxima are kept scaled (m = max(S) * scale); the scale itself
+// is folded into the exponent's FMA, so a score costs one FMNMX, one FFMA, one ex2 and one FADD.
 constexpr int kAttPitch = 40;  // halves
 
 __device__ __forceinline__ void mma16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
@@ -368,192 +368,6 @@ __device__ __forceinline__ float ex2_approx(float x) {   // 2^x, one MUFU op; ex
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
-}
-
-// 4 x 4 transpose of 32-bit words across the four lanes of a quad: afterwards w[l] on lane c holds what
-// w[c] was on lane l.  Turns "16 contiguous bytes of a row per lane" (one 64-byte request per row) into
-// the m16n8k16 fragment layout (4-byte pieces at stride 16 bytes) and back.
-__device__ __forceinline__ void quad_transpose(uint32_t (&w)[4], int c) {
-#pragma unroll
-  for (int s = 1; s < 4; ++s) {   // selects only: a branch here would make the shuffle divergent
-    const int p = c ^ s;
-    const uint32_t lo = (p & 1) ? w[1] : w[0], hi = (p & 1) ? w[3] : w[2];
-    const uint32_t got = __shfl_xor_sync(0xffffffffu, (p & 2) ? hi : lo, s);
-    w[0] = p == 0 ? got : w[0];
-    w[1] = p == 1 ? got : w[1];
-    w[2] = p == 2 ? got : w[2];
-    w[3] = p == 3 ? got : w[3];
-  }
-}
-
-template <bool QUAD>   // QUAD: 16-byte Q loads / context stores through a quad transpose; else (default) 4-byte fragment pieces
-__global__ void __launch_bounds__(128, 5) attention_kernel(const __half* __restrict__ qkv, const int32_t* __restrict__ cu,
-                                                        int H, int n_heads, float scale_log2e, __half* __restrict__ ctx,
-                                                        int len_lo, int len_hi) {
-  extern __shared__ __align__(16) unsigned char att_smem[];
-  const int seq = blockIdx.x, head = blockIdx.y;
-  const int t0 = cu[seq], L = cu[seq + 1] - t0;
-  // Length buckets: the launch's shared memory is sized for len_hi keys, so a launch for the short sequences
-  // keeps five CTAs per SM resident (41 KB each at 256 keys) instead of the three a 512-key allocation allows.
-  if (L <= len_lo || L > len_hi) return;
-  const int Lp = (L + 63) / 64 * 64;
-  __half* Ks = reinterpret_cast<__half*>(att_smem);
-  __half* Vs = Ks + (size_t)Lp * kAttPitch;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const size_t ld = (size_t)3 * H;
-#pragma unroll 4
-  for (int idx = threadIdx.x; idx < Lp * 4; idx += blockDim.x) {
-    const int j = idx >> 2, c = idx & 3;
-    uint4 kv = make_uint4(0u, 0u, 0u, 0u), vv = kv;
-    if (j < L) {
-      const __half* base = qkv + (size_t)(t0 + j) * ld + head * 32 + c * 8;
-      kv = __ldg(reinterpret_cast<const uint4*>(base + H));
-      vv = __ldg(reinterpret_cast<const uint4*>(base + 2 * H));
-    }
-    *reinterpret_cast<uint4*>(Ks + (size_t)j * kAttPitch + c * 8) = kv;
-    *reinterpret_cast<uint4*>(Vs + (size_t)j * kAttPitch + c * 8) = vv;
-  }
-  __syncthreads();
-  const int r = lane >> 2, cp = (lane & 3) * 2;
-  // Q fragments (A operand of S = Q K^T) of a 16-query block; the next block's are fetched while this
-  // one is computed.
-  const int qc = lane & 3;
-  auto load_q = [&](int qb, uint32_t (&a)[2][4]) {   // raw 16-byte row chunks; finish_q turns them into fragments
-    const int q0 = qb * 16 + r, q1 = q0 + 8;
-    if (!QUAD) {
-#pragma unroll
-      for (int ks = 0; ks < 2; ++ks) {
-        const __half* p0 = qkv + (size_t)(t0 + q0) * ld + head * 32 + ks * 16 + cp;
-        const __half* p1 = qkv + (size_t)(t0 + q1) * ld + head * 32 + ks * 16 + cp;
-        a[ks][0] = q0 < L ? __ldg(reinterpret_cast<const uint32_t*>(p0)) : 0u;
-        a[ks][1] = q1 < L ? __ldg(reinterpret_cast<const uint32_t*>(p1)) : 0u;
-        a[ks][2] = q0 < L ? __ldg(reinterpret_cast<const uint32_t*>(p0 + 8)) : 0u;
-        a[ks][3] = q1 < L ? __ldg(reinterpret_cast<const uint32_t*>(p1 + 8)) : 0u;
-      }
-      return;
-    }
-    const uint4 z = make_uint4(0u, 0u, 0u, 0u);
-    const uint4 u0 = q0 < L ? __ldg(reinterpret_cast<const uint4*>(qkv + (size_t)(t0 + q0) * ld + head * 32 + qc * 8)) : z;
-    const uint4 u1 = q1 < L ? __ldg(reinterpret_cast<const uint4*>(qkv + (size_t)(t0 + q1) * ld + head * 32 + qc * 8)) : z;
-    a[0][0] = u0.x; a[0][1] = u0.y; a[0][2] = u0.z; a[0][3] = u0.w;
-    a[1][0] = u1.x; a[1][1] = u1.y; a[1][2] = u1.z; a[1][3] = u1.w;
-  };
-  auto finish_q = [&](const uint32_t (&raw)[2][4], uint32_t (&a)[2][4]) {
-    if (!QUAD) {
-#pragma unroll
-      for (int ks = 0; ks < 2; ++ks)
-#pragma unroll
-        for (int e = 0; e < 4; ++e) a[ks][e] = raw[ks][e];
-      return;
-    }
-    uint32_t w0[4] = {raw[0][0], raw[0][1], raw[0][2], raw[0][3]};
-    uint32_t w1[4] = {raw[1][0], raw[1][1], raw[1][2], raw[1][3]};
-    quad_transpose(w0, qc);   // w0[l] = row q0, columns l*8 + cp, +1
-    quad_transpose(w1, qc);
-    a[0][0] = w0[0]; a[0][2] = w0[1]; a[1][0] = w0[2]; a[1][2] = w0[3];
-    a[0][1] = w1[0]; a[0][3] = w1[1]; a[1][1] = w1[2]; a[1][3] = w1[3];
-  };
-  uint32_t a[2][4], a_next[2][4];
-  load_q(warp, a_next);   // rows >= L read as zero, so a block past the end is harmless
-  for (int qb = warp; qb * 16 < L; qb += 4) {
-    const int q0 = qb * 16 + r, q1 = q0 + 8;
-    finish_q(a_next, a);
-    load_q(qb + 4, a_next);
-    float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
-    float O[4][4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-#pragma unroll
-      for (int e = 0; e < 4; ++e) O[i][e] = 0.f;
-    for (int kb = 0; kb < Lp; kb += 64) {
-      float S[8][4];
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-#pragma unroll
-        for (int e = 0; e < 4; ++e) S[j][e] = 0.f;
-        uint32_t b[4];
-        ldsm_x4(b, Ks + (size_t)(kb + j * 8 + (lane & 7)) * kAttPitch + (lane >> 3) * 8);
-        mma16816(S[j], a[0], b[0], b[1]);
-        mma16816(S[j], a[1], b[2], b[3]);
-      }
-      // Online softmax in the exp2 domain.  The running maxima are kept scaled (m = max(S) * scale);
-      // the scale itself is folded into the exponent's FMA, so a score costs one FMNMX, one FFMA, one
-      // ex2 and one FADD.  Only the last key block holds padding keys.
-      float mx0 = -INFINITY, mx1 = -INFINITY;
-      if (kb + 64 > L) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j)
-#pragma unroll
-          for (int e = 0; e < 4; ++e)
-            if (kb + j * 8 + cp + (e & 1) >= L) S[j][e] = -INFINITY;
-      }
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        mx0 = fmaxf(mx0, fmaxf(S[j][0], S[j][1]));
-        mx1 = fmaxf(mx1, fmaxf(S[j][2], S[j][3]));
-      }
-      mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 1));
-      mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
-      mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1));
-      mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
-      // finite: every key block holds a valid key (scale > 0, so max commutes with the scaling)
-      const float mn0 = fmaxf(m0, mx0 * scale_log2e), mn1 = fmaxf(m1, mx1 * scale_log2e);
-      const float c0 = ex2_approx(m0 - mn0), c1 = ex2_approx(m1 - mn1);
-      l0 *= c0; l1 *= c1;
-#pragma unroll
-      for (int i = 0; i < 4; ++i) { O[i][0] *= c0; O[i][1] *= c0; O[i][2] *= c1; O[i][3] *= c1; }
-#pragma unroll
-      for (int j = 0; j < 8; ++j)
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const float pexp = ex2_approx(fmaf(S[j][e], scale_log2e, e < 2 ? -mn0 : -mn1));   // -inf -> 0
-          S[j][e] = pexp;
-          if (e < 2) l0 += pexp; else l1 += pexp;
-        }
-      m0 = mn0; m1 = mn1;
-#pragma unroll
-      for (int kk = 0; kk < 4; ++kk) {
-        uint32_t pa[4];
-        pa[0] = pack_half2(S[2 * kk][0], S[2 * kk][1]);
-        pa[1] = pack_half2(S[2 * kk][2], S[2 * kk][3]);
-        pa[2] = pack_half2(S[2 * kk + 1][0], S[2 * kk + 1][1]);
-        pa[3] = pack_half2(S[2 * kk + 1][2], S[2 * kk + 1][3]);
-#pragma unroll
-        for (int dn2 = 0; dn2 < 2; ++dn2) {
-          uint32_t vb[4];
-          ldsm_x4_trans(vb, Vs + (size_t)(kb + kk * 16 + (lane & 7) + ((lane >> 3) & 1) * 8) * kAttPitch +
-                                (dn2 * 2 + (lane >> 4)) * 8);
-          mma16816(O[dn2 * 2], pa, vb[0], vb[1]);
-          mma16816(O[dn2 * 2 + 1], pa, vb[2], vb[3]);
-        }
-      }
-    }
-    l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
-    l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
-    l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
-    l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
-    const float inv0 = 1.f / l0, inv1 = 1.f / l1;
-    uint32_t o0[4], o1[4];
-#pragma unroll
-    for (int dn = 0; dn < 4; ++dn) {
-      o0[dn] = pack_half2(O[dn][0] * inv0, O[dn][1] * inv0);
-      o1[dn] = pack_half2(O[dn][2] * inv1, O[dn][3] * inv1);
-    }
-    if (!QUAD) {
-#pragma unroll
-      for (int dn = 0; dn < 4; ++dn) {
-        if (q0 < L) *reinterpret_cast<uint32_t*>(ctx + (size_t)(t0 + q0) * H + head * 32 + dn * 8 + cp) = o0[dn];
-        if (q1 < L) *reinterpret_cast<uint32_t*>(ctx + (size_t)(t0 + q1) * H + head * 32 + dn * 8 + cp) = o1[dn];
-      }
-      continue;
-    }
-    quad_transpose(o0, qc);   // lane qc now holds columns qc*8 .. qc*8+7 of its rows: one 16-byte store each
-    quad_transpose(o1, qc);
-    if (q0 < L)
-      *reinterpret_cast<uint4*>(ctx + (size_t)(t0 + q0) * H + head * 32 + qc * 8) = make_uint4(o0[0], o0[1], o0[2], o0[3]);
-    if (q1 < L)
-      *reinterpret_cast<uint4*>(ctx + (size_t)(t0 + q1) * H + head * 32 + qc * 8) = make_uint4(o1[0], o1[1], o1[2], o1[3]);
-  }
 }
 
 // Sequence indices of a call sorted by length, longest first (counting sort over the lengths; equal lengths in any
@@ -583,45 +397,28 @@ __global__ void __launch_bounds__(1024) seq_order_kernel(const int32_t* __restri
 // the last wave holds the shortest sequences.  The last key block is 32 keys wide when no more than 32 are left.
 __global__ void __launch_bounds__(128, 3) attention2_kernel(const __half* __restrict__ qkv, const int32_t* __restrict__ cu,
                                                          const int32_t* __restrict__ order, int H, int n_heads,
-                                                         float scale_log2e, __half* __restrict__ ctx, int n_seq, int seq_fastest, int stage_async) {
+                                                         float scale_log2e, __half* __restrict__ ctx) {
   extern __shared__ __align__(16) unsigned char att_smem[];
-  // CTA -> (sequence slot, head): heads fastest (the twelve CTAs of a sequence run together and read the same qkv
-  // rows), or sequences fastest (RL_XENC_ATT_ORDER=1, the A/B alternative: every head walks the length-sorted list).
-  const int head = seq_fastest ? (int)(blockIdx.x / (unsigned)n_seq) : (int)(blockIdx.x % (unsigned)n_heads);
-  const int slot = seq_fastest ? (int)(blockIdx.x % (unsigned)n_seq) : (int)(blockIdx.x / (unsigned)n_heads);
-  const int seq = order != nullptr ? order[slot] : slot;
+  // CTA -> (sequence slot, head), heads fastest: the twelve CTAs of a sequence run together and read the same qkv rows.
+  const int head = (int)(blockIdx.x % (unsigned)n_heads);
+  const int seq = order[(int)(blockIdx.x / (unsigned)n_heads)];
   const int t0 = cu[seq], L = cu[seq + 1] - t0;
   const int Lp = (L + 63) / 64 * 64;
   __half* Ks = reinterpret_cast<__half*>(att_smem);
   __half* Vs = Ks + (size_t)Lp * kAttPitch;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const size_t ld = (size_t)3 * H;
-  if (stage_async) {
-    // K / V of the head: global -> shared memory with cp.async (16 bytes each, zero-filled past the sequence), no
-    // registers in between; the first Q fragments are requested below while these copies are in flight.
+  // K / V of the head: global -> shared memory with cp.async (16 bytes each, zero-filled past the sequence), no
+  // registers in between; the first Q fragments are requested below while these copies are in flight.
 #pragma unroll 4
-    for (int idx = threadIdx.x; idx < Lp * 4; idx += blockDim.x) {
-      const int j = idx >> 2, c = idx & 3;
-      const __half* base = qkv + (size_t)(t0 + (j < L ? j : L - 1)) * ld + head * 32 + c * 8;
-      const uint32_t nbytes = j < L ? 16u : 0u;
-      cp_async_16(smem_u32(Ks + (size_t)j * kAttPitch + c * 8), base + H, nbytes);
-      cp_async_16(smem_u32(Vs + (size_t)j * kAttPitch + c * 8), base + 2 * H, nbytes);
-    }
-    asm volatile("cp.async.commit_group;" ::: "memory");
-  } else {
-#pragma unroll 4
-    for (int idx = threadIdx.x; idx < Lp * 4; idx += blockDim.x) {
-      const int j = idx >> 2, c = idx & 3;
-      uint4 kv = make_uint4(0u, 0u, 0u, 0u), vv = kv;
-      if (j < L) {
-        const __half* base = qkv + (size_t)(t0 + j) * ld + head * 32 + c * 8;
-        kv = __ldg(reinterpret_cast<const uint4*>(base + H));
-        vv = __ldg(reinterpret_cast<const uint4*>(base + 2 * H));
-      }
-      *reinterpret_cast<uint4*>(Ks + (size_t)j * kAttPitch + c * 8) = kv;
-      *reinterpret_cast<uint4*>(Vs + (size_t)j * kAttPitch + c * 8) = vv;
-    }
+  for (int idx = threadIdx.x; idx < Lp * 4; idx += blockDim.x) {
+    const int j = idx >> 2, c = idx & 3;
+    const __half* base = qkv + (size_t)(t0 + (j < L ? j : L - 1)) * ld + head * 32 + c * 8;
+    const uint32_t nbytes = j < L ? 16u : 0u;
+    cp_async_16(smem_u32(Ks + (size_t)j * kAttPitch + c * 8), base + H, nbytes);
+    cp_async_16(smem_u32(Vs + (size_t)j * kAttPitch + c * 8), base + 2 * H, nbytes);
   }
+  asm volatile("cp.async.commit_group;" ::: "memory");
   const int r = lane >> 2, cp = (lane & 3) * 2;
   auto load_q = [&](int qb, uint32_t (&a)[2][4]) {   // A fragments of S = Q K^T for one 16-query tile (rows >= L read as zero)
     const int q0 = qb * 16 + r, q1 = q0 + 8;
@@ -639,7 +436,7 @@ __global__ void __launch_bounds__(128, 3) attention2_kernel(const __half* __rest
   uint32_t a[2][2][4];
   load_q(2 * warp, a[0]);
   load_q(2 * warp + 1, a[1]);
-  if (stage_async) asm volatile("cp.async.wait_group 0;" ::: "memory");
+  asm volatile("cp.async.wait_group 0;" ::: "memory");
   __syncthreads();
   for (int pb = warp; pb * 32 < L; pb += 4) {   // this warp's pair of tiles: queries [32 pb, 32 pb + 32)
     float m[2][2], l[2][2], O[2][4][4];
@@ -767,7 +564,7 @@ __global__ void __launch_bounds__(128, 3) attention2_kernel(const __half* __rest
 // shared memory in 64-key blocks, double-buffered with cp.async (zero-filled past the sequence), so a CTA holds 36 KB
 // whatever the length and several CTAs share an SM; the whole head of a 512-token sequence resident (the design of
 // attention2_kernel) would take about 147 KB at this width.  S = Q K^T and O += P V on m16n8k16 (fp16 in, fp32
-// accumulate), online softmax in the exp2 domain as in attention_kernel.  CTAs walk the sequences longest first
+// accumulate), online softmax in the exp2 domain as in attention2_kernel.  CTAs walk the sequences longest first
 // (seq_order_kernel), heads and then query blocks fastest.
 constexpr int kAtt64Dim = 64;
 constexpr int kAtt64Keys = 64;                 // keys per streamed block
@@ -1046,76 +843,30 @@ extern "C" int rl_xenc_linear(const void* X, const void* image, const float* bia
                        (cudaStream_t)stream);
 }
 
-// ---- attention step: variant selection and launches, shared by rl_xenc_score and the rl_xenc_attention test hook ----
-// Each variant switch is an A/B alternative read once per process from its environment variable.
-struct AttVariant {
-  bool lpt;           // RL_XENC_ATT_LPT (default on): walk the sequences longest first (0: arrival order, the A/B baseline)
-  bool stage_async;   // RL_XENC_ATT_CPASYNC (default on): K / V staging through cp.async with the first Q loads
-                      // overlapped (0: plain loads, the A/B baseline)
-  bool seq_fastest;   // RL_XENC_ATT_ORDER=1: sequences fastest in the CTA order of attention2_kernel (default: heads)
-  bool att2;          // RL_XENC_ATT2 (default on): attention2_kernel, two tiles per warp (0: attention_kernel)
-  bool quad;          // RL_XENC_ATT_QUAD=1: Q loads / context stores of attention_kernel as 16-byte rows + a quad
-                      // transpose (default: 4-byte fragment pieces)
-  bool buckets;       // RL_XENC_ATT_BUCKETS=1: two launches bucketed by length (default: one launch)
-};
-static const AttVariant& att_variant() {
-  static const AttVariant v = []() {
-    auto on = [](const char* name, bool dflt) { const char* e = getenv(name); return e == nullptr ? dflt : atoi(e) != 0; };
-    const char* order = getenv("RL_XENC_ATT_ORDER");
-    AttVariant r;
-    r.lpt = on("RL_XENC_ATT_LPT", true);
-    r.stage_async = on("RL_XENC_ATT_CPASYNC", true);
-    r.seq_fastest = order != nullptr && atoi(order) == 1;
-    r.att2 = on("RL_XENC_ATT2", true);
-    r.quad = on("RL_XENC_ATT_QUAD", false);
-    r.buckets = on("RL_XENC_ATT_BUCKETS", false);
-    return r;
-  }();
-  return v;
-}
-
-// Two launches when the batch holds long sequences (RL_XENC_ATT_BUCKETS=1): keys <= kAttShort with a small allocation
-// (occupancy), the rest with the full one (a single launch sized by the longest sequence holds every CTA to the largest
-// allocation).
-constexpr int kAttShort = 256;
+// ---- attention step: setup and launches, shared by rl_xenc_score, rl_xenc_encode and their attention test hooks ----
 static size_t att_smem_bytes(int max_len) { return (size_t)((max_len + 63) / 64 * 64) * kAttPitch * 2 * sizeof(__half); }
 
-// Once per forward: the length-sorted sequence order (seq_order [P], when LPT is on) and the kernels' shared-memory limit.
-static int attention_setup(const int32_t* cu_seqlens, int P, int max_len, int32_t* seq_order, cudaStream_t stream) {
-  const AttVariant& v = att_variant();
-  const size_t att_smem = att_smem_bytes(max_len);
-  RL_REQUIRE(att_smem <= 200 * 1024, RL_EUNSUPPORTED, "max_len=%d too long for the attention kernel", max_len);
-  if (v.lpt) {
-    seq_order_kernel<<<1, 1024, 0, stream>>>(cu_seqlens, P, seq_order);
-    RL_CUDA_CHECK(cudaGetLastError());
+// Once per forward: the length-sorted sequence order (seq_order [P]) that both attention kernels walk and, at head_dim
+// 32, attention2_kernel's shared-memory limit (K and V of the longest sequence).  Refuses a too long max_len before any
+// CUDA call.
+static int attention_setup(int head_dim, const int32_t* cu_seqlens, int P, int max_len, int32_t* seq_order,
+                           cudaStream_t stream) {
+  if (head_dim == 32) {
+    const size_t att_smem = att_smem_bytes(max_len);
+    RL_REQUIRE(att_smem <= 200 * 1024, RL_EUNSUPPORTED, "max_len=%d too long for the attention kernel", max_len);
+    RL_CUDA_CHECK(cudaFuncSetAttribute(attention2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)att_smem));
   }
-  RL_CUDA_CHECK(cudaFuncSetAttribute(attention_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)att_smem));
-  RL_CUDA_CHECK(cudaFuncSetAttribute(attention_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)att_smem));
-  RL_CUDA_CHECK(cudaFuncSetAttribute(attention2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)att_smem));
+  seq_order_kernel<<<1, 1024, 0, stream>>>(cu_seqlens, P, seq_order);
+  RL_CUDA_CHECK(cudaGetLastError());
   return RL_OK;
 }
 
-// Once per layer: ctx = softmax(Q K^T / sqrt(32)) V per sequence and head, from qkv [T, 3H] (Q | K | V).
+// Once per layer at head_dim 32: ctx = softmax(Q K^T / sqrt(32)) V per sequence and head, from qkv [T, 3H] (Q | K | V).
 static int attention_launch(const __half* qkv, const int32_t* cu_seqlens, const int32_t* seq_order, int P, int max_len,
                             int H, int nh, __half* ctx, cudaStream_t stream) {
-  const AttVariant& v = att_variant();
-  const size_t att_smem = att_smem_bytes(max_len), att_smem_short = att_smem_bytes(kAttShort);
   const float scale = 1.4426950408889634f / sqrtf(32.f);  // softmax in the exp2 domain
-  auto attention = [&](size_t smem, int lo, int hi) {
-    if (v.att2 && lo == 0 && hi == max_len)
-      attention2_kernel<<<dim3((unsigned)P * (unsigned)nh), 128, smem, stream>>>(qkv, cu_seqlens, v.lpt ? seq_order : nullptr, H, nh, scale, ctx,
-                                                                                     P, v.seq_fastest ? 1 : 0, v.stage_async ? 1 : 0);
-    else if (v.quad) attention_kernel<true><<<dim3(P, nh), 128, smem, stream>>>(qkv, cu_seqlens, H, nh, scale, ctx, lo, hi);
-    else attention_kernel<false><<<dim3(P, nh), 128, smem, stream>>>(qkv, cu_seqlens, H, nh, scale, ctx, lo, hi);
-  };
-  // Two launches bucketed by length or one launch (the default): the long sequences carry most of the L^2 work either
-  // way, and the split adds a tail.
-  if (v.buckets && max_len > kAttShort) {
-    attention(att_smem_short, 0, kAttShort);
-    attention(att_smem, kAttShort, max_len);
-  } else {
-    attention(att_smem, 0, max_len);
-  }
+  attention2_kernel<<<dim3((unsigned)P * (unsigned)nh), 128, att_smem_bytes(max_len), stream>>>(qkv, cu_seqlens, seq_order,
+                                                                                                  H, nh, scale, ctx);
   RL_CUDA_CHECK(cudaGetLastError());
   return RL_OK;
 }
@@ -1131,7 +882,7 @@ extern "C" int rl_xenc_attention(const void* qkv, const int32_t* cu_seqlens, int
              RL_ENOSPACE, "rl_xenc_attention: workspace must be 16-byte aligned and hold %d int32", P);
   cudaStream_t stream = (cudaStream_t)stream_;
   int32_t* seq_order = reinterpret_cast<int32_t*>(workspace);
-  const int rc = attention_setup(cu_seqlens, P, max_len, seq_order, stream);
+  const int rc = attention_setup(32, cu_seqlens, P, max_len, seq_order, stream);
   if (rc != RL_OK) return rc;
   return attention_launch(reinterpret_cast<const __half*>(qkv), cu_seqlens, seq_order, P, max_len, hidden, n_heads,
                           reinterpret_cast<__half*>(ctx), stream);
@@ -1145,13 +896,7 @@ extern "C" size_t rl_xenc_workspace_bytes(const rl_xenc_weights* w, int T) {
   return ((size_t)T * (H + 3 * H + H + H + F) * sizeof(__half) + (size_t)T * sizeof(int32_t) + 4096);
 }
 
-// ---- attention at head_dim 64: setup and launches, shared by rl_xenc_encode and the rl_xenc_encode_attention hook ----
-static int attention64_setup(const int32_t* cu_seqlens, int P, int32_t* seq_order, cudaStream_t stream) {
-  seq_order_kernel<<<1, 1024, 0, stream>>>(cu_seqlens, P, seq_order);
-  RL_CUDA_CHECK(cudaGetLastError());
-  return RL_OK;
-}
-
+// ---- attention at head_dim 64: launches, shared by rl_xenc_encode and the rl_xenc_encode_attention hook ----------
 static int attention64_launch(const __half* qkv, const int32_t* cu_seqlens, const int32_t* seq_order, int P, int max_len,
                               int H, int nh, __half* ctx, cudaStream_t stream) {
   const int n_qb = (max_len + kAtt64Queries - 1) / kAtt64Queries;
@@ -1162,13 +907,7 @@ static int attention64_launch(const __half* qkv, const int32_t* cu_seqlens, cons
   return RL_OK;
 }
 
-// The attention step of an encoder forward by head_dim: 32 takes the cross-encoder's kernels (and their RL_XENC_ATT*
-// selection), 64 attention64_kernel.
-static int encoder_attention_setup(int head_dim, const int32_t* cu_seqlens, int P, int max_len, int32_t* seq_order,
-                                   cudaStream_t stream) {
-  return head_dim == 64 ? attention64_setup(cu_seqlens, P, seq_order, stream)
-                        : attention_setup(cu_seqlens, P, max_len, seq_order, stream);
-}
+// The attention launch of an encoder forward by head_dim: 32 attention2_kernel, 64 attention64_kernel.
 static int encoder_attention_launch(int head_dim, const __half* qkv, const int32_t* cu_seqlens, const int32_t* seq_order, int P,
                                     int max_len, int H, int nh, __half* ctx, cudaStream_t stream) {
   return head_dim == 64 ? attention64_launch(qkv, cu_seqlens, seq_order, P, max_len, H, nh, ctx, stream)
@@ -1217,7 +956,7 @@ static int encoder_forward(const rl_xenc_weights* w, const int32_t* input_ids, c
   __half* ffn = tmp + (size_t)T * H;
   int32_t* seq_order = reinterpret_cast<int32_t*>(
       (reinterpret_cast<uintptr_t>(ffn + (size_t)T * F) + 15) & ~uintptr_t(15));   // [P] (P <= T)
-  int rc = encoder_attention_setup(head_dim, cu_seqlens, P, max_len, seq_order, stream);
+  int rc = attention_setup(head_dim, cu_seqlens, P, max_len, seq_order, stream);
   if (rc != RL_OK) return rc;
   launch_embed_ln(w, input_ids, type_ids, pos_ids, T, hidden, stream);
   RL_CUDA_CHECK(cudaGetLastError());
@@ -1309,7 +1048,7 @@ extern "C" int rl_xenc_encode_attention(const void* qkv, const int32_t* cu_seqle
   cudaStream_t stream = (cudaStream_t)stream_;
   const int head_dim = hidden / n_heads;
   int32_t* seq_order = reinterpret_cast<int32_t*>(workspace);
-  const int rc = encoder_attention_setup(head_dim, cu_seqlens, P, max_len, seq_order, stream);
+  const int rc = attention_setup(head_dim, cu_seqlens, P, max_len, seq_order, stream);
   if (rc != RL_OK) return rc;
   return encoder_attention_launch(head_dim, reinterpret_cast<const __half*>(qkv), cu_seqlens, seq_order, P, max_len, hidden,
                                   n_heads, reinterpret_cast<__half*>(ctx), stream);
