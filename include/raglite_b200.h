@@ -266,11 +266,13 @@ int rl_segment_mean_pool(const float* X, int64_t ld, int d, const int32_t* row_b
                          const int32_t* row_end, int S, int normalize, uint16_t* out, void* stream);
 
 /* ---- Cross-encoder scoring: _search.py:364-397 (reranker.rank -> FlashRank -> onnxruntime) --------
- * BERT cross-encoder forward (ms-marco-MiniLM-L-12-v2 architecture: LayerNorm(word+pos+type) ->
- * n_layers x [self-attention, dense+residual+LN, dense+GELU(erf), dense+residual+LN] -> pooler
- * (dense+tanh on [CLS]) -> classifier (1 logit)), fp16 storage / fp32 accumulate.  Linear layers are
- * pre-packed once with rl_xenc_pack_linear into the swizzled fp16 image the tensor-core kernel
- * bulk-copies.  All pointers are device pointers except `layers` (host array). */
+ * BERT / XLM-RoBERTa cross-encoder forward (ms-marco-MiniLM-L-12-v2 architecture and wider:
+ * LayerNorm(word+pos+type) -> n_layers x [self-attention, dense+residual+LN, dense+GELU(erf),
+ * dense+residual+LN] -> pooler (dense+tanh on the first token) -> classifier (1 or 2 logits)), fp16
+ * storage / fp32 accumulate.  XLM-RoBERTa's classifier.dense / classifier.out_proj fill the pooler /
+ * classifier slots.  Linear layers are pre-packed once with rl_xenc_pack_linear into the swizzled fp16
+ * image the tensor-core kernel bulk-copies.  All pointers are device pointers except `layers` (host
+ * array). */
 typedef struct rl_xenc_layer {
   const void* qkv_img;   /* packed [3H, H]  (Q | K | V rows) */
   const float* qkv_bias; /* [3H] */
@@ -297,8 +299,9 @@ typedef struct rl_xenc_weights {
   const rl_xenc_layer* layers; /* HOST array of n_layers entries */
   const float* pooler_w; /* fp32 [H, H] */
   const float* pooler_b;
-  const float* cls_w;    /* fp32 [H] (num_labels == 1) */
-  const float* cls_b;    /* fp32 [1] */
+  const float* cls_w;    /* fp32 [n_labels, H] */
+  const float* cls_b;    /* fp32 [n_labels] */
+  int32_t n_labels;      /* 1 or 2; 0 is read as 1 (appended: every earlier field keeps its offset) */
 } rl_xenc_weights;
 
 size_t rl_xenc_linear_image_bytes(int N, int K);
@@ -310,7 +313,14 @@ int rl_xenc_linear(const void* X, const void* image, const float* bias, void* Y,
                    void* stream);
 size_t rl_xenc_workspace_bytes(const rl_xenc_weights* w, int T);
 /* Packed variable-length batch: input_ids/type_ids/pos_ids [T], cu_seqlens [P+1]; max_len = longest
- * sequence.  out_logit[P], out_score[P] = sigmoid(logit) (FlashRank's score). */
+ * sequence.  out_logit [P, n_labels] row-major ([P] at one label); out_score [P] is FlashRank's score:
+ * sigmoid(logit) at one label, softmax(logits)[1] = 1 / (1 + exp(l0 - l1)) at two.
+ * Shapes: either head_dim (hidden / n_heads) 32 with hidden % 32 == 0, hidden <= 512 and
+ * 0 < max_len <= max_pos (bounded by the attention kernel's shared memory: about 1280 tokens), or
+ * everything rl_xenc_encode takes (head_dim 32 or 64, hidden % 32 == 0 and <= 1024, n_layers >= 1,
+ * 0 < max_len <= min(512, max_pos)); ffn % 32 == 0, n_labels 0, 1 or 2, P <= T, workspace >=
+ * rl_xenc_workspace_bytes(w, T).  Anything else is refused with RL_EUNSUPPORTED / RL_EINVAL /
+ * RL_ENOSPACE before any CUDA call. */
 int rl_xenc_score(const rl_xenc_weights* w, const int32_t* input_ids, const int32_t* type_ids, const int32_t* pos_ids,
                   const int32_t* cu_seqlens, int P, int T, int max_len, float* out_logit, float* out_score,
                   void* workspace, size_t workspace_bytes, void* stream);

@@ -61,7 +61,7 @@ class XencWeights(C.Structure):
         ("max_pos", C.c_int32), ("type_vocab", C.c_int32), ("ln_eps", C.c_float),
         ("word_emb", C.c_void_p), ("pos_emb", C.c_void_p), ("type_emb", C.c_void_p), ("emb_ln_g", C.c_void_p),
         ("emb_ln_b", C.c_void_p), ("layers", C.POINTER(XencLayer)), ("pooler_w", C.c_void_p), ("pooler_b", C.c_void_p),
-        ("cls_w", C.c_void_p), ("cls_b", C.c_void_p),
+        ("cls_w", C.c_void_p), ("cls_b", C.c_void_p), ("n_labels", C.c_int32),
     ]
 
 

@@ -56,8 +56,9 @@ class ScoreFnRanker:
 
 
 class B200CrossEncoderRanker(ScoreFnRanker):
-    """BERT cross-encoder (ms-marco-MiniLM-L-12-v2 architecture) scored on the GPU.  Weights are
-    loaded lazily from ``cache_dir/<model_name>`` (HF ``safetensors`` + tokenizer files)."""
+    """Cross-encoder scored on the GPU: a BERT (ms-marco-MiniLM-L-12-v2, multilingual BERT-base) or
+    XLM-RoBERTa sequence classifier with one or two labels.  Weights are loaded lazily from
+    ``cache_dir/<model_name>`` (HF ``config.json`` + ``safetensors`` + ``tokenizer.json``)."""
 
     def __init__(self, model_name: str, *, cache_dir: Path | str | None = None, max_length: int = 512,
                  device: Any | None = None):
@@ -76,9 +77,12 @@ class B200CrossEncoderRanker(ScoreFnRanker):
             if not (path / "config.json").exists():
                 raise FileNotFoundError(
                     f"B200CrossEncoderRanker: no Hugging Face model directory at {path}.  The reference's FlashRank "
-                    "reranker downloads an ONNX file on first use; this ranker needs the same model as HF weights "
-                    "(config.json + model.safetensors + tokenizer.json, e.g. `huggingface-cli download "
-                    f"cross-encoder/{self.model_name} --local-dir {path}`), or pass any object with a "
-                    ".rank(query=, docs=) method as RAGLiteConfig.reranker (None disables reranking).  See INTEGRATION.md.")
+                    "reranker downloads an ONNX file on first use; this ranker needs the model as HF weights in that "
+                    "directory: config.json (model_type bert with BertForSequenceClassification weights, or "
+                    "xlm-roberta / roberta with XLMRobertaForSequenceClassification / RobertaForSequenceClassification "
+                    "weights; 1 or 2 labels, head_dim 32 or 64, hidden <= 1024), model.safetensors (or "
+                    "pytorch_model.bin) and tokenizer.json (e.g. `huggingface-cli download <repo id> --local-dir "
+                    f"{path}` for a checkpoint of that kind), or pass any object with a .rank(query=, docs=) method as "
+                    "RAGLiteConfig.reranker (None disables reranking).  See INTEGRATION.md.")
             self._engine = CrossEncoderEngine.from_pretrained(path, max_length=self.max_length, device=self.device)
         return self._engine.score_pairs([query] * len(docs), list(docs))

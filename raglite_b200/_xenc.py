@@ -1,10 +1,12 @@
-"""BERT cross-encoder engine on the GPU -- the arithmetic behind ``rerank_chunks``.
+"""BERT / XLM-RoBERTa cross-encoder engine on the GPU -- the arithmetic behind ``rerank_chunks``.
 
 The reference calls ``reranker.rank(query=, docs=)`` (``_search.py:395``) on a ``rerankers``
 FlashRankRanker: tokenise (query, passage) pairs, run ms-marco-MiniLM-L-12-v2 (BERT, 12 layers, H=384,
 12 heads, FFN=1536) with onnxruntime, sigmoid the logit, sort.  Here the forward runs in
 ``rl_xenc_score`` (hand-written CUDA: wgmma linear layers with fused bias/GELU, attention,
 LayerNorm, pooler+classifier) on packed variable-length batches -- no padding tokens are computed.
+The same engine scores wider multilingual rerankers: BERT-base and XLM-RoBERTa sequence classifiers
+(head_dim 64, H <= 1024) with one logit, or two scored as ``softmax(logits)[1]``.
 
 ``TokenEmbedderEngine`` runs the same encoder without the head (``rl_xenc_encode``: head_dim 32 or 64, H <= 1024) and
 returns per-token hidden states: the embedding model behind ``embed_strings`` (bge-m3 by default), which the reference
@@ -206,61 +208,115 @@ class _EncoderEngine:
         return dev[:T], dev[T:2 * T], dev[2 * T:3 * T], dev[3 * T:n_in]
 
 
+# Tokens per forward call of CrossEncoderEngine.  The workspace takes T (12 H + 2 F) bytes: 2^18 tokens are 1.9 GB at
+# MiniLM's shape (H = 384, F = 1536) but 4 GB at BERT-base's (H = 768, F = 3072) and 5.4 GB at XLM-R large's (H = 1024,
+# F = 4096), so wider models take 2^16 (1.0 / 1.34 GB).
+XENC_TOKENS_PER_CALL = 1 << 18
+XENC_WIDE_TOKENS_PER_CALL = 1 << 16
+# The families whose sequence classifiers load, and where their head lives in the state dict: (pooler dense, classifier)
+# prefixes.  XLM-RoBERTa's classifier.dense -> tanh -> classifier.out_proj on the first token is BERT's pooler -> classifier.
+_XENC_HEADS = {"bert": ("pooler.dense.", "classifier."), "xlm-roberta": ("classifier.dense.", "classifier.out_proj."),
+               "roberta": ("classifier.dense.", "classifier.out_proj.")}
+XENC_MAX_HIDDEN = 1024
+
+
+def check_cross_encoder_shape(*, model_type: str, num_labels: int, hidden_act: str, hidden: int, n_heads: int) -> None:
+    """Raise ``ValueError`` naming the limit when ``rl_xenc_score`` or the engine cannot run a model (no device work)."""
+    if model_type not in _XENC_HEADS:
+        raise ValueError(f"model_type={model_type!r} unsupported: the cross-encoder loads BERT or XLM-RoBERTa / RoBERTa "
+                         "sequence classifiers")
+    if num_labels not in (1, 2):
+        raise ValueError(f"num_labels={num_labels} unsupported: the classification head computes 1 or 2 labels")
+    if hidden_act != "gelu":
+        raise ValueError(f"hidden_act={hidden_act!r} unsupported: the encoder's FFN computes GELU(erf) only")
+    if n_heads <= 0 or hidden % n_heads or hidden // n_heads not in (32, 64):
+        raise ValueError(f"hidden={hidden} heads={n_heads} unsupported: head_dim (hidden / heads) must be 32 or 64")
+    if hidden % 32 or hidden > XENC_MAX_HIDDEN:
+        raise ValueError(f"hidden={hidden} unsupported: hidden must be a multiple of 32 and at most {XENC_MAX_HIDDEN}")
+
+
 class CrossEncoderEngine(_EncoderEngine):
-    """Device-resident packed weights + tokenizer + batching."""
+    """Device-resident packed weights + tokenizer + batching for BERT and XLM-RoBERTa / RoBERTa sequence classifiers with
+    one or two labels (head_dim 32 or 64, H <= 1024).  ``score_tokens`` returns logits ``[P]`` (one label) or ``[P, 2]``
+    (two) and FlashRank's score ``[P]``: ``sigmoid(logit)``, or ``softmax(logits)[1]``."""
 
     def __init__(self, state_dict: dict[str, torch.Tensor], *, n_layers: int, hidden: int, n_heads: int, ffn: int,
                  max_pos: int, ln_eps: float = 1e-12, tokenizer: Any | None = None, max_length: int = 512,
-                 device: Any | None = None, max_tokens_per_call: int = 1 << 18) -> None:
+                 device: Any | None = None, max_tokens_per_call: int | None = None, model_type: str = "bert",
+                 pos_offset: int = 0, hidden_act: str = "gelu") -> None:
+        head = _XENC_HEADS.get(model_type)
+        cls_weight = state_dict.get(head[1] + "weight") if head else None
+        n_labels = int(cls_weight.shape[0]) if cls_weight is not None and cls_weight.dim() == 2 else 1
+        check_cross_encoder_shape(model_type=model_type, num_labels=n_labels, hidden_act=hidden_act, hidden=hidden,
+                                  n_heads=n_heads)
+        if cls_weight is None or tuple(cls_weight.shape[-1:]) != (hidden,):
+            raise ValueError(f"no {head[1]}weight of shape [num_labels, {hidden}] in the state dict")
+        # head_dim 32 at H <= 512 (MiniLM) keeps rl_xenc_score's own envelope: sequences up to the position table
+        narrow = hidden <= 512 and hidden // n_heads == 32
+        if max_tokens_per_call is None:
+            max_tokens_per_call = XENC_TOKENS_PER_CALL if hidden <= 512 else XENC_WIDE_TOKENS_PER_CALL
         super().__init__(state_dict, n_layers=n_layers, hidden=hidden, n_heads=n_heads, ffn=ffn, max_pos=max_pos,
-                         ln_eps=ln_eps, device=device, max_tokens_per_call=max_tokens_per_call)
+                         ln_eps=ln_eps, device=device, max_tokens_per_call=max_tokens_per_call, pos_offset=pos_offset)
         self.tokenizer = tokenizer
-        self.max_length = min(max_length, max_pos)
+        self.model_type = model_type
+        self.n_labels = n_labels
+        self.max_length = min(max_length, max_pos - pos_offset) if narrow else min(max_length, max_pos - pos_offset, 512)
         w = self.weights
-        w.pooler_w, w.pooler_b = self._f32("pooler.dense.weight").data_ptr(), self._f32("pooler.dense.bias").data_ptr()
-        cls_w = state_dict["classifier.weight"].detach().to(device=self.device, dtype=torch.float32).reshape(-1).contiguous()
-        if cls_w.numel() != hidden:
-            raise ValueError("only single-logit classifiers (num_labels == 1) are supported")
-        cls_b = state_dict["classifier.bias"].detach().to(device=self.device, dtype=torch.float32).contiguous()
-        self._keep += [cls_w, cls_b]
-        w.cls_w, w.cls_b = cls_w.data_ptr(), cls_b.data_ptr()
+        pooler, classifier = head
+        w.pooler_w, w.pooler_b = self._f32(pooler + "weight").data_ptr(), self._f32(pooler + "bias").data_ptr()
+        w.cls_w, w.cls_b = self._f32(classifier + "weight").data_ptr(), self._f32(classifier + "bias").data_ptr()
+        w.n_labels = n_labels
 
     # ---- constructors ------------------------------------------------------------------------------
     @classmethod
     def from_hf(cls, model: Any, tokenizer: Any | None = None, **kw: Any) -> "CrossEncoderEngine":
-        """From a ``transformers.BertForSequenceClassification`` (num_labels == 1)."""
+        """From a ``transformers`` ``BertForSequenceClassification`` or ``XLMRobertaForSequenceClassification`` /
+        ``RobertaForSequenceClassification`` with one or two labels."""
         c = model.config
+        check_cross_encoder_shape(model_type=c.model_type, num_labels=int(c.num_labels),
+                                  hidden_act=getattr(c, "hidden_act", "gelu"), hidden=c.hidden_size,
+                                  n_heads=c.num_attention_heads)
         return cls(model.state_dict(), n_layers=c.num_hidden_layers, hidden=c.hidden_size, n_heads=c.num_attention_heads,
                    ffn=c.intermediate_size, max_pos=c.max_position_embeddings, ln_eps=c.layer_norm_eps,
-                   tokenizer=tokenizer, **kw)
+                   tokenizer=tokenizer, model_type=c.model_type, pos_offset=_position_offset(c),
+                   hidden_act=getattr(c, "hidden_act", "gelu"), **kw)
 
     @classmethod
     def from_pretrained(cls, path: Path | str, **kw: Any) -> "CrossEncoderEngine":
-        """Load HF weights + ``tokenizer.json`` from a local directory (no network access is attempted)."""
+        """Load HF weights + ``tokenizer.json`` from a local directory (no network access is attempted).  The class is
+        chosen by ``config.json``'s ``model_type``: ``bert``, ``xlm-roberta`` or ``roberta``."""
         path = Path(path)
         if not (path / "config.json").exists():
             raise FileNotFoundError(f"No cross-encoder weights at {path} (expected an HF model directory)")
         from tokenizers import Tokenizer
-        from transformers import BertForSequenceClassification
+        from transformers import (AutoConfig, BertForSequenceClassification, RobertaForSequenceClassification,
+                                  XLMRobertaForSequenceClassification)
 
-        model = BertForSequenceClassification.from_pretrained(path, local_files_only=True)
+        config = AutoConfig.from_pretrained(path, local_files_only=True)
+        check_cross_encoder_shape(model_type=config.model_type, num_labels=int(config.num_labels),
+                                  hidden_act=getattr(config, "hidden_act", "gelu"), hidden=config.hidden_size,
+                                  n_heads=config.num_attention_heads)
+        model_cls = {"bert": BertForSequenceClassification, "xlm-roberta": XLMRobertaForSequenceClassification,
+                     "roberta": RobertaForSequenceClassification}[config.model_type]
+        model = model_cls.from_pretrained(path, config=config, local_files_only=True)
         tok = Tokenizer.from_file(str(path / "tokenizer.json")) if (path / "tokenizer.json").exists() else None
         return cls.from_hf(model, tok, **kw)
 
     # ---- scoring ---------------------------------------------------------------------------------------
     def score_tokens(self, ids: Sequence[np.ndarray], type_ids: Sequence[np.ndarray]) -> tuple[np.ndarray, np.ndarray]:
-        """Logits and sigmoid scores for already-tokenised pairs (variable lengths, no padding).
+        """Logits (``[P]`` for one label, ``[P, 2]`` for two) and FlashRank's scores ``[P]`` for already-tokenised pairs
+        (variable lengths, no padding).
 
         The pairs are cut into calls of at most ``max_tokens_per_call`` tokens.  Calls are pipelined: while
         the GPU runs call *i*, the host packs call *i+1* into the other half of a pinned double buffer and
         enqueues its upload and kernels; results come back through pinned memory and are only waited for
         once the next call is in the queue -- the host packing disappears behind the forward."""
-        P = len(ids)
-        logits = np.empty(P, np.float32)
+        P, NL = len(ids), self.n_labels
+        logits = np.empty((P, NL) if NL > 1 else P, np.float32)
         scores = np.empty(P, np.float32)
         lens = np.fromiter((len(x) for x in ids), dtype=np.int64, count=P)
         if P and lens.max() > self.max_length:
-            raise ValueError("sequence longer than max_length")
+            raise ValueError(f"sequence longer than max_length={self.max_length}")
 
         def launch(lo: int, hi: int, slot: int) -> tuple[torch.Tensor, torch.cuda.Event]:
             return self._launch_packed(ids[lo:hi], type_ids[lo:hi], lens[lo:hi], slot=slot)
@@ -268,24 +324,31 @@ class CrossEncoderEngine(_EncoderEngine):
         def collect(lo: int, hi: int, item: tuple[torch.Tensor, torch.cuda.Event]) -> None:
             host, ev = item
             ev.synchronize()
-            res = host.numpy()[: 2 * (hi - lo)].reshape(2, hi - lo)
-            logits[lo:hi], scores[lo:hi] = res[0], res[1]
+            logits[lo:hi], scores[lo:hi] = self._split(host.numpy(), hi - lo)
 
         self._pipelined(lens, launch, collect)
         return logits, scores
 
+    def _split(self, res: np.ndarray, P: int) -> tuple[np.ndarray, np.ndarray]:
+        """The logits [P] / [P, 2] and scores [P] of one call's result buffer (logits [P, n_labels] | scores [P])."""
+        NL = self.n_labels
+        lg = res[: NL * P]
+        return (lg.reshape(P, NL) if NL > 1 else lg), res[NL * P:(NL + 1) * P]
+
     def _launch_packed(self, ids: Sequence[np.ndarray], type_ids: Sequence[np.ndarray], lens: np.ndarray, *, slot: int
                        ) -> tuple[torch.Tensor, torch.cuda.Event]:
         """Pack one call into pinned buffer ``slot``, enqueue upload + forward + download; returns the pinned
-        result buffer and the event that marks it complete.  Caller holds the lock."""
-        P = len(ids)
+        result buffer (logits [P, n_labels] then scores [P]) and the event that marks it complete.  Caller holds the
+        lock."""
+        P, n_out = len(ids), (self.n_labels + 1) * len(ids)
         d_ids, d_types, d_pos, d_cu = self._upload_packed(ids, type_ids, lens, slot=slot)
-        out = torch.empty((2, P), dtype=torch.float32, device=self.device)
+        out = torch.empty(n_out, dtype=torch.float32, device=self.device)
         check(self.lib.rl_xenc_score(C.byref(self.weights), d_ids.data_ptr(), d_types.data_ptr(), d_pos.data_ptr(),
-                                     d_cu.data_ptr(), P, len(d_ids), int(lens.max()), out[0].data_ptr(), out[1].data_ptr(),
-                                     self._ws.data_ptr(), self._ws.numel(), _stream()), "rl_xenc_score")
-        host_out = self._pinned(f"out{slot}", 2 * P, torch.float32)
-        host_out[: 2 * P].copy_(out.reshape(-1), non_blocking=True)
+                                     d_cu.data_ptr(), P, len(d_ids), int(lens.max()), out.data_ptr(),
+                                     out[self.n_labels * P:].data_ptr(), self._ws.data_ptr(), self._ws.numel(), _stream()),
+              "rl_xenc_score")
+        host_out = self._pinned(f"out{slot}", n_out, torch.float32)
+        host_out[:n_out].copy_(out, non_blocking=True)
         ev = torch.cuda.Event()
         ev.record()
         return host_out, ev
@@ -296,8 +359,8 @@ class CrossEncoderEngine(_EncoderEngine):
         with self._lock, torch.cuda.device(self.device):
             host, ev = self._launch_packed(ids, type_ids, np.asarray(lens, dtype=np.int64), slot=0)
             ev.synchronize()
-            res = host.numpy()[: 2 * len(ids)].reshape(2, len(ids)).copy()
-        return res[0], res[1]
+            logits, scores = self._split(host.numpy(), len(ids))
+        return logits.copy(), scores.copy()
 
     def encode_pairs(self, queries: Sequence[str], docs: Sequence[str]) -> tuple[list[np.ndarray], list[np.ndarray]]:
         """[CLS] query [SEP] passage [SEP] with truncation to ``max_length`` (FlashRank's tokenizer setup)."""

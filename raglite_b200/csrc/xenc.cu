@@ -10,7 +10,8 @@
 //   attention2_kernel    softmax(Q K^T / sqrt(dh)) V per (sequence, head) at head_dim 32, fp32 math
 //                        (attention64_kernel: head_dim 64, the token encoder of rl_xenc_encode)
 //   add_ln_kernel        LayerNorm(x + residual)
-//   cls_head_kernel      pooler (dense + tanh on [CLS]) -> classifier -> logit, sigmoid score
+//   cls_head_kernel      pooler (dense + tanh on [CLS]) -> classifier -> 1 or 2 logits, FlashRank's score
+//                        (BERT's pooler + classifier; XLM-RoBERTa's classifier.dense + out_proj is the same head)
 #include <cuda.h>
 #include <cuda_fp16.h>
 
@@ -707,20 +708,23 @@ __global__ void __launch_bounds__(kAtt64Threads, 3) attention64_kernel(const __h
 }
 
 // ---- pooler + classifier ----------------------------------------------------------------------------------
-// logit[s] = Wc . tanh(Wp h_s + bp) + bc with h_s the [CLS] row of sequence s.  A CTA owns kClsSeqs sequences
-// (their [CLS] rows sit in shared memory as fp32) and its H/32 warps share the H pooler outputs; for one output
-// the lanes stride over the H inputs, so every Wp read is a coalesced 128-byte line shared by the CTA's
-// sequences, followed by one warp-shuffle reduction per sequence; the warps' partial logits meet in shared
-// memory and are summed in a fixed order.  (Wp read row-per-lane touches 32 lines per load instruction; one warp per
-// four sequences walking all H outputs one after the other is coalesced but leaves a few CTAs with long serial work.)
+// logit[s][j] = Wc[j] . tanh(Wp h_s + bp) + bc[j] with h_s the [CLS] row of sequence s and NL (1 or 2) labels j.
+// A CTA owns kClsSeqs sequences (their [CLS] rows sit in shared memory as fp32) and its min(H/32, 16) warps share the
+// H pooler outputs; for one output the lanes stride over the H inputs, so every Wp read is a coalesced 128-byte line
+// shared by the CTA's sequences, followed by one warp-shuffle reduction per sequence; the warps' NL partial logits
+// per sequence meet in shared memory and are summed in a fixed order.  (Wp read row-per-lane touches 32 lines per
+// load instruction; one warp per four sequences walking all H outputs one after the other is coalesced but leaves a
+// few CTAs with long serial work.)  logit is [P, NL] row-major; score is sigmoid(l) at one label and softmax(l)[1]
+// = 1 / (1 + exp(l0 - l1)) at two, a form that cannot overflow where exp(l1) / (exp(l0) + exp(l1)) can.
 constexpr int kClsSeqs = 2;
 constexpr int kClsMaxWarps = 16;
+template <int NL>
 __global__ void __launch_bounds__(kClsMaxWarps * 32) cls_head_kernel(const __half* __restrict__ hidden, const int32_t* __restrict__ cu,
                                                                      const float* __restrict__ Wp, const float* __restrict__ bp,
                                                                      const float* __restrict__ Wc, const float* __restrict__ bc,
                                                                      int P, int H, float* __restrict__ logit,
                                                                      float* __restrict__ score) {
-  extern __shared__ float cls_smem[];  // [kClsSeqs][H] [CLS] rows as fp32, then [warps][kClsSeqs] partial logits
+  extern __shared__ float cls_smem[];  // [kClsSeqs][H] [CLS] rows as fp32, then [warps][kClsSeqs][NL] partial logits
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
   const int seq0 = blockIdx.x * kClsSeqs;
   float* h = cls_smem;
@@ -732,9 +736,11 @@ __global__ void __launch_bounds__(kClsMaxWarps * 32) cls_head_kernel(const __hal
     for (int c = threadIdx.x; c < H; c += blockDim.x) h[s * H + c] = ok ? __half2float(src[c]) : 0.f;
   }
   __syncthreads();
-  float out[kClsSeqs];
+  float out[kClsSeqs][NL];
 #pragma unroll
-  for (int s = 0; s < kClsSeqs; ++s) out[s] = 0.f;
+  for (int s = 0; s < kClsSeqs; ++s)
+#pragma unroll
+    for (int j = 0; j < NL; ++j) out[s][j] = 0.f;
 #pragma unroll 2
   for (int o = warp; o < H; o += nw) {   // this warp's pooler outputs
     const float* w = Wp + (size_t)o * H;
@@ -747,20 +753,35 @@ __global__ void __launch_bounds__(kClsMaxWarps * 32) cls_head_kernel(const __hal
 #pragma unroll
       for (int s = 0; s < kClsSeqs; ++s) a[s] = fmaf(wv, h[s * H + c], a[s]);
     }
-    const float b = __ldg(bp + o), wc = __ldg(Wc + o);
+    const float b = __ldg(bp + o);
+    float wc[NL];
 #pragma unroll
-    for (int s = 0; s < kClsSeqs; ++s) out[s] += tanhf(warp_sum_f(a[s]) + b) * wc;   // identical on every lane
+    for (int j = 0; j < NL; ++j) wc[j] = __ldg(Wc + (size_t)j * H + o);
+#pragma unroll
+    for (int s = 0; s < kClsSeqs; ++s) {
+      const float t = tanhf(warp_sum_f(a[s]) + b);   // identical on every lane
+#pragma unroll
+      for (int j = 0; j < NL; ++j) out[s][j] += t * wc[j];
+    }
   }
   if (lane == 0) {
 #pragma unroll
-    for (int s = 0; s < kClsSeqs; ++s) part[warp * kClsSeqs + s] = out[s];
+    for (int s = 0; s < kClsSeqs; ++s)
+#pragma unroll
+      for (int j = 0; j < NL; ++j) part[(warp * kClsSeqs + s) * NL + j] = out[s][j];
   }
   __syncthreads();
   if (threadIdx.x < kClsSeqs && seq0 + threadIdx.x < P) {   // fixed summation order: deterministic logits
-    float v = bc[0];
-    for (int wi = 0; wi < nw; ++wi) v += part[wi * kClsSeqs + threadIdx.x];
-    logit[seq0 + threadIdx.x] = v;
-    score[seq0 + threadIdx.x] = 1.f / (1.f + __expf(-v));  // FlashRank: sigmoid of the single logit
+    const int seq = seq0 + threadIdx.x;
+    float v[NL];
+#pragma unroll
+    for (int j = 0; j < NL; ++j) {
+      v[j] = bc[j];
+      for (int wi = 0; wi < nw; ++wi) v[j] += part[(wi * kClsSeqs + threadIdx.x) * NL + j];
+      logit[(size_t)seq * NL + j] = v[j];
+    }
+    // FlashRank: sigmoid of a single logit, softmax(logits)[1] of two
+    score[seq] = NL == 1 ? 1.f / (1.f + __expf(-v[0])) : 1.f / (1.f + __expf(v[0] - v[NL - 1]));
   }
 }
 
@@ -981,34 +1002,57 @@ static int encoder_forward(const rl_xenc_weights* w, const int32_t* input_ids, c
   return RL_OK;
 }
 
+// Shapes the encoder path takes: head_dim 32 or 64, H <= 1024 (LayerNorm at 32 columns per lane), up to 512 tokens.
+constexpr int kEncodeMaxHidden = 1024;
+constexpr int kEncodeMaxLen = 512;
+
+// rl_xenc_score takes the union of two envelopes.  The cross-encoder's own (head_dim 32, H <= 512, max_len up to the
+// position table, bounded by attention2_kernel's shared memory) and the token encoder's (head_dim 32 or 64, H <= 1024,
+// max_len <= 512, at least one layer, as rl_xenc_encode).  Both run encoder_forward; the envelopes differ in checks only.
 extern "C" int rl_xenc_score(const rl_xenc_weights* w, const int32_t* input_ids, const int32_t* type_ids,
                              const int32_t* pos_ids, const int32_t* cu_seqlens, int P, int T, int max_len,
                              float* out_logit, float* out_score, void* workspace, size_t workspace_bytes, void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   RL_REQUIRE(w && w->layers && input_ids && type_ids && pos_ids && cu_seqlens && out_logit && out_score, RL_EINVAL,
              "rl_xenc_score: null pointer");
+  const int n_labels = w->n_labels == 0 ? 1 : w->n_labels;   // 0: a zero-initialised struct of a one-label caller
+  RL_REQUIRE(n_labels == 1 || n_labels == 2, RL_EUNSUPPORTED, "rl_xenc_score: n_labels=%d unsupported (1 or 2)", w->n_labels);
   if (P == 0 || T == 0) return RL_OK;
   const int H = w->hidden, F = w->ffn, nh = w->n_heads;
-  RL_REQUIRE(H % 32 == 0 && H <= 512 && nh > 0 && H / nh == 32, RL_EUNSUPPORTED,
-             "rl_xenc_score: hidden=%d heads=%d unsupported (head_dim must be 32, hidden <= 512)", H, nh);
+  const bool narrow = H % 32 == 0 && H <= 512 && nh > 0 && H / nh == 32;
+  const bool wide = H % 32 == 0 && H <= kEncodeMaxHidden && nh > 0 && H % nh == 0 && (H / nh == 32 || H / nh == 64);
+  RL_REQUIRE(narrow || wide, RL_EUNSUPPORTED,
+             "rl_xenc_score: hidden=%d heads=%d unsupported (head_dim 32 with hidden <= 512, or head_dim 32 / 64 with "
+             "hidden %% 32 == 0 and hidden <= %d)", H, nh, kEncodeMaxHidden);
   RL_REQUIRE(F % 32 == 0 && max_len > 0 && max_len <= w->max_pos, RL_EUNSUPPORTED, "rl_xenc_score: bad ffn / max_len");
+  if (narrow) {
+    RL_REQUIRE(att_smem_bytes(max_len) <= 200 * 1024, RL_EUNSUPPORTED, "max_len=%d too long for the attention kernel", max_len);
+  } else {
+    RL_REQUIRE(w->n_layers > 0, RL_EUNSUPPORTED, "rl_xenc_score: n_layers > 0 required at hidden=%d heads=%d", H, nh);
+    RL_REQUIRE(max_len <= kEncodeMaxLen, RL_EUNSUPPORTED,
+               "rl_xenc_score: max_len=%d unsupported at hidden=%d heads=%d (at most min(%d, max_pos=%d))", max_len, H, nh,
+               kEncodeMaxLen, w->max_pos);
+  }
   RL_REQUIRE(workspace && workspace_bytes >= rl_xenc_workspace_bytes(w, T), RL_ENOSPACE, "rl_xenc_score: workspace too small");
+  RL_REQUIRE(P <= T, RL_EINVAL, "rl_xenc_score: more sequences than tokens");
   int dev = 0, sms = 132;
   RL_CUDA_CHECK(cudaGetDevice(&dev));
   RL_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  RL_REQUIRE(P <= T, RL_EINVAL, "rl_xenc_score: more sequences than tokens");
   const int rc = encoder_forward(w, input_ids, type_ids, pos_ids, cu_seqlens, P, T, max_len, workspace, nullptr, sms, stream);
   if (rc != RL_OK) return rc;
   const int cls_warps = H / 32 < kClsMaxWarps ? H / 32 : kClsMaxWarps;
-  cls_head_kernel<<<(P + kClsSeqs - 1) / kClsSeqs, cls_warps * 32, ((size_t)kClsSeqs * H + kClsMaxWarps * kClsSeqs) * sizeof(float), stream>>>(
-      reinterpret_cast<const __half*>(workspace), cu_seqlens, w->pooler_w, w->pooler_b, w->cls_w, w->cls_b, P, H, out_logit, out_score);
+  const dim3 cls_grid((P + kClsSeqs - 1) / kClsSeqs);
+  const size_t cls_smem = ((size_t)kClsSeqs * H + (size_t)kClsMaxWarps * kClsSeqs * n_labels) * sizeof(float);
+  const __half* hidden = reinterpret_cast<const __half*>(workspace);
+  if (n_labels == 1)
+    cls_head_kernel<1><<<cls_grid, cls_warps * 32, cls_smem, stream>>>(hidden, cu_seqlens, w->pooler_w, w->pooler_b, w->cls_w,
+                                                                       w->cls_b, P, H, out_logit, out_score);
+  else
+    cls_head_kernel<2><<<cls_grid, cls_warps * 32, cls_smem, stream>>>(hidden, cu_seqlens, w->pooler_w, w->pooler_b, w->cls_w,
+                                                                       w->cls_b, P, H, out_logit, out_score);
   RL_CUDA_CHECK(cudaGetLastError());
   return RL_OK;
 }
-
-// Shapes the encoder path takes: head_dim 32 or 64, H <= 1024 (LayerNorm at 32 columns per lane), up to 512 tokens.
-constexpr int kEncodeMaxHidden = 1024;
-constexpr int kEncodeMaxLen = 512;
 
 extern "C" int rl_xenc_encode(const rl_xenc_weights* w, const int32_t* input_ids, const int32_t* type_ids,
                               const int32_t* pos_ids, const int32_t* cu_seqlens, int P, int T, int max_len, float* out_hidden,
