@@ -23,12 +23,13 @@ from __future__ import annotations
 
 import ctypes as C
 import threading
-from collections.abc import Sequence
+from collections.abc import Callable, Sequence
 from dataclasses import dataclass, field
 from typing import Any
 
 import numpy as np
 import torch
+import torch.distributed as dist
 
 from . import _lib
 from ._lib import (RL_ALGO, RL_FLAG_COUNT_UNFILTERED, RL_FLAG_REUSE_THRESHOLDS, RL_METRIC, RL_STATUS_CAND_OVERFLOW, ScanParams,
@@ -103,19 +104,27 @@ class ScanResult:
     status: torch.Tensor     # [B] int32
     num_hits: int
     k: int
-    packed: torch.Tensor | None = None   # the four tensors above are views of this uint8 buffer (rl_hits_packed_bytes layout)
+    packed: torch.Tensor | None = None   # the uint8 buffer the four tensors above are views of (hits_views); every scan sets it
+
+
+def hits_views(packed: torch.Tensor, R: int, B: int, H: int
+               ) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]:
+    """``(chunk [R, B, H] int64, sim [R, B, H] float32, count [R, B] int32, status [R, B] int32)``: views of ``R``
+    packed hit lists laid end to end in the uint8 buffer ``packed``, ``rl_hits_packed_bytes(B, H, 1)`` bytes each
+    (at least 16).  The scan writes one such list, the sharded search all-gathers R of them, and
+    ``rl_topk_merge_packed`` reads them in place."""
+    per = max(int(_lib.load().rl_hits_packed_bytes(B, H, 1)), 16)
+    lists = packed[: R * per].view(R, per)
+    n8, n4 = B * H * 8, B * H * 4
+    return (lists[:, :n8].view(torch.int64).view(R, B, H), lists[:, n8:n8 + n4].view(torch.float32).view(R, B, H),
+            lists[:, n8 + n4:n8 + n4 + B * 4].view(torch.int32), lists[:, n8 + n4 + B * 4:n8 + n4 + B * 8].view(torch.int32))
 
 
 def new_scan_result(B: int, H: int, num_hits: int, k: int, device: Any) -> ScanResult:
-    """Scan outputs laid out as ONE packed buffer (chunk | sim | count | status): the all-gather of the sharded
-    path sends it as is and ``rl_topk_merge_packed`` reads the gathered copies in place."""
-    n = int(_lib.load().rl_hits_packed_bytes(B, H, 1))
-    buf = torch.empty(max(n, 16), dtype=torch.uint8, device=device)
-    n8, n4 = B * H * 8, B * H * 4
-    return ScanResult(
-        buf[n8:n8 + n4].view(torch.float32).reshape(B, H), buf[:n8].view(torch.int64).reshape(B, H),
-        buf[n8 + n4:n8 + n4 + B * 4].view(torch.int32), buf[n8 + n4 + B * 4:n8 + n4 + B * 8].view(torch.int32),
-        num_hits, k, buf)
+    """Scan outputs laid out as ONE packed hit list: the all-gather of the sharded path sends it as is."""
+    buf = torch.empty(max(int(_lib.load().rl_hits_packed_bytes(B, H, 1)), 16), dtype=torch.uint8, device=device)
+    chunk, sim, count, status = hits_views(buf, 1, B, H)
+    return ScanResult(sim[0], chunk[0], count[0], status[0], num_hits, k, buf)
 
 
 class CorpusIndex:
@@ -746,42 +755,27 @@ class CorpusIndex:
         return dict(zip(("prep", "sample_scan", "select", "main_scan", "finalize"), (float(x) for x in ms), strict=True))
 
     def scan_checked(self, Q: torch.Tensor, **kw: Any) -> ScanResult:
-        """Scan, read the status back and resolve a candidate-list overflow (adversarial corpus order, or
-        more near-ties at the cut than the list holds): first re-run with the tightened thresholds the
-        first pass left in the workspace, then with a four times larger list, until nothing overflows
-        (the list is bounded by the shard's row count, so this terminates).  The index lock is held
-        throughout: the retry reads thresholds that live in this stream's workspace.
+        """Scan, read the status back and resolve a candidate-list overflow with ``run_until_no_overflow``.
+        The index lock is held throughout: the retry reads thresholds that live in this stream's workspace.
 
         More than ``RL_MAX_SURVIVORS`` vectors inside the coarse scan's error band of the cut (tight
         clusters, thousands of near-duplicates) need no retry: ``finalize`` streams them."""
         kw = dict(kw)
-        out = kw.pop("out", None)
-        base_flags = kw.pop("flags", 0)
-        cap = int(kw.pop("cand_cap", 0))
-        with self._lock:
-            res = self.scan(Q, **kw, flags=base_flags, cand_cap=cap, out=out)
-            for attempt in range(1, 16):
-                if not bool((res.status & RL_STATUS_CAND_OVERFLOW).any()):   # (synchronises)
-                    return res
-                cap, flags = next_overflow_attempt(self, attempt, cap, base_flags)
-                res = self.scan(Q, **kw, flags=flags, cand_cap=cap, out=res)
-        raise _lib.RagliteB200Error("candidate lists still overflow with a list as large as the shard")
+        res = kw.pop("out", None)
+        flags0, cap0 = kw.pop("flags", 0), int(kw.pop("cand_cap", 0))
 
-    def search_pipeline(  # noqa: PLR0913
-        self, Q: torch.Tensor, *, k: int, num_hits: int, metric: str = "cosine", algo: str = "auto",
-        row_allowed: torch.Tensor | None = None, mask_has_tombstones: bool = False, flags: int = 0, cand_cap: int = 0,
-        sample_stride: int = 0, rank_first_limit: int | None = None,
-    ) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]:
-        """scan -> [rank-then-filter cut] -> GROUP BY / top-k, all enqueued on the current stream; returns
-        device tensors ``(sim [B, k], chunk [B, k], count [B], status [B])`` without synchronising."""
-        res = self.scan(Q, k=k, num_hits=num_hits, metric=metric, algo=algo, row_allowed=row_allowed,
-                        mask_has_tombstones=mask_has_tombstones, flags=flags, cand_cap=cand_cap, sample_stride=sample_stride)
-        hit_count = res.hit_count
-        if rank_first_limit is not None:
-            hit_count = limit_hits_to_nearest(self, Q, res.hit_sim[None], hit_count[None], k=k, num_hits=num_hits,
-                                              metric=metric, algo=algo, limit=rank_first_limit)[0]
-        sim, chunk, count = merge_hits(res.hit_sim, res.hit_chunk, hit_count, num_hits=num_hits, k=k)
-        return sim, chunk, count, res.status
+        def run(flags: int, cand_cap: int) -> torch.Tensor:
+            nonlocal res
+            res = self.scan(Q, **kw, flags=flags, cand_cap=cand_cap, out=res)
+            return res.status
+
+        with self._lock:
+            run_until_no_overflow(self, run, flags=flags0, cand_cap=cap0)
+        return res
+
+    def search_pipeline(self, Q: torch.Tensor, **kw: Any) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]:
+        """``scan_gather_merge`` over this shard alone."""
+        return scan_gather_merge(self, Q, **kw)
 
     def chunk_id_of(self, global_chunk: int) -> ChunkId:
         local = int(global_chunk) - self.chunk_base
@@ -813,36 +807,83 @@ class CorpusIndex:
         st = int(raw[n8 + n4 + B * 4:].view(np.int32)[0])
         return (ids, sims, counts, st) if ext is None else (ids, sims, counts, st, ext)
 
+    @staticmethod
+    def _enqueue_download(host: torch.Tensor | None, sim: torch.Tensor, chunk: torch.Tensor, count: torch.Tensor,
+                          status: torch.Tensor, extra: torch.Tensor | None = None) -> torch.Tensor:
+        """Enqueue ONE device->host copy of a merged result (``_pack_result`` layout) into the pinned buffer
+        ``host`` -- a new one when ``host`` is missing or of another size -- and return that buffer.  Its contents
+        are valid once the current stream has passed this point; ``_parse_result`` reads them."""
+        dev = CorpusIndex._pack_result(sim, chunk, count, status, extra)
+        if host is None or host.numel() != dev.numel():
+            host = torch.empty(int(dev.numel()), dtype=torch.uint8, pin_memory=True)
+        host.copy_(dev, non_blocking=True)
+        return host
+
     def to_host(self, sim: torch.Tensor, chunk: torch.Tensor, count: torch.Tensor, status: torch.Tensor,
                 extra: torch.Tensor | None = None) -> tuple[np.ndarray, np.ndarray, np.ndarray, int] | tuple:
         """One device->host copy (pinned staging buffer) of a merged result plus the OR of the status words,
         then ONE stream synchronisation -- the only host sync of a search."""
         B, k = int(sim.shape[0]), int(sim.shape[1])
-        dev = self._pack_result(sim, chunk, count, status, extra)
-        n = int(dev.numel())
-        key = (n, _stream())      # one staging buffer per (size, stream): concurrent searches never share one
-        host = self._pinned.get(key)
-        if host is None:
-            if len(self._pinned) >= 16:
-                self._pinned.pop(next(iter(self._pinned)))
-            host = torch.empty(n, dtype=torch.uint8, pin_memory=True)
-            self._pinned[key] = host
-        host.copy_(dev, non_blocking=True)
+        n_extra = 0 if extra is None else int(extra.numel())
+        key = (B, k, n_extra, _stream())   # one staging buffer per (shape, stream): concurrent searches never share one
+        if key not in self._pinned and len(self._pinned) >= 16:
+            self._pinned.pop(next(iter(self._pinned)))
+        host = self._pinned[key] = self._enqueue_download(self._pinned.get(key), sim, chunk, count, status, extra)
         torch.cuda.current_stream().synchronize()
-        return self._parse_result(host.numpy(), B, k, 0 if extra is None else int(extra.numel()))
+        return self._parse_result(host.numpy(), B, k, n_extra)
 
 
-def next_overflow_attempt(local: "CorpusIndex", attempt: int, cap: int, base_flags: int) -> tuple[int, int]:
-    """Retry policy after a candidate-list overflow: odd attempts re-run with the thresholds the failed
-    pass wrote (``RL_FLAG_REUSE_THRESHOLDS``, same list size); even attempts start over with a list four
-    times as large (a larger workspace: thresholds are not carried over)."""
-    if attempt % 2 == 1:
-        return cap, base_flags | RL_FLAG_REUSE_THRESHOLDS
-    if cap <= 0:
-        cap = int(local.scan_stats().get("cand_cap", 1024))
-    if cap >= local.n_rows + 1024:
-        raise _lib.RagliteB200Error("candidate lists still overflow with a list as large as the shard")
-    return min(cap * 4, local.n_rows + 1024), base_flags & ~RL_FLAG_REUSE_THRESHOLDS
+MAX_SCAN_RUNS = 16
+
+
+def run_until_no_overflow(local: "CorpusIndex", run: Callable[[int, int], Any], *, flags: int = 0,
+                          cand_cap: int = 0) -> None:
+    """The candidate-overflow policy of every search.  ``run(flags, cand_cap)`` enqueues one search and returns its
+    status words (an int or an int tensor; on a sharded index the gathered words of every shard).  A candidate list
+    overflows on adversarial corpus order, or when more near-ties sit at the cut than the list holds; then odd
+    re-runs re-use the thresholds the failed pass wrote (``RL_FLAG_REUSE_THRESHOLDS``, same list size) and even
+    re-runs start over with a list four times as large (a larger workspace: thresholds are not carried over).  Each
+    shard grows its own list up to ``n_rows + 1024`` entries, which holds every row of the shard.  The loop ends on
+    the status alone or after ``MAX_SCAN_RUNS`` runs, so the ranks of a sharded index, which all see the same
+    gathered status, stop together; running out of runs raises ``RagliteB200Error``."""
+    cap, fl = cand_cap, flags
+    for n_run in range(1, MAX_SCAN_RUNS + 1):
+        overflow = run(fl, cap) & RL_STATUS_CAND_OVERFLOW
+        if not (bool(overflow.any()) if isinstance(overflow, torch.Tensor) else overflow):   # (a tensor synchronises)
+            return
+        if n_run % 2 == 1:
+            fl = flags | RL_FLAG_REUSE_THRESHOLDS
+        else:
+            if cap <= 0:
+                cap = int(local.scan_stats().get("cand_cap", 1024))
+            cap, fl = min(cap * 4, local.n_rows + 1024), flags & ~RL_FLAG_REUSE_THRESHOLDS
+    raise _lib.RagliteB200Error(f"candidate lists still overflow after {MAX_SCAN_RUNS} runs")
+
+
+def scan_gather_merge(  # noqa: PLR0913
+    index: Any, Q: torch.Tensor, *, k: int, num_hits: int, metric: str = "cosine", algo: str = "auto",
+    row_allowed: torch.Tensor | None = None, mask_has_tombstones: bool = False, flags: int = 0, cand_cap: int = 0,
+    sample_stride: int = 0, rank_first_limit: int | None = None,
+) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]:
+    """The search pipeline of a ``CorpusIndex`` (one shard) or a ``ShardedIndex``: scan the local shard into one
+    packed hit list, all-gather the lists of the R shards (none when R = 1), [rank-then-filter cut], merge the
+    gathered lists in place.  Everything is enqueued on the current stream, nothing synchronises.  Returns
+    ``(sim [B, k], chunk [B, k], count [B], status [R, B])``; every rank holds the same four tensors, and the
+    status words of every shard ride along in the one collective."""
+    local: CorpusIndex = getattr(index, "local", index)
+    R = getattr(index, "world", 1)
+    res = local.scan(Q, k=k, num_hits=num_hits, metric=metric, algo=algo, row_allowed=row_allowed,
+                     mask_has_tombstones=mask_has_tombstones, flags=flags, cand_cap=cand_cap, sample_stride=sample_stride)
+    B, H = int(res.hit_sim.shape[0]), int(res.hit_sim.shape[1])
+    allb = res.packed
+    if R > 1:
+        allb = torch.empty(R * res.packed.numel(), dtype=torch.uint8, device=res.packed.device)
+        dist.all_gather_into_tensor(allb, res.packed, group=index.group)
+    _, sim, count, status = hits_views(allb, R, B, H)
+    if rank_first_limit is not None:
+        count.copy_(limit_hits_to_nearest(index, Q, sim, count, k=k, num_hits=num_hits, metric=metric, algo=algo,
+                                          limit=rank_first_limit))
+    return (*merge_packed(allb, R, B, H, num_hits=num_hits, k=k), status)
 
 
 def search_to_host(  # noqa: PLR0913
@@ -857,29 +898,32 @@ def search_to_host(  # noqa: PLR0913
     local: CorpusIndex = getattr(index, "local", index)
     with local._lock, torch.cuda.device(local.device):
         mask = local.row_mask(chunk_ok)
-        cap, flags = 0, 0
+        kw = dict(k=k, num_hits=num_hits, metric=metric, algo=algo, row_allowed=mask, mask_has_tombstones=True)
         # Rank-then-filter branch (_search.py:122-143): first try to PROVE, from counters the filtered scan keeps
         # anyway, that fewer than `limit` rows of the whole corpus are as near as the worst filtered hit -- then
         # the filter-first answer is the answer and no second pass over the corpus is needed.
         fused = rank_first_limit is not None and mask is not None
-        for attempt in range(16):
-            sim, chunk, count, status = index.search_pipeline(
-                Q, k=k, num_hits=num_hits, metric=metric, algo=algo, row_allowed=mask, mask_has_tombstones=True,
-                flags=flags | (RL_FLAG_COUNT_UNFILTERED if fused else 0), cand_cap=cap,
-                rank_first_limit=None if fused else rank_first_limit)
+        out = None
+
+        def run(flags: int, cand_cap: int) -> int:
+            nonlocal fused, out
             if fused:
+                sim, chunk, count, status = index.search_pipeline(Q, **kw, flags=flags | RL_FLAG_COUNT_UNFILTERED,
+                                                                  cand_cap=cand_cap)
                 bound = index.sum_over_shards(local.unfiltered_bound().clamp(min=-1))
                 neg = index.sum_over_shards((local.unfiltered_bound() < 0).to(torch.int64))   # any shard that did not count
                 ids, sims, counts, st, ub = local.to_host(sim, chunk, count, status, torch.where(neg > 0, -1, bound))
-            else:
-                ids, sims, counts, st = local.to_host(sim, chunk, count, status)
-            if not st & RL_STATUS_CAND_OVERFLOW:
-                if fused and (ub.min() < 0 or ub.max() > rank_first_limit):
-                    fused = False       # not provable from the counters: run the explicit rank probe
-                    continue
-                return ids, sims, counts
-            cap, flags = next_overflow_attempt(local, attempt + 1, cap, 0)
-    raise _lib.RagliteB200Error("candidate lists still overflow with a list as large as the shard")
+                out = ids, sims, counts
+                if st & RL_STATUS_CAND_OVERFLOW or (ub.min() >= 0 and ub.max() <= rank_first_limit):
+                    return st
+                fused = False       # not provable from the counters: run the explicit rank probe
+            ids, sims, counts, st = local.to_host(*index.search_pipeline(Q, **kw, flags=flags, cand_cap=cand_cap,
+                                                                         rank_first_limit=rank_first_limit))
+            out = ids, sims, counts
+            return st
+
+        run_until_no_overflow(local, run)
+        return out
 
 
 class _SearchSlot:
@@ -951,12 +995,9 @@ def search_async(  # noqa: PLR0913
                 return PendingSearch(index, Q, kw, None, None, B, k, ready=out)
             with local._lock:
                 mask = local.row_mask(chunk_ok)
-                sim, chunk, count, status = index.search_pipeline(Q, k=k, num_hits=num_hits, metric=metric, algo=algo,
-                                                                  row_allowed=mask, mask_has_tombstones=True)
-                dev = local._pack_result(sim, chunk, count, status)
-            if slot.host is None or slot.host.numel() != dev.numel():
-                slot.host = torch.empty(int(dev.numel()), dtype=torch.uint8, pin_memory=True)
-            slot.host.copy_(dev, non_blocking=True)
+                out = index.search_pipeline(Q, k=k, num_hits=num_hits, metric=metric, algo=algo, row_allowed=mask,
+                                            mask_has_tombstones=True)
+                slot.host = local._enqueue_download(slot.host, *out)
             event = torch.cuda.Event()
             event.record(slot.stream)
         return PendingSearch(index, Q, kw, slot, event, B, k)

@@ -63,7 +63,8 @@ def _worker(rank: int, world: int, port: int, tmp: str) -> None:
     from synth import make_corpus, make_queries
 
     from oracle import vector_search as ovs
-    from raglite_b200._dist import gather_hits, shard_ranges
+    from raglite_b200._dist import shard_ranges
+    from raglite_b200._index import hits_views, new_scan_result
 
     E, off = make_corpus(600, (1, 9), 32, seed=3)
     Q = make_queries(E, 5, seed=4)
@@ -72,12 +73,26 @@ def _worker(rank: int, world: int, port: int, tmp: str) -> None:
     assert ranges[0][0] == 0 and ranges[-1][1] == len(off) - 1
     assert all(ranges[i][1] == ranges[i + 1][0] for i in range(world - 1))
     lo, hi = ranges[rank]
-    sim, chunk, count = shard_hits_numpy(E, off, Q, lo, hi, num_hits)
-    g_sim, g_chunk, g_count = gather_hits(torch.from_numpy(sim), torch.from_numpy(chunk), torch.from_numpy(count),
-                                          dist.group.WORLD)
-    assert g_sim.shape == (world, len(Q), num_hits)
-    assert torch.equal(g_sim[rank], torch.from_numpy(sim)) and torch.equal(g_chunk[rank], torch.from_numpy(chunk))
-    assert torch.equal(g_count[rank], torch.from_numpy(count))
+
+    def gather(sim, chunk, count, status=0):
+        """The search's one collective: this rank's hits and status words in one packed list (as the scan writes
+        it), all-gathered; returns the ``hits_views`` of the gathered buffer."""
+        res = new_scan_result(len(Q), num_hits, num_hits, k, "cpu")
+        res.hit_sim.copy_(torch.from_numpy(sim))
+        res.hit_chunk.copy_(torch.from_numpy(chunk))
+        res.hit_count.copy_(torch.from_numpy(count))
+        res.status.fill_(status)
+        allb = torch.empty(world * res.packed.numel(), dtype=torch.uint8)
+        dist.all_gather_into_tensor(allb, res.packed)
+        return hits_views(allb, world, len(Q), num_hits)
+
+    # Every rank's list arrives intact, and the status words ride along in the same all-gather.
+    g_chunk, g_sim, g_count, g_status = gather(*shard_hits_numpy(E, off, Q, lo, hi, num_hits), status=rank)
+    assert g_sim.shape == (world, len(Q), num_hits) and g_status.shape == (world, len(Q))
+    for r in range(world):
+        sim, chunk, count = shard_hits_numpy(E, off, Q, *ranges[r], num_hits)
+        assert torch.equal(g_sim[r], torch.from_numpy(sim)) and torch.equal(g_chunk[r], torch.from_numpy(chunk))
+        assert torch.equal(g_count[r], torch.from_numpy(count)) and g_status[r].tolist() == [r] * len(Q)
     merged = merge_numpy(g_sim.numpy(), g_chunk.numpy(), g_count.numpy(), num_hits, k)
     for b, q in enumerate(Q):
         ref_ids, ref_sims, _ = ovs.vector_search_sql(E, off, q, num_results=k, f64=True)
@@ -102,13 +117,14 @@ def _worker(rank: int, world: int, port: int, tmp: str) -> None:
     tagged = np.zeros(len(off) - 1, dtype=bool)
     tagged[order0[len(order0) // 2:]] = True       # far from query 0 ...
     tagged[order0[[0, 3, 7]]] = True               # ... plus three near chunks
-    sim, chunk, count = shard_hits_numpy(E, off, Q, lo, hi, num_hits, allowed_chunks=tagged)
-    g_sim, g_chunk, g_count = gather_hits(torch.from_numpy(sim), torch.from_numpy(chunk), torch.from_numpy(count),
-                                          dist.group.WORLD)
+    g_chunk, g_sim, g_count, _ = gather(*shard_hits_numpy(E, off, Q, lo, hi, num_hits, allowed_chunks=tagged))
     sharded = ShardedIndex(FakeShard(), dist.group.WORLD)
-    kept = limit_hits_to_nearest(sharded, torch.from_numpy(Q), g_sim, g_count, k=k, num_hits=num_hits, metric="cosine",
-                                 limit=limit)
-    merged = merge_numpy(g_sim.numpy(), g_chunk.numpy(), kept.numpy(), num_hits, k)
+    g_count.copy_(limit_hits_to_nearest(sharded, torch.from_numpy(Q), g_sim, g_count, k=k, num_hits=num_hits,
+                                        metric="cosine", limit=limit))
+    both = [torch.zeros_like(g_count) for _ in range(world)]
+    dist.all_gather(both, g_count.contiguous())
+    assert torch.equal(both[0], both[1]), "every rank must keep the same hits"
+    merged = merge_numpy(g_sim.numpy(), g_chunk.numpy(), g_count.numpy(), num_hits, k)
     changed = 0
     for b, q in enumerate(Q):
         ref_ids, ref_sims, _ = ovs.vector_search_sql(E, off, q, num_results=k, allowed_chunks=tagged, f64=True,
@@ -118,12 +134,6 @@ def _worker(rank: int, world: int, port: int, tmp: str) -> None:
         first_ids, _, _ = ovs.vector_search_sql(E, off, q, num_results=k, allowed_chunks=tagged, f64=True)
         changed += ref_ids.tolist() != first_ids.tolist()
     assert changed >= 1, "the cut must change at least query 0's answer"
-
-    # The status words ride along in the same all-gather (one collective per search).
-    st = torch.full((len(Q),), rank, dtype=torch.int32)
-    g4 = gather_hits(torch.from_numpy(sim), torch.from_numpy(chunk), torch.from_numpy(count), dist.group.WORLD, st)
-    assert len(g4) == 4 and g4[3].shape == (world, len(Q)) and g4[3][1].tolist() == [1] * len(Q)
-    assert torch.equal(g4[0], g_sim) and torch.equal(g4[1], g_chunk)
 
     # ADVICE r1: dot metric, shards whose largest row norms differ -- the bisection bracket must be the
     # same on every rank (max over shards), or the summed counts mix different thresholds.
@@ -151,16 +161,14 @@ def _worker(rank: int, world: int, port: int, tmp: str) -> None:
             sim_[b, :len(o_)] = (1.0 - d_[o_]).astype(np.float32); ch_[b, :len(o_)] = r2c[o_]; cn_[b] = len(o_)
         return sim_, ch_, cn_
 
-    sim, chunk, count = shard_hits_dot(tagged)
-    g_sim, g_chunk, g_count = gather_hits(torch.from_numpy(sim), torch.from_numpy(chunk), torch.from_numpy(count),
-                                          dist.group.WORLD)
+    g_chunk, g_sim, g_count, _ = gather(*shard_hits_dot(tagged))
     sharded = ShardedIndex(FakeDotShard(), dist.group.WORLD)
-    kept = limit_hits_to_nearest(sharded, torch.from_numpy(Q), g_sim, g_count, k=k, num_hits=num_hits, metric="dot",
-                                 limit=limit)
-    both = [torch.zeros_like(kept) for _ in range(world)]
-    dist.all_gather(both, kept)
+    g_count.copy_(limit_hits_to_nearest(sharded, torch.from_numpy(Q), g_sim, g_count, k=k, num_hits=num_hits,
+                                        metric="dot", limit=limit))
+    both = [torch.zeros_like(g_count) for _ in range(world)]
+    dist.all_gather(both, g_count.contiguous())
     assert torch.equal(both[0], both[1]), "every rank must keep the same hits"
-    merged = merge_numpy(g_sim.numpy(), g_chunk.numpy(), kept.numpy(), num_hits, k)
+    merged = merge_numpy(g_sim.numpy(), g_chunk.numpy(), g_count.numpy(), num_hits, k)
     for b, q in enumerate(Q):
         ref_ids, ref_sims, _ = ovs.vector_search_sql(Ed, off, q, num_results=k, metric="dot", allowed_chunks=tagged, f64=True,
                                                      filter_first_max=0, rank_first_limit=limit)
@@ -190,7 +198,7 @@ def _worker(rank: int, world: int, port: int, tmp: str) -> None:
     Path(tmp, f"ok{rank}").write_text("ok")
 
 
-def test_two_rank_gather_and_merge(tmp_path):
+def test_two_rank_packed_gather_and_merge(tmp_path):
     port = 29500 + (os.getpid() % 2000)
     mp.spawn(_worker, args=(2, port, str(tmp_path)), nprocs=2, join=True)
     assert (tmp_path / "ok0").exists() and (tmp_path / "ok1").exists()
@@ -208,9 +216,10 @@ def test_shard_ranges_balance_and_edges():
     assert shard_ranges(np.array([0, 5]), 4) == [(0, 0), (0, 0), (0, 0), (0, 1)] or sum(b - a for a, b in shard_ranges(np.array([0, 5]), 4)) == 1
 
 
-def test_pack_unpack_roundtrip():
+def test_hits_views_roundtrip():
+    """Hit lists written through one scan result's views and laid end to end read back through ``hits_views``."""
     sys.path.insert(0, str(ROOT))
-    from raglite_b200._dist import pack_hits, unpack_hits
+    from raglite_b200._index import hits_views, new_scan_result
 
     g = torch.Generator().manual_seed(0)
     B, H, R = 3, 7, 2
@@ -219,7 +228,11 @@ def test_pack_unpack_roundtrip():
         s = torch.randn((B, H), generator=g)
         c = torch.randint(0, 1 << 40, (B, H), generator=g)
         n = torch.randint(0, H, (B,), generator=g, dtype=torch.int32)
-        bufs.append(pack_hits(s, c, n)); want.append((s, c, n))
-    sim, chunk, count = unpack_hits(torch.cat(bufs), R, B, H)
+        st = torch.randint(0, 4, (B,), generator=g, dtype=torch.int32)
+        res = new_scan_result(B, H, H, 1, "cpu")
+        res.hit_sim.copy_(s); res.hit_chunk.copy_(c); res.hit_count.copy_(n); res.status.copy_(st)
+        bufs.append(res.packed); want.append((s, c, n, st))
+    chunk, sim, count, status = hits_views(torch.cat(bufs), R, B, H)
     for r in range(R):
         assert torch.equal(sim[r], want[r][0]) and torch.equal(chunk[r], want[r][1]) and torch.equal(count[r], want[r][2])
+        assert torch.equal(status[r], want[r][3])

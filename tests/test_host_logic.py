@@ -253,5 +253,10 @@ def test_scan_checked_resolves_or_raises():
     with pytest.raises(_lib.RagliteB200Error):
         idx.scan_checked(Q, k=1, num_hits=2)
     assert max(c[1] for c in idx.calls) == 10_000 + 1024
+    # ... and the last run's status is read: a list that clears on the last allowed run is a result, not an error
+    from raglite_b200._index import MAX_SCAN_RUNS
+
+    idx = fake_index(lambda n, B, kw: [1] * B if n < MAX_SCAN_RUNS else [0] * B, n_rows=10_000)
+    assert idx.scan_checked(Q, k=1, num_hits=2).hit_sim[0, 0] == MAX_SCAN_RUNS and len(idx.calls) == MAX_SCAN_RUNS
 
 
