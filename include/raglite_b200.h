@@ -342,6 +342,30 @@ int rl_xenc_encode(const rl_xenc_weights* w, const int32_t* input_ids, const int
 int rl_xenc_encode_attention(const void* qkv, const int32_t* cu_seqlens, int P, int T, int max_len, int hidden, int n_heads,
                              void* ctx, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- BM25 keyword search: _search.py:203-225 (DuckDB fts match_bm25 at its defaults) -------------------------------
+ * Inverted index over the chunk bodies (device arrays): term_off int64 [n_terms + 1], a term-major postings CSR whose
+ * doc int32 / tf int32 [P] are sorted by chunk within each term; doc_len int32 [n_chunks] = terms left after stop-word
+ * removal.  chunk_alive / chunk_mask: uint8 [n_chunks] or NULL (= every chunk).
+ *
+ * rl_bm25_stats: over the chunks with chunk_alive set, df[t] (int32 [n_terms], may be NULL) = number of such chunks that
+ * contain t, idf[t] (float64) = log10((N - df + 0.5) / (df + 0.5) + 1), corpus (float64 [3]) = {N, sum of doc_len,
+ * avgdl = sum / N}.  Every double is rounded as the SQL expression reads (no contraction). */
+int rl_bm25_stats(const int64_t* term_off, const int32_t* doc, const int32_t* doc_len, const uint8_t* chunk_alive,
+                  int64_t n_terms, int64_t n_chunks, int32_t* df, double* idf, double* corpus, void* stream);
+/* Workspace that lets the top-k call below score `group` queries at a time: group * n_chunks * 8 bytes. */
+size_t rl_bm25_workspace_bytes(int64_t n_chunks, int group);
+/* rl_bm25_topk: B queries, query b = the term ids q_terms[q_off[b] .. q_off[b+1]) (device int32; distinct, ascending --
+ * the order the per-chunk sum runs in).  score(d) = sum over the query terms t in d of
+ * idf[t] * (tf * (k1 + 1) / (tf + k1 * (1 - b + b * (doc_len[d] / avgdl)))), float64, rounded as written.  A chunk is a
+ * result when it contains a query term and chunk_mask allows it (tombstones AND the metadata filter: the mask changes
+ * nothing in idf / avgdl, which come from rl_bm25_stats).  Outputs, best first by (score desc, chunk asc):
+ * out_chunk int64 [B, k] (-1 padded), out_score float64 [B, k] (-inf padded), out_count int32 [B].  1 <= k <= 4096
+ * (RL_MAX_SURVIVORS); the queries are scored in groups of as many as the workspace holds (at least one). */
+int rl_bm25_topk(const int64_t* term_off, const int32_t* doc, const int32_t* tf, const int32_t* doc_len, const double* idf,
+                 const double* corpus, int64_t n_terms, int64_t n_chunks, const uint8_t* chunk_mask, const int32_t* q_off,
+                 const int32_t* q_terms, int B, int k, double k1, double b, int64_t* out_chunk, double* out_score,
+                 int32_t* out_count, void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

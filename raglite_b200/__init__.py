@@ -1,8 +1,9 @@
 """raglite_b200 -- H100-native (sm_90a) implementation of RAGLite's retrieval hot path.
 
 Drop-in surface (reference ``raglite/__init__.py`` names for this path): ``RAGLiteConfig``,
-``vector_search``, ``rerank_chunks``, ``embed_strings``; plus the device-resident ``CorpusIndex`` /
-``ShardedIndex`` that replace the database for this path and the batched ``vector_search_batch``; and
+``vector_search``, ``keyword_search``, ``hybrid_search``, ``rerank_chunks``, ``embed_strings``; plus the device-resident ``CorpusIndex`` /
+``ShardedIndex`` that replace the database for this path and the batched ``vector_search_batch`` /
+``keyword_search_batch``; and
 ``TokenEmbedderEngine``, the embedding model's encoder on the GPU behind ``embed_strings`` / ``embed_queries``.
 """
 
@@ -14,6 +15,8 @@ from ._search import (
     ChunkSpan,
     collate_spans_device,
     hybrid_search,
+    keyword_search,
+    keyword_search_batch,
     reciprocal_rank_fusion,
     register_keyword_search,
     rerank_chunks,
@@ -36,6 +39,8 @@ __all__ = [
     "TokenEmbedderEngine",
     "collate_spans_device",
     "hybrid_search",
+    "keyword_search",
+    "keyword_search_batch",
     "register_keyword_search",
     "rrf_fuse_device",
     "embed_queries",

@@ -191,6 +191,7 @@ class CorpusIndex:
         self._meta_inv: dict[tuple[str, Any], np.ndarray] | None = None   # (key, value) -> chunk indices
         self._meta_inv_chunks = 0                      # chunks covered by _meta_inv
         self._filter_cache: dict[Any, tuple[torch.Tensor, int]] = {}      # filter -> (chunk_ok uint8 [C], matching live rows)
+        self._keyword: Any | None = None               # BM25 postings of the chunk bodies (keyword_index), built on demand
         self._pinned: dict[Any, torch.Tensor] = {}     # result staging buffers (pinned host memory) by (size, stream)
         self._slots: list[Any] = []                    # streams + pinned buffers of the asynchronous searches (search_async)
         self.last_params: ScanParams | None = None
@@ -469,6 +470,8 @@ class CorpusIndex:
                     setattr(self, name, [x for x, ok in zip(have, keep, strict=True) if ok])
             self.n_rows, self.n_chunks = dst, int(keep.sum())
             self.max_vecs = int(counts.max()) if len(counts) else 1
+            if self._keyword is not None:
+                self._keyword.compact(keep)
             self._chunk_alive = np.ones(self.n_chunks, dtype=bool)
             self._chunk_pos, self._alive = None, None
             for name in self._ROW_ARRAYS:
@@ -568,6 +571,26 @@ class CorpusIndex:
         self._filter_cache.clear()
         self._n_live_rows = None
         self._span_tables = None
+        if self._keyword is not None:
+            self._keyword.stale = True
+
+    def keyword_index(self) -> Any:
+        """The BM25 index over ``chunks[i].body`` (``_keyword.KeywordIndex``), brought up to date with the table:
+        built on the first call, appended chunks analysed, statistics recomputed over the live chunks after any
+        change.  Needs the ``Chunk`` records (``ValueError`` otherwise, as ``retrieve_chunks``)."""
+        if self.chunks is None:
+            raise ValueError("The registered index holds no chunk texts")
+        from ._keyword import KeywordIndex
+
+        with self._lock, torch.cuda.device(self.device):
+            if self._keyword is None:
+                self._keyword = KeywordIndex(self.device)
+            kw = self._keyword
+            if kw.n_chunks < self.n_chunks:
+                kw.extend([c.body for c in self.chunks[kw.n_chunks:]])
+            if kw.stale:
+                kw.refresh(self._chunk_alive)
+            return kw
 
     def span_tables(self) -> dict[str, torch.Tensor]:
         """Device tables ``rl_span_collate`` needs (built once per index change from the ``Chunk`` records):

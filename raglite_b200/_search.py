@@ -1,8 +1,8 @@
-"""Drop-in ``vector_search`` / ``rerank_chunks`` over the device-resident index.
+"""Drop-in ``vector_search`` / ``keyword_search`` / ``rerank_chunks`` over the device-resident index.
 
-Signatures follow the reference (``raglite/_search.py:36-43`` and ``:364-366``); the arithmetic that
-the reference delegates to DuckDB SQL runs in the CUDA library instead.  ``vector_search_batch`` is
-the batched entry the benchmark configs use (the reference API is single-query, ``_search.py:54-56``).
+Signatures follow the reference (``raglite/_search.py:36-43``, ``:156-162`` and ``:364-366``); the arithmetic that
+the reference delegates to DuckDB SQL runs in the CUDA library instead.  ``vector_search_batch`` /
+``keyword_search_batch`` are the batched entries (the reference API is single-query, ``_search.py:54-56``).
 """
 
 from __future__ import annotations
@@ -230,6 +230,68 @@ def rerank_chunks(
     return chunks
 
 
+# ---- BM25 keyword search: the DuckDB branch of _search.py:156-230 ------------------------------------------------
+def keyword_search_batch(
+    queries: Sequence[str],
+    *,
+    num_results: int = 3,
+    metadata_filter: MetadataFilter | None = None,
+    config: RAGLiteConfig | None = None,
+    index: Any | None = None,
+) -> tuple[np.ndarray, np.ndarray, np.ndarray]:
+    """Batched ``keyword_search``: BM25 as DuckDB's ``fts_main_chunk.match_bm25(id, query)`` computes it at its
+    defaults, over the ``Chunk`` bodies of the index (``CorpusIndex.keyword_index``; ``_fts`` has the text analysis).
+
+    Returns host arrays ``(chunk_index [B, k] int64 (-1 padded), score [B, k] float64 (-inf padded), count [B])``,
+    ordered by descending score, ties by ascending chunk index.  The metadata filter only decides which chunks can be
+    results: ``N``, ``avgdl`` and ``df`` always cover every live chunk, as the reference's ``WHERE`` around the macro
+    does.  Host work per call: analysing the queries, one upload, the kernel launches, one pinned download and one
+    stream synchronisation."""
+    from ._keyword import MAX_RESULTS
+
+    config = config or RAGLiteConfig()
+    if str(config.db_url).startswith("postgresql"):
+        raise NotImplementedError("keyword_search on PostgreSQL ranks with ts_rank over to_tsvector('simple', body), "
+                                  "a different formula; only the DuckDB branch (match_bm25) is implemented")
+    index = index if index is not None else get_index(config)
+    if index is None:
+        raise ValueError(f"No index registered for db_url={config.db_url!r}; use raglite_b200.register_index")
+    if hasattr(index, "group"):
+        raise NotImplementedError("keyword_search on a ShardedIndex: document frequencies need the vocabulary of every rank")
+    local: CorpusIndex = index
+    queries = list(queries)
+    k = int(num_results)
+    if k < 0 or k > MAX_RESULTS:
+        raise ValueError(f"num_results={k} is outside [0, {MAX_RESULTS}]")
+    B = len(queries)
+    empty = (np.full((B, k), -1, np.int64), np.full((B, k), -np.inf, np.float64), np.zeros(B, np.int32))
+    if B == 0 or k == 0 or local.n_live_chunks == 0:
+        return empty
+    with local._lock:
+        kw = local.keyword_index()
+        chunk_ok, _ = _filter_on_device(local, _adapt_metadata(metadata_filter))
+        return kw.topk_to_host(queries, k=k, chunk_mask=chunk_ok if chunk_ok is not None else kw.alive)
+
+
+def keyword_search(
+    query: str,
+    *,
+    num_results: int = 3,
+    metadata_filter: MetadataFilter | None = None,
+    config: RAGLiteConfig | None = None,
+) -> tuple[list[ChunkId], list[float]]:
+    """Search chunks with BM25 keyword search -- drop-in for ``raglite.keyword_search`` (``_search.py:156-230``, the
+    DuckDB branch): the chunks that contain at least one query term, best ``num_results`` first."""
+    config = config or RAGLiteConfig()
+    if config.self_query and isinstance(query, str):
+        raise NotImplementedError("self_query needs an LLM and is outside the accelerated hot path")
+    index = get_index(config)
+    ids, scores, counts = keyword_search_batch([query], num_results=num_results, metadata_filter=metadata_filter,
+                                               config=config, index=index)
+    n = int(counts[0])
+    return ([index.chunk_id_of(index.chunk_base + int(c)) for c in ids[0, :n]], [float(s) for s in scores[0, :n]])
+
+
 # ---- the steps right after the hot path (SURVEY.md section 8f-3) ------------------------------------------
 @dataclass
 class ChunkSpan:
@@ -258,9 +320,9 @@ _KEYWORD_SEARCH: dict[str, Any] = {}
 
 
 def register_keyword_search(config_or_url: Any, fn: Any) -> None:
-    """Provide the BM25 keyword search for a database (the reference runs it as SQL full-text search inside
-    DuckDB / PostgreSQL, ``_search.py:156-230`` -- storage-engine territory, out of scope here): any callable with
-    ``keyword_search``'s signature ``(query, *, num_results, metadata_filter, config) -> (chunk_ids, scores)``."""
+    """Replace the keyword search ``hybrid_search`` uses for a database (by default the device ``keyword_search``):
+    any callable with ``keyword_search``'s signature ``(query, *, num_results, metadata_filter, config) ->
+    (chunk_ids, scores)`` -- e.g. one that queries PostgreSQL, whose ``ts_rank`` branch is not implemented here."""
     _KEYWORD_SEARCH[str(getattr(config_or_url, "db_url", config_or_url))] = fn
 
 
@@ -319,14 +381,13 @@ def hybrid_search(  # noqa: PLR0913
     query: str, *, num_results: int = 3, oversample: int = 2, vector_search_weight: float = 0.75,
     keyword_search_weight: float = 0.25, metadata_filter: MetadataFilter | None = None, config: RAGLiteConfig | None = None,
 ) -> tuple[list[ChunkId], list[float]]:
-    """Drop-in ``hybrid_search`` (``_search.py:257-280``): vector search on the device index, the registered keyword
-    search (``register_keyword_search``), Reciprocal Rank Fusion of the two rankings on the device."""
+    """Drop-in ``hybrid_search`` (``_search.py:257-280``): vector search on the device index, keyword search -- the
+    callable registered with ``register_keyword_search`` if there is one, the device ``keyword_search`` otherwise --
+    and Reciprocal Rank Fusion of the two rankings on the device."""
     config = config or RAGLiteConfig()
-    keyword_search = _KEYWORD_SEARCH.get(str(config.db_url))
-    if keyword_search is None:
-        raise ValueError("hybrid_search needs a keyword search for this database: raglite_b200.register_keyword_search")
+    ks = _KEYWORD_SEARCH.get(str(config.db_url), keyword_search)
     vs_ids, _ = vector_search(query, num_results=oversample * num_results, metadata_filter=metadata_filter, config=config)
-    ks_ids, _ = keyword_search(query, num_results=oversample * num_results, metadata_filter=metadata_filter, config=config)
+    ks_ids, _ = ks(query, num_results=oversample * num_results, metadata_filter=metadata_filter, config=config)
     ids, score = reciprocal_rank_fusion([vs_ids, list(ks_ids)], weights=[vector_search_weight, keyword_search_weight])
     return ids[:num_results], score[:num_results]
 
@@ -431,8 +492,8 @@ def search_and_rerank_chunks(  # noqa: PLR0913
     config: RAGLiteConfig | None = None, metadata_filter: MetadataFilter | None = None,
 ) -> list[Chunk]:
     """Search ``oversample * num_results`` chunks, rerank, keep ``num_results`` (``_search.py:400-413``).
-    The reference defaults ``search`` to hybrid search; keyword search is out of scope here, so the
-    default is ``vector_search``."""
+    The default ``search`` is ``vector_search``; the reference defaults to hybrid search, which
+    ``search=raglite_b200.hybrid_search`` gives."""
     search = search or vector_search
     chunk_ids, _ = search(query, num_results=oversample * num_results, metadata_filter=metadata_filter, config=config)
     return rerank_chunks(query, chunk_ids, config=config)[:num_results]
@@ -442,7 +503,8 @@ def search_and_rerank_chunk_spans(  # noqa: PLR0913
     query: str, *, num_results: int = 8, oversample: int = 4, neighbors: tuple[int, ...] | None = (-1, 1),
     search: Any = None, config: RAGLiteConfig | None = None, metadata_filter: MetadataFilter | None = None,
 ) -> list[ChunkSpan]:
-    """``search_and_rerank_chunks`` followed by span collation (``_search.py:416-433``)."""
+    """``search_and_rerank_chunks`` followed by span collation (``_search.py:416-433``); as there, the default ``search``
+    is ``vector_search`` and ``search=raglite_b200.hybrid_search`` gives the reference's default."""
     chunks = search_and_rerank_chunks(query, num_results=num_results, oversample=oversample, search=search,
                                       config=config, metadata_filter=metadata_filter)
     return retrieve_chunk_spans(chunks, neighbors=neighbors, config=config)
