@@ -163,7 +163,8 @@ int rl_maxsim_stats(const rl_scan_params* p, const void* workspace, rl_scan_stat
  * the rows counted against the thresholds (allowed ones = the candidate count, masked ones = the extra counter)
  * plus the whole sample are a superset.  bound <= 1 000 000 proves that the filter-first answer is also the
  * rank-then-filter answer, without the second pass over the corpus rl_maxsim_count_at_least needs.  Returns
- * RL_EUNSUPPORTED when the last call did not count (fp32 scan, flag not set). */
+ * RL_EUNSUPPORTED when the last call did not count (fp32 scan, flag not set).  An empty shard (p->n_rows == 0)
+ * gets bound 0 without the workspace being read: rl_maxsim_topk writes nothing there for it. */
 int rl_maxsim_unfiltered_bound(const rl_scan_params* p, const void* workspace, int64_t* bound, void* stream);
 
 /* Rank probe for the reference's rank-then-filter metadata branch (_search.py:122-143, which keeps the

@@ -52,10 +52,11 @@ class ShardedIndex:
         self.world = dist.get_world_size(group) if group is not None else 1
         self.rank = dist.get_rank(group) if group is not None else 0
         self.shard_chunk_ids: list[list[str] | None] | None = None
+        self._any_chunk_ids = False   # some shard held chunk ids at the last gather of the tables
         self.last_status: torch.Tensor | None = None
         self.ranges: list[tuple[int, int]] = []
         if hasattr(local, "chunk_base"):
-            self.refresh()
+            self.refresh(chunk_ids=True)   # hits owned by other ranks resolve to their ids from the first search on
             local._shard_guard = self
 
     @staticmethod
@@ -66,7 +67,8 @@ class ShardedIndex:
     def refresh(self, *, chunk_ids: bool = False) -> None:
         """(Collective) re-gather ``(chunk_base, n_chunks)`` of every shard -- after ``append`` / ``compact`` on
         any rank -- and check that the ranges are disjoint; ``chunk_ids=True`` also gathers each shard's
-        chunk-id table so that ``chunk_id_of`` resolves hits owned by other ranks."""
+        chunk-id table so that ``chunk_id_of`` resolves hits owned by other ranks.  The constructor gathers the
+        tables; after ``append`` / ``compact`` on any rank call ``refresh(chunk_ids=True)`` on every rank."""
         mine = (int(self.local.chunk_base), int(self.local.n_chunks))
         if self.group is not None and self.world > 1:
             got: list[Any] = [None] * self.world
@@ -85,6 +87,7 @@ class ShardedIndex:
                 self.shard_chunk_ids = tables
             else:
                 self.shard_chunk_ids = [self.local.chunk_ids]
+            self._any_chunk_ids = any(t is not None for t in self.shard_chunk_ids)
 
     def check_local_growth(self, new_n_chunks: int) -> None:
         """Called by ``CorpusIndex.append``: the shard must stay below the next shard's base."""
@@ -95,7 +98,6 @@ class ShardedIndex:
                 f"appending to shard {self.rank} would run its global chunk indices [{base}, {base + new_n_chunks}) into "
                 f"the next shard's range starting at {nxt}; build the shards with spaced bases (ShardedIndex.shard_bases) "
                 "to let them follow inserts")
-        self.shard_chunk_ids = None   # stale until the next refresh(chunk_ids=True)
 
     def search_pipeline(self, Q: torch.Tensor, **kw: Any) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]:
         """``scan_gather_merge`` over the shards of the group; ``last_status`` keeps the gathered status words."""
@@ -141,13 +143,21 @@ class ShardedIndex:
         return x
 
     def chunk_id_of(self, global_chunk: int) -> str:
+        """The chunk id of a global chunk index: this rank's own chunks from the shard itself, the other ranks' from
+        the tables the last ``refresh(chunk_ids=True)`` gathered.  An index whose shards hold no chunk ids names a
+        chunk by its number (``str``, as ``CorpusIndex.chunk_id_of``).  A chunk outside every gathered table -- one
+        that another rank appended after that refresh -- raises ``LookupError`` rather than pass a number off as an
+        id: call ``refresh(chunk_ids=True)`` on every rank after ``append`` or ``compact``."""
         g = int(global_chunk)
-        if self.shard_chunk_ids is not None:
-            for r, (base, n) in enumerate(self.ranges):
-                table = self.shard_chunk_ids[r]
-                if base <= g < base + n and table is not None:
-                    return table[g - base]
         lo = self.local.chunk_base
         if self.local.chunk_ids is not None and lo <= g < lo + self.local.n_chunks:
             return self.local.chunk_ids[g - lo]
+        if self.shard_chunk_ids is not None:
+            for r, (base, n) in enumerate(self.ranges):
+                table = self.shard_chunk_ids[r]
+                if table is not None and base <= g < base + min(n, len(table)):
+                    return table[g - base]
+        if self._any_chunk_ids or self.local.chunk_ids is not None:
+            raise LookupError(f"global chunk {g} is in no chunk-id table gathered by the last refresh: call "
+                              "refresh(chunk_ids=True) on every rank after append or compact")
         return str(g)

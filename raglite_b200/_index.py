@@ -300,8 +300,8 @@ class CorpusIndex:
         if self.n_rows:
             st = self.stats.cpu().numpy()
             self._rows_unit_scale = bool(0.0 < st[2] <= 2.0 and st[1] <= 1024.0 and st[3] == 0.0)
-        if self.storage == "fp16":
-            self._fp16_cosine_ok = self._rows_unit_scale
+        if self.storage == "fp16":   # an empty shard holds no row too small for the cosine fast path
+            self._fp16_cosine_ok = self._rows_unit_scale or self.n_rows == 0
 
     @property
     def rows_unit_scale(self) -> bool:

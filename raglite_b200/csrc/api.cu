@@ -81,9 +81,12 @@ int make_layout(const rl_scan_params* p, int sm_count, Layout* L) {
   const bool tc_ok = wgmma_scan_supported(p);
   if (algo == RL_ALGO_AUTO) algo = tc_ok ? RL_ALGO_TCGEN05 : RL_ALGO_FP32;
   RL_REQUIRE(algo == RL_ALGO_FP32 || algo == RL_ALGO_TCGEN05, RL_EINVAL, "unknown algo %d", p->algo);
-  RL_REQUIRE(p->e_dtype == 0 || algo == RL_ALGO_TCGEN05, RL_EUNSUPPORTED,
+  // An empty shard (a sharded corpus with fewer chunks than ranks, or emptied by compact) scans nothing: every
+  // entry point returns before its first launch, so it takes any storage and algo.
+  const bool empty = p->n_rows == 0;
+  RL_REQUIRE(empty || p->e_dtype == 0 || algo == RL_ALGO_TCGEN05, RL_EUNSUPPORTED,
              "float16 storage needs the tensor-core scan (d %% 8 == 0, ld %% 8 == 0, 16-byte aligned E)");
-  RL_REQUIRE(algo != RL_ALGO_TCGEN05 || tc_ok, RL_EUNSUPPORTED,
+  RL_REQUIRE(empty || algo != RL_ALGO_TCGEN05 || tc_ok, RL_EUNSUPPORTED,
              "RL_ALGO_TCGEN05 needs d %% 4 == 0, ld %% 4 == 0, 16-byte aligned E and a supported metric");
   L->algo = algo;
 
@@ -488,11 +491,16 @@ __global__ void unfiltered_bound_kernel(const Header* hdr, const int32_t* cand_c
 }  // namespace rl
 
 extern "C" int rl_maxsim_unfiltered_bound(const rl_scan_params* p, const void* workspace, int64_t* bound, void* stream) {
-  RL_REQUIRE(p && workspace && bound, RL_EINVAL, "rl_maxsim_unfiltered_bound: null pointer");
+  RL_REQUIRE(p && bound, RL_EINVAL, "rl_maxsim_unfiltered_bound: null pointer");
   Layout L;
   int rc = make_layout(p, 132, &L);
   if (rc != RL_OK) return rc;
   if (p->B == 0) return RL_OK;
+  if (p->n_rows == 0) {  // empty shard: rl_maxsim_topk wrote nothing to the workspace, and no row can be near
+    RL_CUDA_CHECK(cudaMemsetAsync(bound, 0, (size_t)p->B * sizeof(int64_t), (cudaStream_t)stream));
+    return RL_OK;
+  }
+  RL_REQUIRE(workspace, RL_EINVAL, "rl_maxsim_unfiltered_bound: null workspace");
   const unsigned char* ws = static_cast<const unsigned char*>(workspace);
   unfiltered_bound_kernel<<<(p->B + 127) / 128, 128, 0, (cudaStream_t)stream>>>(
       reinterpret_cast<const Header*>(ws + L.off_hdr), reinterpret_cast<const int32_t*>(ws + L.off_cnt),
