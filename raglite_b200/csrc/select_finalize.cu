@@ -393,7 +393,9 @@ __global__ void __launch_bounds__(kSelThreads) select_kernel(const SelectArgs a)
 }
 
 // ---- finalize --------------------------------------------------------------------------------------
-__device__ __forceinline__ float exact_sim(int metric, double dot, double ne, double nq) {
+// d2 = sum (e - q)^2, accumulated directly: ne + nq - 2 dot cancels to its rounding error for a row that (nearly)
+// duplicates a query of large norm.
+__device__ __forceinline__ float exact_sim(int metric, double dot, double ne, double nq, double d2) {
   if (metric == RL_METRIC_COSINE) {
     double s = dot / sqrt(ne * nq);
     s = fmin(1.0, fmax(-1.0, s));
@@ -401,7 +403,6 @@ __device__ __forceinline__ float exact_sim(int metric, double dot, double ne, do
     return 1.0f - dist;                  // sim = 1 - dist (_search.py:72)
   }
   if (metric == RL_METRIC_DOT) return 1.0f - (float)(-dot);
-  const double d2 = fmax(0.0, ne + nq - 2.0 * dot);
   return 1.0f - (float)sqrt(d2);
 }
 
@@ -543,9 +544,41 @@ __global__ void __launch_bounds__(kSelThreads) finalize_kernel(const FinalizeArg
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
   const double nq = f.q_sq[b];
   const bool vec = (f.d % 4 == 0) && (f.ld % 4 == 0) && ((reinterpret_cast<uintptr_t>(f.E) & 15) == 0);
+  // l2 needs only d2 = sum (e - q)^2, cosine and dot only dot and ne: one loop each, chosen once per row (the metric
+  // is uniform per launch), so the cosine / dot loop is the one it always was.
+  const bool l2 = f.metric == RL_METRIC_L2;
   auto exact_row_sim = [&](int32_t row) -> float {   // all 32 lanes call it; every lane gets the result
     const float* e = f.E + (int64_t)row * f.ld;
-    double dot = 0.0, ne = 0.0;
+    double dot = 0.0, ne = 0.0, d2 = 0.0;
+    if (l2) {
+      if (f.e_f16) {
+        const __half* eh = reinterpret_cast<const __half*>(f.E) + (int64_t)row * f.ld;
+        for (int c = lane * 8; c < f.d; c += 256) {
+          const uint4 v = __ldg(reinterpret_cast<const uint4*>(eh + c));
+          const __half2* h = reinterpret_cast<const __half2*>(&v);
+#pragma unroll
+          for (int k2 = 0; k2 < 4; ++k2) {
+            const float2 ev = __half22float2(h[k2]);
+            const double tx = (double)ev.x - qv[c + 2 * k2], ty = (double)ev.y - qv[c + 2 * k2 + 1];
+            d2 += tx * tx + ty * ty;
+          }
+        }
+      } else if (vec) {
+        for (int c = lane * 4; c < f.d; c += 128) {
+          const float4 ev = __ldg(reinterpret_cast<const float4*>(e + c));
+          const float4 qq = *reinterpret_cast<const float4*>(qv + c);
+          const double tx = (double)ev.x - qq.x, ty = (double)ev.y - qq.y, tz = (double)ev.z - qq.z, tw = (double)ev.w - qq.w;
+          d2 += tx * tx + ty * ty + tz * tz + tw * tw;
+        }
+      } else {
+        for (int c = lane; c < f.d; c += 32) {
+          const double t = (double)__ldg(e + c) - qv[c];
+          d2 += t * t;
+        }
+      }
+      d2 = warp_sum_d(d2);
+      return exact_sim(f.metric, dot, ne, nq, d2);
+    }
     if (f.e_f16) {   // float16 storage: 8 halves per 16-byte load (d % 8 == 0)
       const __half* eh = reinterpret_cast<const __half*>(f.E) + (int64_t)row * f.ld;
       for (int c = lane * 8; c < f.d; c += 256) {
@@ -574,7 +607,7 @@ __global__ void __launch_bounds__(kSelThreads) finalize_kernel(const FinalizeArg
     }
     dot = warp_sum_d(dot);
     ne = warp_sum_d(ne);
-    return exact_sim(f.metric, dot, ne, nq);
+    return exact_sim(f.metric, dot, ne, nq, d2);
   };
 
   if (ns_all <= RL_MAX_SURVIVORS) {
