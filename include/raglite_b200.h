@@ -367,6 +367,35 @@ int rl_bm25_topk(const int64_t* term_off, const int32_t* doc, const int32_t* tf,
                  const int32_t* q_terms, int B, int k, double k1, double b, int64_t* out_chunk, double* out_score,
                  int32_t* out_count, void* workspace, size_t workspace_bytes, void* stream);
 
+/* Sharded BM25 (one shard per rank; every rank makes the same calls with the same queries).  The queries are planned
+ * on the host as "entries": each query's distinct stems sorted by code point, q_off int32 [B + 1] and q_terms int32 [J]
+ * = the shard's local term id of each entry, -1 where the shard has never seen the stem.  The per-chunk sum runs in
+ * entry order, which no shard's dictionary influences, so every shard layout rounds alike.
+ *
+ * rl_bm25_local_stats: out int64 [2 + J] = {live N, sum of live doc_len, live df of entry 0 .. J-1} of this shard (0 for
+ * an entry of -1).  n_chunks may be 0.  Summed over the ranks (all-reduce SUM: integers, exact) these are the corpus-wide
+ * statistics. */
+int rl_bm25_local_stats(const int64_t* term_off, const int32_t* doc, const int32_t* doc_len, const uint8_t* chunk_alive,
+                        int64_t n_terms, int64_t n_chunks, const int32_t* q_terms, int64_t n_entries, int64_t* out,
+                        void* stream);
+/* Bytes of one rank's packed top-k buffer: chunk int64 [B, k] | score float64 [B, k] | count int32 [B], padded to a
+ * multiple of 16 (0 when B or k is not positive). */
+size_t rl_bm25_packed_bytes(int B, int k);
+/* rl_bm25_topk_global: rl_bm25_topk with the weights from global_stats (the summed rl_bm25_local_stats buffer: N,
+ * avgdl = sum / N and idf of entry j = log10((N - df_j + 0.5) / (df_j + 0.5) + 1), the expressions of rl_bm25_stats) and
+ * chunk_base added to every chunk written.  Output: one rl_bm25_packed_bytes(B, k) buffer (16-byte aligned), padding
+ * zeroed.  n_chunks == 0 (an empty shard) is valid: every count is 0 and workspace may be NULL.  Same k / k1 / b /
+ * workspace rules as rl_bm25_topk. */
+int rl_bm25_topk_global(const int64_t* term_off, const int32_t* doc, const int32_t* tf, const int32_t* doc_len,
+                        const int64_t* global_stats, int64_t n_terms, int64_t n_chunks, const uint8_t* chunk_mask,
+                        const int32_t* q_off, const int32_t* q_terms, int B, int k, double k1, double b, int64_t chunk_base,
+                        void* out_packed, void* workspace, size_t workspace_bytes, void* stream);
+/* rl_bm25_merge_packed: gathered = R packed buffers of rl_bm25_packed_bytes(B, k) bytes end to end (16-byte aligned);
+ * per query, the top k of the R lists by (score desc, chunk asc) -- exact, chunks being unique across the shards.
+ * Outputs as rl_bm25_topk.  1 <= R <= 64, 1 <= k <= 4096; one CTA per query, no global atomics. */
+int rl_bm25_merge_packed(const void* gathered, int R, int B, int k, int64_t* out_chunk, double* out_score,
+                         int32_t* out_count, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

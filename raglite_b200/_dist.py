@@ -129,10 +129,20 @@ class ShardedIndex:
         return out[:3]
 
     def sum_over_shards(self, x: torch.Tensor) -> torch.Tensor:
-        """All-reduce (sum) of a small per-query tensor: row counts of the rank-then-filter probe."""
+        """All-reduce (sum) of a small tensor: row counts of the rank-then-filter probe, the BM25 statistics of a
+        keyword search."""
         if self.group is not None and self.world > 1:
             x = x.clone()
             dist.all_reduce(x, op=dist.ReduceOp.SUM, group=self.group)
+        return x
+
+    def gather_shards(self, x: torch.Tensor) -> torch.Tensor:
+        """All-gather (into one tensor) of an equally sized per-rank buffer: ``[R * x.numel()]``, rank r's part at
+        ``r * x.numel()``; ``x`` itself on a one-rank index."""
+        if self.group is not None and self.world > 1:
+            out = torch.empty(self.world * x.numel(), dtype=x.dtype, device=x.device)
+            dist.all_gather_into_tensor(out, x, group=self.group)
+            return out
         return x
 
     def max_over_shards(self, x: torch.Tensor) -> torch.Tensor:

@@ -202,3 +202,16 @@ class Analyzer:
         """Distinct term ids of a query's stems that are in the dictionary, ascending (unknown stems are ignored)."""
         ids = {self.term_ids[t] for t in query_terms(query) if t in self.term_ids}
         return np.fromiter(sorted(ids), dtype=np.int32, count=len(ids))
+
+    def query_plan(self, queries: Sequence[str]) -> tuple[np.ndarray, list[str], np.ndarray]:
+        """The entries of a sharded search: each query's distinct stems sorted by code point (stems are ASCII, so that
+        order is the same on every shard whatever its dictionary).  Returns ``(q_off int32 [B + 1], stems [J], ids int32
+        [J])``: query ``b`` is entries ``q_off[b] .. q_off[b + 1]``, ``ids`` the local term ids, ``-1`` for a stem this
+        dictionary does not hold.  Unlike ``query_ids``, unknown stems stay: another shard may hold them."""
+        per = [sorted(set(query_terms(q))) for q in queries]
+        q_off = np.zeros(len(per) + 1, dtype=np.int32)
+        np.cumsum([len(s) for s in per], out=q_off[1:])
+        stems = list(chain.from_iterable(per))
+        get = self.term_ids.get
+        ids = np.fromiter((get(t, -1) for t in stems), dtype=np.int32, count=len(stems))
+        return q_off, stems, ids

@@ -173,14 +173,52 @@ class KeywordIndex:
                 _ptr(self.term_off), _ptr(self.doc), _ptr(self.tf), _ptr(self.doc_len), _ptr(self.idf), _ptr(self.corpus),
                 self.n_terms, C, _ptr(chunk_mask), _ptr(qd), _ptr(qd) + 4 * (B + 1), B, int(k), K1, B_PARAM, _ptr(chunk),
                 _ptr(score), _ptr(count), _ptr(ws), need, _stream()), "rl_bm25_topk")
-            pkey = (out.numel(), _stream())
-            host = self._pinned.get(pkey)
-            if host is None:
-                if len(self._pinned) >= 8:
-                    self._pinned.pop(next(iter(self._pinned)))
-                host = self._pinned[pkey] = torch.empty(out.numel(), dtype=torch.uint8, pin_memory=True)
-            host.copy_(out, non_blocking=True)
-            torch.cuda.current_stream().synchronize()
+            return self._download(out, B, k)
+
+    def _download(self, out: torch.Tensor, B: int, k: int) -> tuple[np.ndarray, np.ndarray, np.ndarray]:
+        """One pinned copy of ``chunk int64 [B, k] | score float64 [B, k] | count int32 [B]`` and one synchronisation."""
+        pkey = (out.numel(), _stream())
+        host = self._pinned.get(pkey)
+        if host is None:
+            if len(self._pinned) >= 8:
+                self._pinned.pop(next(iter(self._pinned)))
+            host = self._pinned[pkey] = torch.empty(out.numel(), dtype=torch.uint8, pin_memory=True)
+        host.copy_(out, non_blocking=True)
+        torch.cuda.current_stream().synchronize()
         raw = host.numpy()
         return (raw[: B * k * 8].view(np.int64).reshape(B, k).copy(), raw[B * k * 8: B * k * 16].view(np.float64).reshape(B, k).copy(),
-                raw[B * k * 16:].view(np.int32).copy())
+                raw[B * k * 16: B * k * 16 + B * 4].view(np.int32).copy())
+
+    def sharded_topk_to_host(self, index: Any, queries: Sequence[str], *, k: int, chunk_mask: torch.Tensor | None,
+                             chunk_base: int) -> tuple[np.ndarray, np.ndarray, np.ndarray]:
+        """The BM25 top k over every shard of ``index`` (a ``ShardedIndex`` whose shard this is), a collective: every rank
+        calls it with the same queries and ``k``.  The entries of ``Analyzer.query_plan``, ``rl_bm25_local_stats``, ONE
+        all-reduce of its integers (``index.sum_over_shards``), ``rl_bm25_topk_global`` into a packed buffer, ONE
+        all-gather of the buffers (``index.gather_shards``), ``rl_bm25_merge_packed``, one pinned download and one
+        synchronisation.  Returns what ``topk_to_host`` returns, with global chunk indices."""
+        B, C = len(queries), self.n_chunks
+        q_off, _, ids = self.analyzer.query_plan(queries)
+        J = len(ids)
+        group = max(1, min(B, WORKSPACE_BYTES // max(8 * C, 1)))
+        dev, lib = self.device, self.lib
+        with torch.cuda.device(dev):
+            qd = torch.from_numpy(np.concatenate([q_off, ids]).astype(np.int32)).to(dev, non_blocking=True)
+            q_terms = _ptr(qd) + 4 * (B + 1)
+            stats = torch.empty(2 + J, dtype=torch.int64, device=dev)
+            _lib.check(lib.rl_bm25_local_stats(_ptr(self.term_off), _ptr(self.doc), _ptr(self.doc_len), _ptr(self.alive),
+                                               self.n_terms, C, q_terms, J, _ptr(stats), _stream()), "rl_bm25_local_stats")
+            stats = index.sum_over_shards(stats)
+            nbytes = int(lib.rl_bm25_packed_bytes(B, k))
+            packed = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+            need = int(lib.rl_bm25_workspace_bytes(C, group))
+            ws = self._workspace(need) if need else None
+            _lib.check(lib.rl_bm25_topk_global(
+                _ptr(self.term_off), _ptr(self.doc), _ptr(self.tf), _ptr(self.doc_len), _ptr(stats), self.n_terms, C,
+                _ptr(chunk_mask), _ptr(qd), q_terms, B, int(k), K1, B_PARAM, int(chunk_base), _ptr(packed), _ptr(ws), need,
+                _stream()), "rl_bm25_topk_global")
+            gathered = index.gather_shards(packed)
+            R = gathered.numel() // nbytes
+            out = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+            _lib.check(lib.rl_bm25_merge_packed(_ptr(gathered), R, B, int(k), _ptr(out), _ptr(out) + B * k * 8,
+                                                _ptr(out) + B * k * 16, _stream()), "rl_bm25_merge_packed")
+            return self._download(out, B, k)

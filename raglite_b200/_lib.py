@@ -27,6 +27,7 @@ EXPORTS = [
     "rl_segment_mean_pool", "rl_xenc_linear_image_bytes", "rl_xenc_pack_linear", "rl_xenc_linear",
     "rl_xenc_workspace_bytes", "rl_xenc_score", "rl_xenc_attention", "rl_xenc_encode", "rl_xenc_encode_attention",
     "rl_bm25_stats", "rl_bm25_workspace_bytes", "rl_bm25_topk",
+    "rl_bm25_local_stats", "rl_bm25_packed_bytes", "rl_bm25_topk_global", "rl_bm25_merge_packed",
 ]
 
 
@@ -114,9 +115,15 @@ def _declare(lib: C.CDLL) -> None:
     lib.rl_bm25_workspace_bytes.restype = C.c_size_t
     lib.rl_bm25_topk.argtypes = [vp, vp, vp, vp, vp, vp, i64, i64, vp, vp, vp, i32, i32, C.c_double, C.c_double, vp, vp, vp,
                                  vp, C.c_size_t, vp]
+    lib.rl_bm25_local_stats.argtypes = [vp, vp, vp, vp, i64, i64, vp, i64, vp, vp]
+    lib.rl_bm25_packed_bytes.argtypes = [i32, i32]
+    lib.rl_bm25_packed_bytes.restype = C.c_size_t
+    lib.rl_bm25_topk_global.argtypes = [vp, vp, vp, vp, vp, i64, i64, vp, vp, vp, i32, i32, C.c_double, C.c_double, i64, vp,
+                                        vp, C.c_size_t, vp]
+    lib.rl_bm25_merge_packed.argtypes = [vp, i32, i32, i32, vp, vp, vp, vp]
     for name in EXPORTS:
         if name not in ("rl_last_error", "rl_maxsim_workspace_bytes", "rl_xenc_linear_image_bytes", "rl_xenc_workspace_bytes",
-                        "rl_hits_packed_bytes", "rl_bm25_workspace_bytes"):
+                        "rl_hits_packed_bytes", "rl_bm25_workspace_bytes", "rl_bm25_packed_bytes"):
             getattr(lib, name).restype = C.c_int
 
 

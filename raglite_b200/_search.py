@@ -246,7 +246,14 @@ def keyword_search_batch(
     ordered by descending score, ties by ascending chunk index.  The metadata filter only decides which chunks can be
     results: ``N``, ``avgdl`` and ``df`` always cover every live chunk, as the reference's ``WHERE`` around the macro
     does.  Host work per call: analysing the queries, one upload, the kernel launches, one pinned download and one
-    stream synchronisation."""
+    stream synchronisation.
+
+    On a ``ShardedIndex`` the call is a collective, as the sharded ``vector_search_batch`` is: every rank passes the same
+    queries, ``num_results`` and filter.  ``N``, ``avgdl`` and each query term's ``df`` are then summed over the shards
+    (one all-reduce), each shard ranks its own chunks with those corpus-wide statistics, and the per-shard top k are
+    merged after one all-gather; the returned chunk indices are GLOBAL (``chunk_base`` of the owning shard + local
+    index), identical on every rank and for every shard layout of the same corpus (DESIGN.md section 3.7).  The
+    metadata filter is applied by each rank to its own chunks."""
     from ._keyword import MAX_RESULTS
 
     config = config or RAGLiteConfig()
@@ -256,21 +263,23 @@ def keyword_search_batch(
     index = index if index is not None else get_index(config)
     if index is None:
         raise ValueError(f"No index registered for db_url={config.db_url!r}; use raglite_b200.register_index")
-    if hasattr(index, "group"):
-        raise NotImplementedError("keyword_search on a ShardedIndex: document frequencies need the vocabulary of every rank")
-    local: CorpusIndex = index
+    sharded = hasattr(index, "group")
+    local: CorpusIndex = getattr(index, "local", index)
     queries = list(queries)
     k = int(num_results)
     if k < 0 or k > MAX_RESULTS:
         raise ValueError(f"num_results={k} is outside [0, {MAX_RESULTS}]")
     B = len(queries)
     empty = (np.full((B, k), -1, np.int64), np.full((B, k), -np.inf, np.float64), np.zeros(B, np.int32))
-    if B == 0 or k == 0 or local.n_live_chunks == 0:
+    if B == 0 or k == 0 or (local.n_live_chunks == 0 and not sharded):   # a shard takes part in the collectives even empty
         return empty
     with local._lock:
         kw = local.keyword_index()
         chunk_ok, _ = _filter_on_device(local, _adapt_metadata(metadata_filter))
-        return kw.topk_to_host(queries, k=k, chunk_mask=chunk_ok if chunk_ok is not None else kw.alive)
+        mask = chunk_ok if chunk_ok is not None else kw.alive
+        if sharded:
+            return kw.sharded_topk_to_host(index, queries, k=k, chunk_mask=mask, chunk_base=local.chunk_base)
+        return kw.topk_to_host(queries, k=k, chunk_mask=mask)
 
 
 def keyword_search(
@@ -281,7 +290,8 @@ def keyword_search(
     config: RAGLiteConfig | None = None,
 ) -> tuple[list[ChunkId], list[float]]:
     """Search chunks with BM25 keyword search -- drop-in for ``raglite.keyword_search`` (``_search.py:156-230``, the
-    DuckDB branch): the chunks that contain at least one query term, best ``num_results`` first."""
+    DuckDB branch): the chunks that contain at least one query term, best ``num_results`` first.  On a registered
+    ``ShardedIndex`` a collective (see ``keyword_search_batch``) that returns the ids of chunks owned by every rank."""
     config = config or RAGLiteConfig()
     if config.self_query and isinstance(query, str):
         raise NotImplementedError("self_query needs an LLM and is outside the accelerated hot path")
@@ -289,7 +299,8 @@ def keyword_search(
     ids, scores, counts = keyword_search_batch([query], num_results=num_results, metadata_filter=metadata_filter,
                                                config=config, index=index)
     n = int(counts[0])
-    return ([index.chunk_id_of(index.chunk_base + int(c)) for c in ids[0, :n]], [float(s) for s in scores[0, :n]])
+    base = 0 if hasattr(index, "group") else index.chunk_base   # a ShardedIndex returns global indices
+    return ([index.chunk_id_of(base + int(c)) for c in ids[0, :n]], [float(s) for s in scores[0, :n]])
 
 
 # ---- the steps right after the hot path (SURVEY.md section 8f-3) ------------------------------------------

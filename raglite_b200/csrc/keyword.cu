@@ -4,6 +4,11 @@
 //   rl_bm25_stats  df(t) over live chunks, N, sum of len and avgdl, idf(t) = log10((N - df + 0.5) / (df + 0.5) + 1)
 //   rl_bm25_topk   per query, the k best chunks by (score desc, chunk asc)
 //
+// A ShardedIndex runs the same arithmetic over corpus-wide statistics (DESIGN.md section 3.7):
+//   rl_bm25_local_stats   this shard's live N, sum of len and the df of each query entry, as integers (then all-reduced)
+//   rl_bm25_topk_global   rl_bm25_topk with the weights from those sums, global chunk numbers, one packed buffer out
+//   rl_bm25_merge_packed  the top k of the R gathered buffers
+//
 // Index layout (include/raglite_b200.h): term-major postings CSR term_off [V + 1], doc / tf [P] sorted by chunk within a
 // term, doc_len [C].  Every double is rounded exactly as the SQL expression reads (explicit _rn intrinsics: no FMA
 // contraction), so a score differs from a float64 NumPy restatement only through log10 in idf.
@@ -34,6 +39,15 @@ constexpr int kBm25MaxK = 4096;        // RL_MAX_SURVIVORS: the num_hits cap of 
 constexpr int kSelBins = 2048;        // 11-bit digits
 constexpr uint64_t kSign = 1ull << 63;
 
+// ---- corpus statistics -> BM25 weights (shared by the single-index and the sharded path, so both round alike) --------
+__device__ __forceinline__ double bm25_avgdl(double n, double sum_len) {
+  return __ddiv_rn(sum_len, n);   // AVG(len); NaN for an empty corpus (nothing is scored then)
+}
+__device__ __forceinline__ double bm25_idf(double N, double df) {
+  const double ratio = __ddiv_rn(__dadd_rn(__dsub_rn(N, df), 0.5), __dadd_rn(df, 0.5));
+  return log10(__dadd_rn(ratio, 1.0));
+}
+
 // ---- rl_bm25_stats ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(1024) bm25_corpus_kernel(const int32_t* __restrict__ doc_len, const uint8_t* __restrict__ alive,
                                                            int64_t n_chunks, double* __restrict__ corpus) {
@@ -57,7 +71,7 @@ __global__ void __launch_bounds__(1024) bm25_corpus_kernel(const int32_t* __rest
     for (int w = 0; w < (int)(blockDim.x >> 5); ++w) { tn += s_n[w]; tl += s_len[w]; }
     corpus[0] = (double)tn;
     corpus[1] = (double)tl;
-    corpus[2] = __ddiv_rn((double)tl, (double)tn);   // AVG(len); NaN for an empty corpus (nothing is scored then)
+    corpus[2] = bm25_avgdl((double)tn, (double)tl);
   }
 }
 
@@ -77,28 +91,31 @@ __global__ void __launch_bounds__(256) bm25_idf_kernel(const int64_t* __restrict
     if (threadIdx.x == 0) {
       int df = 0;
       for (int w = 0; w < 8; ++w) df += s_part[w];
-      const double d = (double)df;
-      const double ratio = __ddiv_rn(__dadd_rn(__dsub_rn(N, d), 0.5), __dadd_rn(d, 0.5));
-      idf[t] = log10(__dadd_rn(ratio, 1.0));
+      idf[t] = bm25_idf(N, (double)df);
       if (df_out) df_out[t] = df;
     }
     __syncthreads();
   }
 }
 
-// ---- rl_bm25_topk: scores of one (query, tile) -------------------------------------------------------------------------
+// ---- rl_bm25_topk / rl_bm25_topk_global: scores of one (query, tile) ---------------------------------------------------
+// kGlobal = false: idf[t] and corpus[2] from rl_bm25_stats.  kGlobal = true: the weights come from the corpus-wide
+// integers gstats = {N, sum of doc_len, df of entry 0, 1, ...} (rl_bm25_local_stats summed over the shards): avgdl once
+// per CTA, the idf of entry j where the term is met -- the same expressions rl_bm25_stats evaluates, so the same bits.
+// gstats is the last parameter so that the kGlobal = false instantiation keeps the parameter layout it always had.
+template <bool kGlobal>
 __global__ void __launch_bounds__(kScoreThreads) bm25_score_kernel(
     const int64_t* __restrict__ term_off, const int32_t* __restrict__ doc, const int32_t* __restrict__ tf,
     const int32_t* __restrict__ doc_len, const double* __restrict__ idf, const double* __restrict__ corpus, int64_t n_terms,
     int64_t n_chunks, const uint8_t* __restrict__ mask, const int32_t* __restrict__ q_off, const int32_t* __restrict__ q_terms,
-    int q0, double k1, double b, uint64_t* __restrict__ keys) {
+    int q0, double k1, double b, uint64_t* __restrict__ keys, const int64_t* __restrict__ gstats) {
   __shared__ double acc[kTile];
   __shared__ int64_t range[2];
   const int q = q0 + (int)blockIdx.y;
   const int64_t c0 = (int64_t)blockIdx.x * kTile;
   const int n = (int)min((int64_t)kTile, n_chunks - c0);
   for (int i = threadIdx.x; i < n; i += blockDim.x) acc[i] = 0.0;
-  const double avgdl = corpus[2];
+  const double avgdl = kGlobal ? bm25_avgdl((double)gstats[0], (double)gstats[1]) : corpus[2];
   const double k1p1 = __dadd_rn(k1, 1.0), one_minus_b = __dsub_rn(1.0, b);
   const int j0 = q_off[q], j1 = q_off[q + 1];
   for (int j = j0; j < j1; ++j) {
@@ -116,7 +133,7 @@ __global__ void __launch_bounds__(kScoreThreads) bm25_score_kernel(
     }
     __syncthreads();
     const int64_t p0 = range[0], p1 = range[1];
-    const double w = idf[t];
+    const double w = kGlobal ? bm25_idf((double)gstats[0], (double)gstats[2 + j]) : idf[t];
     for (int64_t p = p0 + threadIdx.x; p < p1; p += blockDim.x) {
       const int c = doc[p];
       const double f = (double)tf[p];
@@ -149,9 +166,13 @@ __device__ __forceinline__ bool ge_prefix(uint64_t key, uint32_t lo, uint64_t m_
   return a > p_hi || (a == p_hi && (lo & m_lo) >= p_lo);
 }
 
+// kGlobal: out_chunk holds chunk_base + chunk (the shard's global numbering).  chunk_base is the last parameter for the
+// reason given at the score kernel.  With n_chunks == 0 (an empty shard) nothing is read and every row comes out empty.
+template <bool kGlobal>
 __global__ void __launch_bounds__(kSelectThreads) bm25_select_kernel(const uint64_t* __restrict__ keys, int64_t n_chunks, int q0,
                                                                      int k, int64_t* __restrict__ out_chunk,
-                                                                     double* __restrict__ out_score, int32_t* __restrict__ out_count) {
+                                                                     double* __restrict__ out_score, int32_t* __restrict__ out_count,
+                                                                     int64_t chunk_base) {
   extern __shared__ __align__(16) unsigned char smem[];
   uint64_t* s_key = reinterpret_cast<uint64_t*>(smem);              // [kBm25MaxK]
   int32_t* s_chunk = reinterpret_cast<int32_t*>(s_key + kBm25MaxK);  // [kBm25MaxK]
@@ -276,7 +297,7 @@ __global__ void __launch_bounds__(kSelectThreads) bm25_select_kernel(const uint6
   double* os = out_score + (int64_t)q * k;
   for (int i = tid; i < k; i += blockDim.x) {
     if (i < m) {
-      oc[i] = s_chunk[i];
+      oc[i] = kGlobal ? chunk_base + s_chunk[i] : s_chunk[i];
       os[i] = __longlong_as_double((long long)(s_key[i] & ~kSign));
     } else {
       oc[i] = -1;
@@ -284,6 +305,175 @@ __global__ void __launch_bounds__(kSelectThreads) bm25_select_kernel(const uint6
     }
   }
   if (tid == 0) out_count[q] = m;
+}
+
+// ---- rl_bm25_local_stats ---------------------------------------------------------------------------------------------
+// Block 0: this shard's live N and sum of doc_len; block 1 + i (grid-stride): the live df of entry i.  Integers only,
+// so the sum over the shards is exact whatever order the all-reduce adds them in.
+constexpr int kStatThreads = 256;
+__global__ void __launch_bounds__(kStatThreads) bm25_local_stats_kernel(
+    const int64_t* __restrict__ term_off, const int32_t* __restrict__ doc, const int32_t* __restrict__ doc_len,
+    const uint8_t* __restrict__ alive, int64_t n_terms, int64_t n_chunks, const int32_t* __restrict__ q_terms,
+    int64_t n_entries, int64_t* __restrict__ out) {
+  __shared__ long long s_a[kStatThreads / 32], s_b[kStatThreads / 32];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (blockIdx.x == 0) {
+    long long n = 0, len = 0;
+    for (int64_t c = threadIdx.x; c < n_chunks; c += blockDim.x) {
+      if (alive == nullptr || alive[c]) {
+        ++n;
+        len += doc_len[c];
+      }
+    }
+    for (int off = 16; off > 0; off >>= 1) {
+      n += __shfl_down_sync(0xffffffffu, n, off);
+      len += __shfl_down_sync(0xffffffffu, len, off);
+    }
+    if (lane == 0) { s_a[warp] = n; s_b[warp] = len; }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      long long tn = 0, tl = 0;
+      for (int w = 0; w < kStatThreads / 32; ++w) { tn += s_a[w]; tl += s_b[w]; }
+      out[0] = tn;
+      out[1] = tl;
+    }
+    return;
+  }
+  for (int64_t j = blockIdx.x - 1; j < n_entries; j += gridDim.x - 1) {
+    const int t = q_terms[j];
+    long long cnt = 0;
+    if (t >= 0 && (int64_t)t < n_terms) {   // uniform over the CTA
+      for (int64_t p = term_off[t] + threadIdx.x; p < term_off[t + 1]; p += blockDim.x)
+        cnt += (alive == nullptr || alive[doc[p]]) ? 1 : 0;
+    }
+    for (int off = 16; off > 0; off >>= 1) cnt += __shfl_down_sync(0xffffffffu, cnt, off);
+    if (lane == 0) s_a[warp] = cnt;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      long long df = 0;
+      for (int w = 0; w < kStatThreads / 32; ++w) df += s_a[w];
+      out[2 + j] = df;
+    }
+    __syncthreads();
+  }
+}
+
+// ---- rl_bm25_merge_packed ----------------------------------------------------------------------------------------------
+// One CTA per query merges the R sorted lists of the gathered per-shard buffers (rl_bm25_packed_bytes each) into the top
+// k by (score desc, global chunk asc).  Global chunks are unique, so that order is total and every entry has one rank.
+//   cut     how many entries of each list make the top want = min(k, sum of counts): a binary search over the list's
+//           positions whose predicate "rank of the entry <= want" costs one lower-bound search per list (ranks are
+//           counted in shared-memory integer atomics); every list halves its window each round, 13 rounds at k = 4096.
+//   place   the survivors, at most k, are staged in shared memory by list; each one's output position is its index in
+//           its own list plus the number of better survivors of every other list (binary searches in shared memory).
+constexpr int kMergeThreads = 512;
+constexpr int kMergeMaxR = 64;
+
+struct PackedList {   // one shard's row of one query inside a gathered buffer
+  const int64_t* chunk;
+  const double* score;
+  int n;
+};
+
+// Entries of a sorted run (score, chunk)[0, n) that come before (s, c) or are (s, c) itself.
+__device__ __forceinline__ int count_at_or_before(const double* score, const int64_t* chunk, int n, double s, int64_t c) {
+  int lo = 0, hi = n;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    const double sm = score[mid];
+    const int64_t cm = chunk[mid];
+    if (sm > s || (sm == s && cm <= c)) lo = mid + 1; else hi = mid;
+  }
+  return lo;
+}
+
+__device__ __forceinline__ PackedList packed_list(const unsigned char* gathered, size_t stride, int r, int B, int k, int q) {
+  const unsigned char* base = gathered + (size_t)r * stride;
+  const size_t bk = (size_t)B * k;
+  PackedList L;
+  L.chunk = reinterpret_cast<const int64_t*>(base) + (size_t)q * k;
+  L.score = reinterpret_cast<const double*>(base + bk * 8) + (size_t)q * k;
+  L.n = min(max(reinterpret_cast<const int32_t*>(base + bk * 16)[q], 0), k);
+  return L;
+}
+
+__global__ void __launch_bounds__(kMergeThreads) bm25_merge_kernel(const unsigned char* __restrict__ gathered, size_t stride,
+                                                                    int R, int B, int k, int64_t* __restrict__ out_chunk,
+                                                                    double* __restrict__ out_score,
+                                                                    int32_t* __restrict__ out_count) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  double* s_score = reinterpret_cast<double*>(smem);                  // [k]
+  int64_t* s_chunk = reinterpret_cast<int64_t*>(s_score + k);         // [k]
+  __shared__ int s_lo[kMergeMaxR], s_hi[kMergeMaxR], s_rank[kMergeMaxR], s_off[kMergeMaxR + 1];
+  __shared__ int s_want;
+  const int q = blockIdx.x, tid = threadIdx.x;
+  if (tid < R) {
+    s_lo[tid] = 0;
+    s_hi[tid] = packed_list(gathered, stride, tid, B, k, q).n;
+    s_rank[tid] = 0;
+  }
+  __syncthreads();
+  if (tid == 0) {
+    int total = 0;
+    for (int r = 0; r < R; ++r) total += s_hi[r];
+    s_want = min(total, k);
+  }
+  __syncthreads();
+  const int want = s_want;
+  // cut: afterwards s_lo[r] = the number of list r's entries among the best `want`
+  for (;;) {
+    const bool open = tid < R && s_lo[tid] < s_hi[tid];
+    if (!__syncthreads_or(open)) break;
+    for (int p = tid; p < R * R; p += blockDim.x) {
+      const int r = p / R, o = p - r * R;
+      const int lo = s_lo[r], hi = s_hi[r];
+      if (lo >= hi) continue;
+      const int mid = (lo + hi) >> 1;
+      const PackedList a = packed_list(gathered, stride, r, B, k, q);
+      const PackedList other = packed_list(gathered, stride, o, B, k, q);
+      const int c = o == r ? mid + 1 : count_at_or_before(other.score, other.chunk, other.n, a.score[mid], a.chunk[mid]);
+      atomicAdd(&s_rank[r], c);
+    }
+    __syncthreads();
+    if (tid < R && s_lo[tid] < s_hi[tid]) {
+      const int mid = (s_lo[tid] + s_hi[tid]) >> 1;
+      if (s_rank[tid] <= want) s_lo[tid] = mid + 1; else s_hi[tid] = mid;
+      s_rank[tid] = 0;
+    }
+  }
+  if (tid == 0) {
+    s_off[0] = 0;
+    for (int r = 0; r < R; ++r) s_off[r + 1] = s_off[r] + s_lo[r];
+  }
+  __syncthreads();
+  // place: stage the survivors list by list, then scatter each to its rank
+  for (int r = 0; r < R; ++r) {
+    const PackedList a = packed_list(gathered, stride, r, B, k, q);
+    for (int i = tid; i < s_lo[r]; i += blockDim.x) {
+      s_score[s_off[r] + i] = a.score[i];
+      s_chunk[s_off[r] + i] = a.chunk[i];
+    }
+  }
+  __syncthreads();
+  int64_t* oc = out_chunk + (int64_t)q * k;
+  double* os = out_score + (int64_t)q * k;
+  for (int i = tid; i < want; i += blockDim.x) {
+    int r = 0;
+    while (s_off[r + 1] <= i) ++r;
+    const double s = s_score[i];
+    const int64_t c = s_chunk[i];
+    int pos = i - s_off[r];
+    for (int o = 0; o < R; ++o) {
+      if (o != r) pos += count_at_or_before(s_score + s_off[o], s_chunk + s_off[o], s_off[o + 1] - s_off[o], s, c);
+    }
+    oc[pos] = c;
+    os[pos] = s;
+  }
+  for (int i = want + tid; i < k; i += blockDim.x) {
+    oc[i] = -1;
+    os[i] = -__builtin_huge_val();
+  }
+  if (tid == 0) out_count[q] = want;
 }
 
 }  // namespace
@@ -329,17 +519,106 @@ extern "C" int rl_bm25_topk(const int64_t* term_off, const int32_t* doc, const i
              rl_bm25_workspace_bytes(n_chunks, 1));
   const int group = (int)std::min<int64_t>(std::min<int64_t>(group64, B), 65535);
   const size_t sel_smem = (size_t)kBm25MaxK * (sizeof(uint64_t) + sizeof(int32_t)) + kSelBins * sizeof(uint32_t);
-  RL_CUDA_CHECK(cudaFuncSetAttribute(bm25_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sel_smem));
+  RL_CUDA_CHECK(cudaFuncSetAttribute(bm25_select_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sel_smem));
   const unsigned n_tiles = (unsigned)((n_chunks + kTile - 1) / kTile);
   uint64_t* keys = static_cast<uint64_t*>(workspace);
   cudaStream_t st = (cudaStream_t)stream;
   for (int q0 = 0; q0 < B; q0 += group) {
     const int g = min(group, B - q0);
-    bm25_score_kernel<<<dim3(n_tiles, g), kScoreThreads, 0, st>>>(term_off, doc, tf, doc_len, idf, corpus, n_terms, n_chunks,
-                                                                  chunk_mask, q_off, q_terms, q0, k1, b, keys);
+    bm25_score_kernel<false><<<dim3(n_tiles, g), kScoreThreads, 0, st>>>(term_off, doc, tf, doc_len, idf, corpus, n_terms,
+                                                                         n_chunks, chunk_mask, q_off, q_terms, q0, k1, b, keys,
+                                                                         nullptr);
     RL_CUDA_CHECK(cudaGetLastError());
-    bm25_select_kernel<<<g, kSelectThreads, sel_smem, st>>>(keys, n_chunks, q0, k, out_chunk, out_score, out_count);
+    bm25_select_kernel<false><<<g, kSelectThreads, sel_smem, st>>>(keys, n_chunks, q0, k, out_chunk, out_score, out_count, 0);
     RL_CUDA_CHECK(cudaGetLastError());
   }
+  return RL_OK;
+}
+
+// ---- the sharded path: rl_bm25_local_stats -> all-reduce -> rl_bm25_topk_global -> all-gather -> rl_bm25_merge_packed --
+extern "C" int rl_bm25_local_stats(const int64_t* term_off, const int32_t* doc, const int32_t* doc_len,
+                                   const uint8_t* chunk_alive, int64_t n_terms, int64_t n_chunks, const int32_t* q_terms,
+                                   int64_t n_entries, int64_t* out, void* stream) {
+  RL_REQUIRE(n_terms >= 0 && n_chunks >= 0 && n_chunks <= INT32_MAX && n_entries >= 0, RL_EINVAL,
+             "rl_bm25_local_stats: bad sizes");
+  RL_REQUIRE(term_off && out && (n_chunks == 0 || doc_len) && (n_entries == 0 || q_terms) && (n_terms == 0 || n_chunks == 0 || doc),
+             RL_EINVAL, "rl_bm25_local_stats: null pointer");
+  const int grid = 1 + (int)std::min<int64_t>(n_entries, 1 << 16);
+  bm25_local_stats_kernel<<<grid, kStatThreads, 0, (cudaStream_t)stream>>>(term_off, doc, doc_len, chunk_alive, n_terms,
+                                                                            n_chunks, q_terms, n_entries, out);
+  RL_CUDA_CHECK(cudaGetLastError());
+  return RL_OK;
+}
+
+extern "C" size_t rl_bm25_packed_bytes(int B, int k) {
+  if (B <= 0 || k <= 0) return 0;
+  const size_t raw = (size_t)B * (size_t)k * 16 + (size_t)B * 4;
+  return (raw + 15) & ~(size_t)15;
+}
+
+extern "C" int rl_bm25_topk_global(const int64_t* term_off, const int32_t* doc, const int32_t* tf, const int32_t* doc_len,
+                                   const int64_t* global_stats, int64_t n_terms, int64_t n_chunks, const uint8_t* chunk_mask,
+                                   const int32_t* q_off, const int32_t* q_terms, int B, int k, double k1, double b,
+                                   int64_t chunk_base, void* out_packed, void* workspace, size_t workspace_bytes,
+                                   void* stream) {
+  RL_REQUIRE(B >= 0 && n_terms >= 0 && n_chunks >= 0 && n_chunks <= INT32_MAX && chunk_base >= 0, RL_EINVAL,
+             "rl_bm25_topk_global: bad sizes");
+  RL_REQUIRE(k >= 1 && k <= kBm25MaxK, RL_EINVAL, "rl_bm25_topk_global: k=%d outside [1, %d]", k, kBm25MaxK);
+  RL_REQUIRE(k1 >= 0.0 && b >= 0.0 && b <= 1.0, RL_EINVAL, "rl_bm25_topk_global: k1 must be >= 0 and b in [0, 1]");
+  if (B == 0) return RL_OK;
+  RL_REQUIRE(term_off && global_stats && q_off && out_packed && (n_chunks == 0 || (doc_len && workspace)) &&
+                 (n_terms == 0 || n_chunks == 0 || (doc && tf)),
+             RL_EINVAL, "rl_bm25_topk_global: null pointer");
+  RL_REQUIRE(((uintptr_t)out_packed & 15) == 0 && ((uintptr_t)workspace & 7) == 0, RL_EINVAL,
+             "rl_bm25_topk_global: out_packed must be 16-byte and workspace 8-byte aligned");
+  int group = std::min(B, 65535);
+  if (n_chunks > 0) {
+    const int64_t group64 = (int64_t)(workspace_bytes / ((size_t)n_chunks * sizeof(uint64_t)));
+    RL_REQUIRE(group64 >= 1, RL_ENOSPACE, "rl_bm25_topk_global: workspace of %zu bytes holds no query (needs %zu)",
+               workspace_bytes, rl_bm25_workspace_bytes(n_chunks, 1));
+    group = (int)std::min<int64_t>(group64, group);
+  }
+  unsigned char* out = static_cast<unsigned char*>(out_packed);
+  const size_t bk = (size_t)B * k;
+  int64_t* out_chunk = reinterpret_cast<int64_t*>(out);
+  double* out_score = reinterpret_cast<double*>(out + bk * 8);
+  int32_t* out_count = reinterpret_cast<int32_t*>(out + bk * 16);
+  cudaStream_t st = (cudaStream_t)stream;
+  const size_t used = bk * 16 + (size_t)B * 4, total = rl_bm25_packed_bytes(B, k);
+  if (total > used) RL_CUDA_CHECK(cudaMemsetAsync(out + used, 0, total - used, st));   // the padding travels too
+  const size_t sel_smem = (size_t)kBm25MaxK * (sizeof(uint64_t) + sizeof(int32_t)) + kSelBins * sizeof(uint32_t);
+  RL_CUDA_CHECK(cudaFuncSetAttribute(bm25_select_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sel_smem));
+  const unsigned n_tiles = (unsigned)((n_chunks + kTile - 1) / kTile);
+  uint64_t* keys = static_cast<uint64_t*>(workspace);
+  for (int q0 = 0; q0 < B; q0 += group) {
+    const int g = min(group, B - q0);
+    if (n_chunks > 0) {
+      bm25_score_kernel<true><<<dim3(n_tiles, g), kScoreThreads, 0, st>>>(term_off, doc, tf, doc_len, nullptr, nullptr,
+                                                                          n_terms, n_chunks, chunk_mask, q_off, q_terms, q0,
+                                                                          k1, b, keys, global_stats);
+      RL_CUDA_CHECK(cudaGetLastError());
+    }
+    bm25_select_kernel<true><<<g, kSelectThreads, sel_smem, st>>>(keys, n_chunks, q0, k, out_chunk, out_score, out_count,
+                                                                  chunk_base);
+    RL_CUDA_CHECK(cudaGetLastError());
+  }
+  return RL_OK;
+}
+
+extern "C" int rl_bm25_merge_packed(const void* gathered, int R, int B, int k, int64_t* out_chunk, double* out_score,
+                                    int32_t* out_count, void* stream) {
+  RL_REQUIRE(R >= 1 && R <= kMergeMaxR && B >= 0, RL_EINVAL, "rl_bm25_merge_packed: R=%d outside [1, %d] or B < 0", R,
+             kMergeMaxR);
+  RL_REQUIRE(k >= 1 && k <= kBm25MaxK, RL_EINVAL, "rl_bm25_merge_packed: k=%d outside [1, %d]", k, kBm25MaxK);
+  if (B == 0) return RL_OK;
+  RL_REQUIRE(gathered && out_chunk && out_score && out_count, RL_EINVAL, "rl_bm25_merge_packed: null pointer");
+  RL_REQUIRE(((uintptr_t)gathered & 15) == 0, RL_EINVAL, "rl_bm25_merge_packed: gathered must be 16-byte aligned");
+  const size_t smem = (size_t)k * (sizeof(double) + sizeof(int64_t));
+  RL_CUDA_CHECK(cudaFuncSetAttribute(bm25_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  cudaStream_t st = (cudaStream_t)stream;
+  const size_t stride = rl_bm25_packed_bytes(B, k);
+  bm25_merge_kernel<<<B, kMergeThreads, smem, st>>>(static_cast<const unsigned char*>(gathered), stride, R, B, k, out_chunk,
+                                                    out_score, out_count);
+  RL_CUDA_CHECK(cudaGetLastError());
   return RL_OK;
 }

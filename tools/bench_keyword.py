@@ -8,7 +8,10 @@ Prints one JSON line: index build time (host analysis / device postings / statis
 time of the top-k launches, per-kernel device times (torch.profiler), algorithmic bytes over kernel time against the
 H100's 3.35 TB/s, the port's queries/s for ``--oracle-queries`` queries, and how many of those the device matched.
 At the default size the host stages dominate the run (generating 375 M words, analysing them for the index and again for
-the port): about ten minutes on a 16-thread host; ``--chunks 250000`` takes about three."""
+the port): about ten minutes on a 16-thread host; ``--chunks 250000`` takes about three.
+``--shards 1`` adds the sharded path on one GPU: ``ShardedIndex(group=None)`` over the same index against the bare index
+(per-batch medians, alternating), CUDA-event times of ``rl_bm25_local_stats``, ``rl_bm25_topk_global`` and
+``rl_bm25_merge_packed``, and the merge alone on synthetic full lists at R = 2, 8 and k = 64, 4096 (B = 256)."""
 import argparse, json, operator, subprocess, sys, time
 from pathlib import Path
 ROOT = Path(__file__).resolve().parents[1]
@@ -26,7 +29,12 @@ ap.add_argument("--k", type=int, default=64)
 ap.add_argument("--reps", type=int, default=10)
 ap.add_argument("--oracle-queries", type=int, default=16)
 ap.add_argument("--seed", type=int, default=0)
+ap.add_argument("--shards", type=int, default=0,
+                help="1: also time the sharded path (ShardedIndex(group=None)) against the bare index, alternating, "
+                     "its three kernels, and the merge alone at R = 2, 8 and k = 64, 4096")
 args = ap.parse_args()
+if args.shards not in (0, 1):
+    sys.exit("--shards: only 1 (one GPU) is implemented; a multi-GPU run under torchrun is not")
 T0 = time.perf_counter()
 
 
@@ -142,6 +150,80 @@ for b in range(nq):
     n = int(counts_[b])
     w_ids, w_sc = want[b]
     ok += int(n == len(w_ids) and np.allclose(scores_[b, :n], w_sc, rtol=1e-12, atol=0) and list(ids_[b, :n]) == w_ids)
+sharded = {}
+if args.shards == 1:
+    from raglite_b200._dist import ShardedIndex
+
+    sh = ShardedIndex(idx)
+    s_ids, s_sc, s_cnt = rl.keyword_search_batch(queries, num_results=k, index=sh)
+    sharded["sharded_same_counts"] = bool(np.array_equal(s_cnt, counts_))
+    # the sum runs over sorted stems instead of first-appearance ids: scores agree to the last bits, not bit for bit
+    n_ok = [np.allclose(s_sc[b, :counts_[b]], scores_[b, :counts_[b]], rtol=1e-12, atol=0) for b in range(B)]
+    sharded["sharded_scores_within_1e-12"] = f"{sum(n_ok)}/{B}"
+    t_bare, t_sh = [], []
+    for _ in range(args.reps):   # alternate the two paths so that drift on a shared host hits both alike
+        t0 = time.perf_counter()
+        rl.keyword_search_batch(queries, num_results=k, index=idx)
+        t_bare.append(time.perf_counter() - t0)
+        t0 = time.perf_counter()
+        rl.keyword_search_batch(queries, num_results=k, index=sh)
+        t_sh.append(time.perf_counter() - t0)
+    sharded["bare_batch_ms_median"] = 1e3 * float(np.median(t_bare))
+    sharded["sharded_r1_batch_ms_median"] = 1e3 * float(np.median(t_sh))
+    # the three kernels of the sharded path alone, CUDA events around `reps` launches each
+    q_off_s, _, ids_s = kw.analyzer.query_plan(queries)
+    J = len(ids_s)
+    qs = torch.from_numpy(np.concatenate([q_off_s, ids_s]).astype(np.int32)).cuda()
+    st = torch.cuda.current_stream().cuda_stream
+    gstats = torch.empty(2 + J, dtype=torch.int64, device="cuda")
+    nb = int(kw.lib.rl_bm25_packed_bytes(B, k))
+    packed = torch.empty(nb, dtype=torch.uint8, device="cuda")
+    merged = torch.empty(nb, dtype=torch.uint8, device="cuda")
+
+    def local_stats():
+        _lib.check(kw.lib.rl_bm25_local_stats(kw.term_off.data_ptr(), kw.doc.data_ptr(), kw.doc_len.data_ptr(), None,
+                                              kw.n_terms, C, qs.data_ptr() + 4 * (B + 1), J, gstats.data_ptr(), st),
+                   "rl_bm25_local_stats")
+
+    def topk_global():
+        _lib.check(kw.lib.rl_bm25_topk_global(kw.term_off.data_ptr(), kw.doc.data_ptr(), kw.tf.data_ptr(),
+                                              kw.doc_len.data_ptr(), gstats.data_ptr(), kw.n_terms, C, None, qs.data_ptr(),
+                                              qs.data_ptr() + 4 * (B + 1), B, k, K1, B_PARAM, 0, packed.data_ptr(),
+                                              ws.data_ptr(), need, st), "rl_bm25_topk_global")
+
+    def merge(src, R, Bm, km, dst):
+        _lib.check(kw.lib.rl_bm25_merge_packed(src.data_ptr(), R, Bm, km, dst.data_ptr(), dst.data_ptr() + Bm * km * 8,
+                                               dst.data_ptr() + Bm * km * 16, st), "rl_bm25_merge_packed")
+
+    def event_ms(fn):
+        fn()
+        e = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
+        e[0].record()
+        for _ in range(args.reps):
+            fn()
+        e[1].record()
+        torch.cuda.synchronize()
+        return e[0].elapsed_time(e[1]) / args.reps
+
+    sharded["local_stats_ms"] = event_ms(local_stats)
+    sharded["topk_global_ms"] = event_ms(topk_global)
+    sharded["merge_r1_ms"] = event_ms(lambda: merge(packed, 1, B, k, merged))
+    # the merge alone on synthetic full lists: R shards x B queries x k entries, sorted, unique global chunks
+    for R in (2, 8):
+        for km in (64, 4096):
+            Bm = 256
+            g = torch.empty(R * int(kw.lib.rl_bm25_packed_bytes(Bm, km)), dtype=torch.uint8, device="cuda")
+            per = g.view(R, -1)
+            for r in range(R):
+                sc = torch.sort(torch.rand(Bm, km, dtype=torch.float64, device="cuda") * 20, dim=1, descending=True).values
+                ch = (r << 40) + torch.arange(km, dtype=torch.int64, device="cuda").expand(Bm, km)
+                per[r, : Bm * km * 8].copy_(ch.contiguous().view(torch.uint8).reshape(-1))
+                per[r, Bm * km * 8: Bm * km * 16].copy_(sc.contiguous().view(torch.uint8).reshape(-1))
+                per[r, Bm * km * 16: Bm * km * 16 + Bm * 4].copy_(
+                    torch.full((Bm,), km, dtype=torch.int32, device="cuda").view(torch.uint8))
+            dst = torch.empty(int(kw.lib.rl_bm25_packed_bytes(Bm, km)), dtype=torch.uint8, device="cuda")
+            sharded[f"merge_r{R}_k{km}_b{Bm}_ms"] = event_ms(lambda g=g, R=R, Bm=Bm, km=km, dst=dst: merge(g, R, Bm, km, dst))
+    stage("sharded path timed")
 try:
     card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
                           text=True, timeout=30, check=False).stdout.strip().splitlines()[0]
@@ -156,5 +238,5 @@ print(json.dumps({
     "algorithmic_gb": alg_bytes / 1e9, "algorithmic_tb_per_s": alg_bytes / (kernel_ms * 1e-3) / 1e12,
     "share_of_hbm": alg_bytes / (kernel_ms * 1e-3) / 1e12 / HBM_TBPS,
     "port_numpy_queries_per_s": nq / oracle_s, "port_build_s": oracle_build_s, "port_queries": nq,
-    "cpu_threads": torch.get_num_threads(), "oracle_match": f"{ok}/{nq}",
+    "cpu_threads": torch.get_num_threads(), "oracle_match": f"{ok}/{nq}", **sharded,
 }))
