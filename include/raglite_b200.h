@@ -342,6 +342,22 @@ int rl_xenc_encode(const rl_xenc_weights* w, const int32_t* input_ids, const int
  * hidden <= 1024, max_len <= 512). */
 int rl_xenc_encode_attention(const void* qkv, const int32_t* cu_seqlens, int P, int T, int max_len, int hidden, int n_heads,
                              void* ctx, void* workspace, size_t workspace_bytes, void* stream);
+/* Debug/test hook: the embeddings + LayerNorm step of rl_xenc_score / rl_xenc_encode on its own (same launch): out_f16
+ * [T, hidden] fp16 from w's word / position / token-type tables, emb_ln_g / emb_ln_b and ln_eps.  ids / type_ids /
+ * pos_ids [T] (device) index the tables (clamped to them).  hidden % 32 == 0 and <= 1024. */
+int rl_xenc_embed_ln(const rl_xenc_weights* w, const int32_t* ids, const int32_t* type_ids, const int32_t* pos_ids, int T,
+                     void* out_f16, void* stream);
+/* Debug/test hook: the residual + LayerNorm step of the encoder on its own (same launch): out [T, H] =
+ * LayerNorm(x + res) * gamma + beta with variance eps, x and res fp16 [T, H], out fp16 (out_f32 = 0) or fp32
+ * (out_f32 = 1, the last layer of rl_xenc_encode).  H % 32 == 0 and <= 1024, every pointer 16-byte aligned; out may be
+ * res (the encoder normalises in place). */
+int rl_xenc_add_ln(const void* x, const void* res, const float* gamma, const float* beta, float eps, int T, int H,
+                   int out_f32, void* out, void* stream);
+/* Debug/test hook: the pooler + classifier + score step of rl_xenc_score on its own (same launch): out_logit
+ * [P, n_labels] and out_score [P] from the fp16 rows hidden_f16 [T, hidden], the [CLS] row of sequence s at
+ * cu_seqlens[s] (device).  w's pooler_* / cls_* / n_labels (0 read as 1) and hidden (% 32 == 0, <= 1024). */
+int rl_xenc_cls_head(const rl_xenc_weights* w, const void* hidden_f16, const int32_t* cu_seqlens, int P, float* out_logit,
+                     float* out_score, void* stream);
 
 /* ---- BM25 keyword search: _search.py:203-225 (DuckDB fts match_bm25 at its defaults) -------------------------------
  * Inverted index over the chunk bodies (device arrays): term_off int64 [n_terms + 1], a term-major postings CSR whose

@@ -864,6 +864,8 @@ extern "C" int rl_xenc_linear(const void* X, const void* image, const float* bia
                        (cudaStream_t)stream);
 }
 
+static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
 // ---- attention step: setup and launches, shared by rl_xenc_score, rl_xenc_encode and their attention test hooks ----
 static size_t att_smem_bytes(int max_len) { return (size_t)((max_len + 63) / 64 * 64) * kAttPitch * 2 * sizeof(__half); }
 
@@ -963,6 +965,21 @@ static void launch_add_ln(const __half* x, const __half* res, const float* g, co
   }
 }
 
+// Pooler + classifier + score of P sequences from the fp16 rows `hidden` [T, H] (their [CLS] rows at cu_seqlens[s]).
+static void launch_cls_head(const rl_xenc_weights* w, int n_labels, const __half* hidden, const int32_t* cu_seqlens, int P,
+                            float* out_logit, float* out_score, cudaStream_t stream) {
+  const int H = w->hidden;
+  const int cls_warps = H / 32 < kClsMaxWarps ? H / 32 : kClsMaxWarps;
+  const dim3 cls_grid((P + kClsSeqs - 1) / kClsSeqs);
+  const size_t cls_smem = ((size_t)kClsSeqs * H + (size_t)kClsMaxWarps * kClsSeqs * n_labels) * sizeof(float);
+  if (n_labels == 1)
+    cls_head_kernel<1><<<cls_grid, cls_warps * 32, cls_smem, stream>>>(hidden, cu_seqlens, w->pooler_w, w->pooler_b, w->cls_w,
+                                                                       w->cls_b, P, H, out_logit, out_score);
+  else
+    cls_head_kernel<2><<<cls_grid, cls_warps * 32, cls_smem, stream>>>(hidden, cu_seqlens, w->pooler_w, w->pooler_b, w->cls_w,
+                                                                       w->cls_b, P, H, out_logit, out_score);
+}
+
 // Embeddings and every encoder layer of a packed batch, shared by rl_xenc_score and rl_xenc_encode (arguments checked by
 // the caller).  The last layer's output LayerNorm writes fp16 rows into the workspace's hidden buffer or, when out_f32 is
 // set, fp32 rows to out_f32 [T, H].
@@ -1040,16 +1057,7 @@ extern "C" int rl_xenc_score(const rl_xenc_weights* w, const int32_t* input_ids,
   RL_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   const int rc = encoder_forward(w, input_ids, type_ids, pos_ids, cu_seqlens, P, T, max_len, workspace, nullptr, sms, stream);
   if (rc != RL_OK) return rc;
-  const int cls_warps = H / 32 < kClsMaxWarps ? H / 32 : kClsMaxWarps;
-  const dim3 cls_grid((P + kClsSeqs - 1) / kClsSeqs);
-  const size_t cls_smem = ((size_t)kClsSeqs * H + (size_t)kClsMaxWarps * kClsSeqs * n_labels) * sizeof(float);
-  const __half* hidden = reinterpret_cast<const __half*>(workspace);
-  if (n_labels == 1)
-    cls_head_kernel<1><<<cls_grid, cls_warps * 32, cls_smem, stream>>>(hidden, cu_seqlens, w->pooler_w, w->pooler_b, w->cls_w,
-                                                                       w->cls_b, P, H, out_logit, out_score);
-  else
-    cls_head_kernel<2><<<cls_grid, cls_warps * 32, cls_smem, stream>>>(hidden, cu_seqlens, w->pooler_w, w->pooler_b, w->cls_w,
-                                                                       w->cls_b, P, H, out_logit, out_score);
+  launch_cls_head(w, n_labels, reinterpret_cast<const __half*>(workspace), cu_seqlens, P, out_logit, out_score, stream);
   RL_CUDA_CHECK(cudaGetLastError());
   return RL_OK;
 }
@@ -1096,4 +1104,53 @@ extern "C" int rl_xenc_encode_attention(const void* qkv, const int32_t* cu_seqle
   if (rc != RL_OK) return rc;
   return encoder_attention_launch(head_dim, reinterpret_cast<const __half*>(qkv), cu_seqlens, seq_order, P, max_len, hidden,
                                   n_heads, reinterpret_cast<__half*>(ctx), stream);
+}
+
+// ---- test hooks of the other forward steps: each runs the launch function that the forward itself runs ------------------
+extern "C" int rl_xenc_embed_ln(const rl_xenc_weights* w, const int32_t* ids, const int32_t* type_ids, const int32_t* pos_ids,
+                                int T, void* out_f16, void* stream) {
+  RL_REQUIRE(w && ids && type_ids && pos_ids && out_f16 && T >= 0, RL_EINVAL, "rl_xenc_embed_ln: bad arguments");
+  RL_REQUIRE(w->word_emb && w->pos_emb && w->type_emb && w->emb_ln_g && w->emb_ln_b, RL_EINVAL,
+             "rl_xenc_embed_ln: null embedding table or LayerNorm");
+  RL_REQUIRE(w->hidden > 0 && w->hidden % 32 == 0 && w->hidden <= kEncodeMaxHidden, RL_EUNSUPPORTED,
+             "rl_xenc_embed_ln: hidden=%d unsupported (hidden %% 32 == 0, hidden <= %d)", w->hidden, kEncodeMaxHidden);
+  RL_REQUIRE(w->vocab > 0 && w->max_pos > 0 && w->type_vocab > 0, RL_EINVAL, "rl_xenc_embed_ln: empty embedding table");
+  if (T == 0) return RL_OK;
+  launch_embed_ln(w, ids, type_ids, pos_ids, T, reinterpret_cast<__half*>(out_f16), (cudaStream_t)stream);
+  RL_CUDA_CHECK(cudaGetLastError());
+  return RL_OK;
+}
+
+extern "C" int rl_xenc_add_ln(const void* x, const void* res, const float* gamma, const float* beta, float eps, int T, int H,
+                              int out_f32, void* out, void* stream) {
+  RL_REQUIRE(x && res && gamma && beta && out && T >= 0, RL_EINVAL, "rl_xenc_add_ln: bad arguments");
+  RL_REQUIRE(H > 0 && H % 32 == 0 && H <= kEncodeMaxHidden, RL_EUNSUPPORTED,
+             "rl_xenc_add_ln: H=%d unsupported (H %% 32 == 0, H <= %d)", H, kEncodeMaxHidden);
+  // the vectorised path reads x / res in 8-byte and gamma / beta in 16-byte pieces and stores 8 / 16 bytes per piece
+  RL_REQUIRE(aligned16(x) && aligned16(res) && aligned16(gamma) && aligned16(beta) && aligned16(out), RL_EINVAL,
+             "rl_xenc_add_ln: every pointer must be 16-byte aligned");
+  if (T == 0) return RL_OK;
+  const __half* xh = reinterpret_cast<const __half*>(x);
+  const __half* rh = reinterpret_cast<const __half*>(res);
+  if (out_f32)
+    launch_add_ln(xh, rh, gamma, beta, eps, T, H, reinterpret_cast<float*>(out), (cudaStream_t)stream);
+  else
+    launch_add_ln(xh, rh, gamma, beta, eps, T, H, reinterpret_cast<__half*>(out), (cudaStream_t)stream);
+  RL_CUDA_CHECK(cudaGetLastError());
+  return RL_OK;
+}
+
+extern "C" int rl_xenc_cls_head(const rl_xenc_weights* w, const void* hidden_f16, const int32_t* cu_seqlens, int P,
+                                float* out_logit, float* out_score, void* stream) {
+  RL_REQUIRE(w && hidden_f16 && cu_seqlens && out_logit && out_score && P >= 0, RL_EINVAL, "rl_xenc_cls_head: bad arguments");
+  RL_REQUIRE(w->pooler_w && w->pooler_b && w->cls_w && w->cls_b, RL_EINVAL, "rl_xenc_cls_head: null head weights");
+  const int n_labels = w->n_labels == 0 ? 1 : w->n_labels;
+  RL_REQUIRE(n_labels == 1 || n_labels == 2, RL_EUNSUPPORTED, "rl_xenc_cls_head: n_labels=%d unsupported (1 or 2)", w->n_labels);
+  RL_REQUIRE(w->hidden > 0 && w->hidden % 32 == 0 && w->hidden <= kEncodeMaxHidden, RL_EUNSUPPORTED,
+             "rl_xenc_cls_head: hidden=%d unsupported (hidden %% 32 == 0, hidden <= %d)", w->hidden, kEncodeMaxHidden);
+  if (P == 0) return RL_OK;
+  launch_cls_head(w, n_labels, reinterpret_cast<const __half*>(hidden_f16), cu_seqlens, P, out_logit, out_score,
+                  (cudaStream_t)stream);
+  RL_CUDA_CHECK(cudaGetLastError());
+  return RL_OK;
 }

@@ -35,7 +35,10 @@ def test_linear_layer_matches_torch():
     """``rl_xenc_linear`` against float64 from the fp16-rounded X and W, GELU(erf) exact.  Shapes: the model's, short
     last 128-column passes (N % 128 != 0: stale weight rows may only feed columns that are not stored), K tails
     (K % 64 != 0: the tensor map zero-fills), ragged token tiles, and T = 20000 (more work items than SMs, so every
-    CTA loops over items and reuses its stage ring and epilogue staging)."""
+    CTA loops over items and reuses its stage ring and epilogue staging).  The widths the served models run: BERT-base /
+    XLM-R base (qkv 2304 x 768, o 768 x 768, up 3072 x 768 + GELU, down 768 x 3072) and XLM-R large / bge-m3 (qkv
+    3072 x 1024, o, up 4096 x 1024 + GELU, down 1024 x 4096: 32 column passes, or 64 K slices, about a dozen trips
+    round the stage ring per item), each at T = 1, 129 and 20000."""
     import itertools
 
     import torch
@@ -47,6 +50,9 @@ def test_linear_layer_matches_torch():
     shapes = [(300, 384, 384, 0), (1000, 1536, 384, 1), (777, 384, 1536, 0), (64, 1152, 384, 0)]
     Ts = (1, 127, 128, 129, 20000)
     shapes += [(T, N, K, act) for N, K, T, act in itertools.product((32, 96, 160, 416, 480), (8, 72, 160, 416), Ts, (0, 1))]
+    served = [(2304, 768, 0), (768, 768, 0), (3072, 768, 1), (768, 3072, 0), (3072, 1024, 0), (1024, 1024, 0),
+              (4096, 1024, 1), (1024, 4096, 0)]
+    shapes += [(T, N, K, act) for (N, K, act), T in itertools.product(served, (1, 129, 20000))]
     s = torch.cuda.current_stream().cuda_stream
     worst, worst_at = 0.0, None
     for (T, N, K, act) in shapes:

@@ -82,6 +82,70 @@ def test_attention_hook_refuses_what_rl_xenc_score_refuses():
     assert b"max_len=1281" in lib.rl_last_error()
 
 
+def test_layernorm_and_head_hooks_refuse_bad_arguments():
+    """``rl_xenc_embed_ln``, ``rl_xenc_add_ln`` and ``rl_xenc_cls_head`` check their arguments before any CUDA call (the
+    pointers here are never dereferenced; a zero-sized call returns before any launch)."""
+    from raglite_b200 import _lib
+
+    lib = _lib.load()
+    ptr = 4096                                                  # placeholder, 16-byte aligned
+
+    def weights(hidden=384, vocab=100, max_pos=512, type_vocab=2, n_labels=1, tables=True, head=True):
+        w = _lib.XencWeights()
+        w.hidden, w.vocab, w.max_pos, w.type_vocab, w.n_labels, w.ln_eps = hidden, vocab, max_pos, type_vocab, n_labels, 1e-12
+        if tables:
+            w.word_emb = w.pos_emb = w.type_emb = w.emb_ln_g = w.emb_ln_b = ptr
+        if head:
+            w.pooler_w = w.pooler_b = w.cls_w = w.cls_b = ptr
+        return ctypes.byref(w)
+
+    def embed(w=None, ids=ptr, out=ptr, T=5):
+        return lib.rl_xenc_embed_ln(weights() if w is None else w, ids, ptr, ptr, T, out, None)
+
+    assert embed(ids=None) == -1
+    assert embed(out=None) == -1
+    assert embed(T=-1) == -1
+    assert embed(w=weights(tables=False)) == -1
+    assert embed(w=weights(hidden=48)) == -4                    # hidden % 32
+    assert embed(w=weights(hidden=1056)) == -4                  # hidden > 1024
+    assert embed(w=weights(hidden=0)) == -4
+    assert embed(w=weights(vocab=0)) == -1
+    assert embed(w=weights(type_vocab=0)) == -1
+    assert embed(T=0) == 0
+
+    def add_ln(x=ptr, res=ptr, gamma=ptr, beta=ptr, out=ptr, T=5, H=384, out_f32=0):
+        return lib.rl_xenc_add_ln(x, res, gamma, beta, 1e-5, T, H, out_f32, out, None)
+
+    assert add_ln(x=None) == -1
+    assert add_ln(beta=None) == -1
+    assert add_ln(T=-1) == -1
+    assert add_ln(H=48) == -4
+    assert add_ln(H=1056) == -4
+    assert add_ln(H=0) == -4
+    for name in ("x", "res", "gamma", "beta", "out"):          # the vectorised path's 8- / 16-byte pieces
+        assert add_ln(**{name: ptr + 8}) == -1, name
+        assert b"16-byte aligned" in lib.rl_last_error()
+    assert add_ln(out_f32=1, out=ptr + 4) == -1
+    assert add_ln(T=0) == 0
+    assert add_ln(T=0, out=ptr, res=ptr) == 0                   # in place (out == res) is allowed
+
+    def head(w=None, hidden=ptr, cu=ptr, P=3, logit=ptr, score=ptr):
+        return lib.rl_xenc_cls_head(weights() if w is None else w, hidden, cu, P, logit, score, None)
+
+    assert head(hidden=None) == -1
+    assert head(cu=None) == -1
+    assert head(score=None) == -1
+    assert head(P=-1) == -1
+    assert head(w=weights(head=False)) == -1
+    assert head(w=weights(n_labels=3)) == -4
+    assert b"n_labels=3" in lib.rl_last_error()
+    assert head(w=weights(hidden=48)) == -4
+    assert head(w=weights(hidden=1056)) == -4
+    assert head(P=0) == 0
+    assert head(P=0, w=weights(n_labels=0)) == 0                # 0 labels is read as 1
+    assert head(P=0, w=weights(n_labels=2)) == 0
+
+
 def test_config_mirrors_reference_fields():
     from raglite_b200 import RAGLiteConfig
 
