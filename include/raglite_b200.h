@@ -364,51 +364,36 @@ int rl_xenc_cls_head(const rl_xenc_weights* w, const void* hidden_f16, const int
  * doc int32 / tf int32 [P] are sorted by chunk within each term; doc_len int32 [n_chunks] = terms left after stop-word
  * removal.  chunk_alive / chunk_mask: uint8 [n_chunks] or NULL (= every chunk).
  *
- * rl_bm25_stats: over the chunks with chunk_alive set, df[t] (int32 [n_terms], may be NULL) = number of such chunks that
- * contain t, idf[t] (float64) = log10((N - df + 0.5) / (df + 0.5) + 1), corpus (float64 [3]) = {N, sum of doc_len,
- * avgdl = sum / N}.  Every double is rounded as the SQL expression reads (no contraction). */
+ * rl_bm25_stats: over the chunks with chunk_alive set, df[t] (int32 [n_terms]) = number of such chunks that contain t,
+ * corpus (float64 [3]) = {N, sum of doc_len, avgdl = sum / N}.  Every double is rounded as the SQL expression reads (no
+ * contraction). */
 int rl_bm25_stats(const int64_t* term_off, const int32_t* doc, const int32_t* doc_len, const uint8_t* chunk_alive,
-                  int64_t n_terms, int64_t n_chunks, int32_t* df, double* idf, double* corpus, void* stream);
-/* Workspace that lets the top-k call below score `group` queries at a time: group * n_chunks * 8 bytes. */
+                  int64_t n_terms, int64_t n_chunks, int32_t* df, double* corpus, void* stream);
+/* Workspace that lets rl_bm25_topk_global score `group` queries at a time: group * n_chunks * 8 bytes. */
 size_t rl_bm25_workspace_bytes(int64_t n_chunks, int group);
-/* rl_bm25_topk: B queries, query b = the term ids q_terms[q_off[b] .. q_off[b+1]) (device int32; distinct, ascending --
- * the order the per-chunk sum runs in).  score(d) = sum over the query terms t in d of
- * idf[t] * (tf * (k1 + 1) / (tf + k1 * (1 - b + b * (doc_len[d] / avgdl)))), float64, rounded as written.  A chunk is a
- * result when it contains a query term and chunk_mask allows it (tombstones AND the metadata filter: the mask changes
- * nothing in idf / avgdl, which come from rl_bm25_stats).  Outputs, best first by (score desc, chunk asc):
- * out_chunk int64 [B, k] (-1 padded), out_score float64 [B, k] (-inf padded), out_count int32 [B].  1 <= k <= 4096
- * (RL_MAX_SURVIVORS); the queries are scored in groups of as many as the workspace holds (at least one). */
-int rl_bm25_topk(const int64_t* term_off, const int32_t* doc, const int32_t* tf, const int32_t* doc_len, const double* idf,
-                 const double* corpus, int64_t n_terms, int64_t n_chunks, const uint8_t* chunk_mask, const int32_t* q_off,
-                 const int32_t* q_terms, int B, int k, double k1, double b, int64_t* out_chunk, double* out_score,
-                 int32_t* out_count, void* workspace, size_t workspace_bytes, void* stream);
-
-/* Sharded BM25 (one shard per rank; every rank makes the same calls with the same queries).  The queries are planned
- * on the host as "entries": each query's distinct stems sorted by code point, q_off int32 [B + 1] and q_terms int32 [J]
- * = the shard's local term id of each entry, -1 where the shard has never seen the stem.  The per-chunk sum runs in
- * entry order, which no shard's dictionary influences, so every shard layout rounds alike.
- *
- * rl_bm25_local_stats: out int64 [2 + J] = {live N, sum of live doc_len, live df of entry 0 .. J-1} of this shard (0 for
- * an entry of -1).  n_chunks may be 0.  Summed over the ranks (all-reduce SUM: integers, exact) these are the corpus-wide
- * statistics. */
-int rl_bm25_local_stats(const int64_t* term_off, const int32_t* doc, const int32_t* doc_len, const uint8_t* chunk_alive,
-                        int64_t n_terms, int64_t n_chunks, const int32_t* q_terms, int64_t n_entries, int64_t* out,
-                        void* stream);
-/* Bytes of one rank's packed top-k buffer: chunk int64 [B, k] | score float64 [B, k] | count int32 [B], padded to a
- * multiple of 16 (0 when B or k is not positive). */
+/* Bytes of one packed top-k buffer: chunk int64 [B, k] | score float64 [B, k] | count int32 [B], padded to a multiple of
+ * 16 (0 when B or k is not positive). */
 size_t rl_bm25_packed_bytes(int B, int k);
-/* rl_bm25_topk_global: rl_bm25_topk with the weights from global_stats (the summed rl_bm25_local_stats buffer: N,
- * avgdl = sum / N and idf of entry j = log10((N - df_j + 0.5) / (df_j + 0.5) + 1), the expressions of rl_bm25_stats) and
- * chunk_base added to every chunk written.  Output: one rl_bm25_packed_bytes(B, k) buffer (16-byte aligned), padding
- * zeroed.  n_chunks == 0 (an empty shard) is valid: every count is 0 and workspace may be NULL.  Same k / k1 / b /
- * workspace rules as rl_bm25_topk. */
+/* rl_bm25_topk_global: B queries, query b = the entries q_off[b] .. q_off[b+1] (device int32), q_terms[j] the term id of
+ * entry j or -1 (a term this index does not hold; skipped), distinct within a query.  The per-chunk sum runs in entry
+ * order.  stats (device int64
+ * [2 + J]) = {N, sum of doc_len, df of entry 0 .. J-1}: on a single index its own live counts, on a ShardedIndex their
+ * sums over the shards (integers, so exact on every rank).  avgdl = sum / N, idf_j = log10((N - df_j + 0.5) / (df_j +
+ * 0.5) + 1), score(d) = sum over the entries j with a term in d of idf_j * (tf * (k1 + 1) / (tf + k1 * (1 - b + b *
+ * (doc_len[d] / avgdl)))), float64, rounded as written.  A chunk is a result when it contains an entry's term and
+ * chunk_mask allows it (tombstones AND the metadata filter: the mask changes nothing in the statistics).  Output: one
+ * rl_bm25_packed_bytes(B, k) buffer (16-byte aligned), best first by (score desc, chunk asc), chunk_base added to every
+ * chunk: chunk -1 padded, score -inf padded, padding zeroed.  1 <= k <= 4096 (RL_MAX_SURVIVORS), k1 >= 0, 0 <= b <= 1;
+ * the queries are scored in groups of as many as the workspace holds (at least one, else RL_ENOSPACE).
+ * n_chunks == 0 (an empty shard) is valid: every count is 0 and workspace may be NULL. */
 int rl_bm25_topk_global(const int64_t* term_off, const int32_t* doc, const int32_t* tf, const int32_t* doc_len,
-                        const int64_t* global_stats, int64_t n_terms, int64_t n_chunks, const uint8_t* chunk_mask,
+                        const int64_t* stats, int64_t n_terms, int64_t n_chunks, const uint8_t* chunk_mask,
                         const int32_t* q_off, const int32_t* q_terms, int B, int k, double k1, double b, int64_t chunk_base,
                         void* out_packed, void* workspace, size_t workspace_bytes, void* stream);
 /* rl_bm25_merge_packed: gathered = R packed buffers of rl_bm25_packed_bytes(B, k) bytes end to end (16-byte aligned);
  * per query, the top k of the R lists by (score desc, chunk asc) -- exact, chunks being unique across the shards.
- * Outputs as rl_bm25_topk.  1 <= R <= 64, 1 <= k <= 4096; one CTA per query, no global atomics. */
+ * Outputs, best first: out_chunk int64 [B, k] (-1 padded), out_score float64 [B, k] (-inf padded), out_count int32 [B].
+ * 1 <= R <= 64, 1 <= k <= 4096; one CTA per query, no global atomics. */
 int rl_bm25_merge_packed(const void* gathered, int R, int B, int k, int64_t* out_chunk, double* out_score,
                          int32_t* out_count, void* stream);
 

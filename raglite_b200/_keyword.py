@@ -2,18 +2,19 @@
 ``docs``, ``terms``, ``stats``) that ``create_fts_index`` builds for the reference's ``keyword_search``
 (``_database.py:618``, rebuilt after every insert and delete: ``_insert.py:268``, ``_delete.py:173``).
 
-Layout on the device (``rl_bm25_stats`` / ``rl_bm25_topk``, include/raglite_b200.h):
+Layout on the device (``rl_bm25_stats`` / ``rl_bm25_topk_global``, include/raglite_b200.h):
 
     term_off  int64   [V + 1]   term-major postings CSR
     doc, tf   int32   [P]       postings sorted by chunk within each term (tf = occurrences of the term in the chunk)
     doc_len   int32   [C]       terms of each chunk after stop-word removal
     df        int32   [V]       live chunks holding each term       (rl_bm25_stats, recomputed after every change)
-    idf       float64 [V]       log10((N - df + 0.5) / (df + 0.5) + 1)
     corpus    float64 [3]       N, sum of doc_len, avgdl over the live chunks
 
-The host keeps the ``stem -> term id`` dictionary only (``_fts.Analyzer``).  A ``CorpusIndex`` owns one of these and
-builds it on its first keyword search; appended chunks are analysed on the next search, deletes only make the
-statistics stale (tombstoned chunks keep their postings and are masked), ``compact`` remaps the postings.
+The host keeps the ``stem -> term id`` dictionary (``_fts.Analyzer``) and, from each refresh, ``df``, ``N`` and the sum
+of ``doc_len`` as integers: a search looks up the statistics of its query terms there and uploads them with its plan.
+A ``CorpusIndex`` owns one of these and builds it on its first keyword search; appended chunks are analysed on the next
+search, deletes only make the statistics stale (tombstoned chunks keep their postings and are masked), ``compact``
+remaps the postings.
 """
 
 from __future__ import annotations
@@ -55,8 +56,9 @@ class KeywordIndex:
             self.tf = torch.zeros(0, dtype=torch.int32, device=device)
             self.doc_len = torch.zeros(0, dtype=torch.int32, device=device)
             self.df = torch.zeros(0, dtype=torch.int32, device=device)
-            self.idf = torch.zeros(0, dtype=torch.float64, device=device)
             self.corpus = torch.zeros(3, dtype=torch.float64, device=device)
+        self.df_host = np.zeros(1, dtype=np.int64)   # df of every term, then a 0 that an entry of -1 looks up
+        self.n_live, self.sum_len = 0, 0
         self.alive: torch.Tensor | None = None   # uint8 [C] of the last refresh; None = no tombstones
         self.stale = True
         self.build_seconds = {"analysis": 0.0, "postings": 0.0}
@@ -120,18 +122,18 @@ class KeywordIndex:
         self.alive, self.stale = None, True
 
     def refresh(self, chunk_alive: np.ndarray) -> None:
-        """``rl_bm25_stats`` over the live chunks (``chunk_alive[:n_chunks]``); synchronises, so that searches on other
-        streams see the new statistics."""
+        """``rl_bm25_stats`` over the live chunks (``chunk_alive[:n_chunks]``), then host copies of ``df``, ``N`` and the
+        sum of ``doc_len``; the copies synchronise, so that searches on other streams see the new statistics."""
         alive = np.asarray(chunk_alive[: self.n_chunks], dtype=bool)
         with torch.cuda.device(self.device):
             self.alive = None if alive.all() else torch.from_numpy(alive.astype(np.uint8)).to(self.device)
             V = self.n_terms
             self.df = torch.empty(V, dtype=torch.int32, device=self.device)
-            self.idf = torch.empty(V, dtype=torch.float64, device=self.device)
             _lib.check(self.lib.rl_bm25_stats(_ptr(self.term_off), _ptr(self.doc), _ptr(self.doc_len), _ptr(self.alive), V,
-                                              self.n_chunks, _ptr(self.df), _ptr(self.idf), _ptr(self.corpus), _stream()),
-                       "rl_bm25_stats")
-            torch.cuda.current_stream().synchronize()
+                                              self.n_chunks, _ptr(self.df), _ptr(self.corpus), _stream()), "rl_bm25_stats")
+            self.df_host = np.append(self.df.cpu().numpy().astype(np.int64), 0)
+            corpus = self.corpus.cpu().numpy()
+        self.n_live, self.sum_len = int(corpus[0]), int(corpus[1])   # integer counts, exact in float64
         self.stale = False
 
     def stats(self) -> dict[str, Any]:
@@ -149,31 +151,52 @@ class KeywordIndex:
             ws = self._ws[key] = torch.empty(need, dtype=torch.uint8, device=self.device)
         return ws
 
-    def topk_to_host(self, queries: Sequence[str], *, k: int, chunk_mask: torch.Tensor | None, max_group: int | None = None
-                     ) -> tuple[np.ndarray, np.ndarray, np.ndarray]:
-        """Analyse the queries, then one upload, the ``rl_bm25_topk`` launches, one pinned download and one
-        synchronisation.  ``chunk_mask``: uint8 [C] (tombstones AND metadata filter), ``None`` = every chunk.
-        Returns host ``(chunk int64 [B, k] (-1 padded), score float64 [B, k] (-inf padded), count int32 [B])``."""
+    def topk_to_host(self, queries: Sequence[str], *, k: int, chunk_mask: torch.Tensor | None, max_group: int | None = None,
+                     index: Any | None = None) -> tuple[np.ndarray, np.ndarray, np.ndarray]:
+        """The BM25 top k over ``index``: ``None`` or the ``CorpusIndex`` that owns these postings (one shard), or a
+        ``ShardedIndex`` around it (a collective then: every rank calls it with the same queries and ``k``).  The query plan and its entries'
+        statistics (``int64 [2 + J]`` = N, sum of doc_len, df of each entry) from the host, ONE upload of both, on more
+        than one shard ONE all-reduce of the statistics (``index.sum_over_shards``), ``rl_bm25_topk_global`` into a
+        packed buffer, on more than one shard ONE all-gather of the buffers (``index.gather_shards``) and
+        ``rl_bm25_merge_packed``, then one pinned download and one synchronisation.  ``chunk_mask``: uint8 [C]
+        (tombstones AND metadata filter), ``None`` = every chunk; ``max_group`` caps the queries scored at once.
+        Returns host ``(chunk int64 [B, k] (-1 padded), score float64 [B, k] (-inf padded), count int32 [B])``, local
+        chunk indices on a ``CorpusIndex`` and global ones (``chunk_base`` + local) on a ``ShardedIndex``."""
         B, C = len(queries), self.n_chunks
-        ids = [self.analyzer.query_ids(q) for q in queries]
-        q_off = np.zeros(B + 1, dtype=np.int32)
-        np.cumsum([len(x) for x in ids], out=q_off[1:])
-        packed_q = np.concatenate([q_off, *ids]).astype(np.int32)
+        sharded = hasattr(index, "group")
+        if sharded:   # sorted stems, -1 kept: every shard sums the same entries in the same order
+            q_off, _, ids = self.analyzer.query_plan(queries)
+        else:         # the known term ids, ascending
+            per = [self.analyzer.query_ids(q) for q in queries]
+            q_off = np.zeros(B + 1, dtype=np.int32)
+            np.cumsum([len(x) for x in per], out=q_off[1:])
+            ids = np.concatenate([np.zeros(0, np.int32), *per])
+        J = len(ids)
+        stats = np.concatenate([[self.n_live, self.sum_len], self.df_host[ids]]).astype(np.int64)
+        R = index.world if sharded else 1
+        chunk_base = int(index.local.chunk_base) if sharded else 0
         group = max(1, min(B, int(max_group) if max_group else WORKSPACE_BYTES // max(8 * C, 1)))
-        dev = self.device
+        dev, lib = self.device, self.lib
         with torch.cuda.device(dev):
-            qd = torch.from_numpy(packed_q).to(dev, non_blocking=True)
-            out = torch.empty(B * k * 16 + B * 4, dtype=torch.uint8, device=dev)
-            chunk = out[: B * k * 8].view(torch.int64)
-            score = out[B * k * 8: B * k * 16].view(torch.float64)
-            count = out[B * k * 16:].view(torch.int32)
-            need = int(self.lib.rl_bm25_workspace_bytes(C, group))
-            ws = self._workspace(need)
-            _lib.check(self.lib.rl_bm25_topk(
-                _ptr(self.term_off), _ptr(self.doc), _ptr(self.tf), _ptr(self.doc_len), _ptr(self.idf), _ptr(self.corpus),
-                self.n_terms, C, _ptr(chunk_mask), _ptr(qd), _ptr(qd) + 4 * (B + 1), B, int(k), K1, B_PARAM, _ptr(chunk),
-                _ptr(score), _ptr(count), _ptr(ws), need, _stream()), "rl_bm25_topk")
-            return self._download(out, B, k)
+            plan = np.concatenate([stats.view(np.int32), q_off, ids])   # stats int64 [2 + J] | q_off [B + 1] | ids [J]
+            plan = torch.from_numpy(plan).to(dev, non_blocking=True)
+            stats_d, q_off_d = plan[: 2 * (2 + J)].view(torch.int64), _ptr(plan) + 8 * (2 + J)
+            if R > 1:
+                stats_d = index.sum_over_shards(stats_d)
+            nbytes = int(lib.rl_bm25_packed_bytes(B, k))
+            packed = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+            need = int(lib.rl_bm25_workspace_bytes(C, group))
+            ws = self._workspace(need) if need else None
+            _lib.check(lib.rl_bm25_topk_global(
+                _ptr(self.term_off), _ptr(self.doc), _ptr(self.tf), _ptr(self.doc_len), _ptr(stats_d), self.n_terms, C,
+                _ptr(chunk_mask), q_off_d, q_off_d + 4 * (B + 1), B, int(k), K1, B_PARAM, chunk_base, _ptr(packed), _ptr(ws),
+                need, _stream()), "rl_bm25_topk_global")
+            if R > 1:
+                gathered = index.gather_shards(packed)
+                packed = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+                _lib.check(lib.rl_bm25_merge_packed(_ptr(gathered), R, B, int(k), _ptr(packed), _ptr(packed) + B * k * 8,
+                                                    _ptr(packed) + B * k * 16, _stream()), "rl_bm25_merge_packed")
+            return self._download(packed, B, k)
 
     def _download(self, out: torch.Tensor, B: int, k: int) -> tuple[np.ndarray, np.ndarray, np.ndarray]:
         """One pinned copy of ``chunk int64 [B, k] | score float64 [B, k] | count int32 [B]`` and one synchronisation."""
@@ -188,37 +211,3 @@ class KeywordIndex:
         raw = host.numpy()
         return (raw[: B * k * 8].view(np.int64).reshape(B, k).copy(), raw[B * k * 8: B * k * 16].view(np.float64).reshape(B, k).copy(),
                 raw[B * k * 16: B * k * 16 + B * 4].view(np.int32).copy())
-
-    def sharded_topk_to_host(self, index: Any, queries: Sequence[str], *, k: int, chunk_mask: torch.Tensor | None,
-                             chunk_base: int) -> tuple[np.ndarray, np.ndarray, np.ndarray]:
-        """The BM25 top k over every shard of ``index`` (a ``ShardedIndex`` whose shard this is), a collective: every rank
-        calls it with the same queries and ``k``.  The entries of ``Analyzer.query_plan``, ``rl_bm25_local_stats``, ONE
-        all-reduce of its integers (``index.sum_over_shards``), ``rl_bm25_topk_global`` into a packed buffer, ONE
-        all-gather of the buffers (``index.gather_shards``), ``rl_bm25_merge_packed``, one pinned download and one
-        synchronisation.  Returns what ``topk_to_host`` returns, with global chunk indices."""
-        B, C = len(queries), self.n_chunks
-        q_off, _, ids = self.analyzer.query_plan(queries)
-        J = len(ids)
-        group = max(1, min(B, WORKSPACE_BYTES // max(8 * C, 1)))
-        dev, lib = self.device, self.lib
-        with torch.cuda.device(dev):
-            qd = torch.from_numpy(np.concatenate([q_off, ids]).astype(np.int32)).to(dev, non_blocking=True)
-            q_terms = _ptr(qd) + 4 * (B + 1)
-            stats = torch.empty(2 + J, dtype=torch.int64, device=dev)
-            _lib.check(lib.rl_bm25_local_stats(_ptr(self.term_off), _ptr(self.doc), _ptr(self.doc_len), _ptr(self.alive),
-                                               self.n_terms, C, q_terms, J, _ptr(stats), _stream()), "rl_bm25_local_stats")
-            stats = index.sum_over_shards(stats)
-            nbytes = int(lib.rl_bm25_packed_bytes(B, k))
-            packed = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-            need = int(lib.rl_bm25_workspace_bytes(C, group))
-            ws = self._workspace(need) if need else None
-            _lib.check(lib.rl_bm25_topk_global(
-                _ptr(self.term_off), _ptr(self.doc), _ptr(self.tf), _ptr(self.doc_len), _ptr(stats), self.n_terms, C,
-                _ptr(chunk_mask), _ptr(qd), q_terms, B, int(k), K1, B_PARAM, int(chunk_base), _ptr(packed), _ptr(ws), need,
-                _stream()), "rl_bm25_topk_global")
-            gathered = index.gather_shards(packed)
-            R = gathered.numel() // nbytes
-            out = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-            _lib.check(lib.rl_bm25_merge_packed(_ptr(gathered), R, B, int(k), _ptr(out), _ptr(out) + B * k * 8,
-                                                _ptr(out) + B * k * 16, _stream()), "rl_bm25_merge_packed")
-            return self._download(out, B, k)

@@ -26,8 +26,8 @@ EXPORTS = [
     "rl_maxsim_workspace_bytes", "rl_maxsim_topk", "rl_maxsim_count_at_least", "rl_maxsim_unfiltered_bound", "rl_maxsim_stats", "rl_maxsim_kernel_times", "rl_maxsim_release", "rl_maxsim_copy_dump", "rl_maxsim_copy_eps", "rl_topk_merge", "rl_topk_merge_packed", "rl_hits_packed_bytes", "rl_row_mask", "rl_rrf_fuse", "rl_span_collate", "rl_best_vectors", "rl_adapter_targets",
     "rl_segment_mean_pool", "rl_xenc_linear_image_bytes", "rl_xenc_pack_linear", "rl_xenc_linear",
     "rl_xenc_workspace_bytes", "rl_xenc_score", "rl_xenc_attention", "rl_xenc_encode", "rl_xenc_encode_attention",
-    "rl_xenc_embed_ln", "rl_xenc_add_ln", "rl_xenc_cls_head", "rl_bm25_stats", "rl_bm25_workspace_bytes", "rl_bm25_topk",
-    "rl_bm25_local_stats", "rl_bm25_packed_bytes", "rl_bm25_topk_global", "rl_bm25_merge_packed",
+    "rl_xenc_embed_ln", "rl_xenc_add_ln", "rl_xenc_cls_head", "rl_bm25_stats", "rl_bm25_workspace_bytes",
+    "rl_bm25_packed_bytes", "rl_bm25_topk_global", "rl_bm25_merge_packed",
 ]
 
 
@@ -113,12 +113,9 @@ def _declare(lib: C.CDLL) -> None:
     lib.rl_xenc_embed_ln.argtypes = [C.POINTER(XencWeights), vp, vp, vp, i32, vp, vp]
     lib.rl_xenc_add_ln.argtypes = [vp, vp, vp, vp, C.c_float, i32, i32, i32, vp, vp]
     lib.rl_xenc_cls_head.argtypes = [C.POINTER(XencWeights), vp, vp, i32, vp, vp, vp]
-    lib.rl_bm25_stats.argtypes = [vp, vp, vp, vp, i64, i64, vp, vp, vp, vp]
+    lib.rl_bm25_stats.argtypes = [vp, vp, vp, vp, i64, i64, vp, vp, vp]
     lib.rl_bm25_workspace_bytes.argtypes = [i64, i32]
     lib.rl_bm25_workspace_bytes.restype = C.c_size_t
-    lib.rl_bm25_topk.argtypes = [vp, vp, vp, vp, vp, vp, i64, i64, vp, vp, vp, i32, i32, C.c_double, C.c_double, vp, vp, vp,
-                                 vp, C.c_size_t, vp]
-    lib.rl_bm25_local_stats.argtypes = [vp, vp, vp, vp, i64, i64, vp, i64, vp, vp]
     lib.rl_bm25_packed_bytes.argtypes = [i32, i32]
     lib.rl_bm25_packed_bytes.restype = C.c_size_t
     lib.rl_bm25_topk_global.argtypes = [vp, vp, vp, vp, vp, i64, i64, vp, vp, vp, i32, i32, C.c_double, C.c_double, i64, vp,

@@ -276,10 +276,7 @@ def keyword_search_batch(
     with local._lock:
         kw = local.keyword_index()
         chunk_ok, _ = _filter_on_device(local, _adapt_metadata(metadata_filter))
-        mask = chunk_ok if chunk_ok is not None else kw.alive
-        if sharded:
-            return kw.sharded_topk_to_host(index, queries, k=k, chunk_mask=mask, chunk_base=local.chunk_base)
-        return kw.topk_to_host(queries, k=k, chunk_mask=mask)
+        return kw.topk_to_host(queries, k=k, chunk_mask=chunk_ok if chunk_ok is not None else kw.alive, index=index)
 
 
 def keyword_search(

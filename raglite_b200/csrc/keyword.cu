@@ -1,23 +1,20 @@
 // BM25 keyword search over a resident inverted index: the arithmetic of DuckDB's fts `match_bm25` macro, which the
 // reference's keyword_search runs at its defaults (reference _search.py:203-225).
 //
-//   rl_bm25_stats  df(t) over live chunks, N, sum of len and avgdl, idf(t) = log10((N - df + 0.5) / (df + 0.5) + 1)
-//   rl_bm25_topk   per query, the k best chunks by (score desc, chunk asc)
-//
-// A ShardedIndex runs the same arithmetic over corpus-wide statistics (DESIGN.md section 3.7):
-//   rl_bm25_local_stats   this shard's live N, sum of len and the df of each query entry, as integers (then all-reduced)
-//   rl_bm25_topk_global   rl_bm25_topk with the weights from those sums, global chunk numbers, one packed buffer out
-//   rl_bm25_merge_packed  the top k of the R gathered buffers
+//   rl_bm25_stats         df(t) over live chunks, N, sum of len and avgdl (refreshed after every change to the index)
+//   rl_bm25_topk_global   per query, the k best chunks by (score desc, chunk asc), with idf and avgdl computed from the
+//                         integers N, sum of len and the df of each query entry; chunk_base added; one packed buffer out
+//   rl_bm25_merge_packed  the top k of R gathered buffers (a ShardedIndex of R > 1 shards, DESIGN.md section 3.7)
 //
 // Index layout (include/raglite_b200.h): term-major postings CSR term_off [V + 1], doc / tf [P] sorted by chunk within a
 // term, doc_len [C].  Every double is rounded exactly as the SQL expression reads (explicit _rn intrinsics: no FMA
 // contraction), so a score differs from a float64 NumPy restatement only through log10 in idf.
 //
-// rl_bm25_topk processes the batch in groups of G queries, G set by the workspace (G * C keys of 8 bytes):
+// rl_bm25_topk_global processes the batch in groups of G queries, G set by the workspace (G * C keys of 8 bytes):
 //   score kernel   one CTA per (query, tile of kTile chunks); float64 accumulators in shared memory; for each query
-//                  term in ascending id order, the term's postings inside the tile are found by binary search and
-//                  each adds its contribution (a term touches a chunk at most once; a barrier separates the terms, so
-//                  a chunk's sum runs in term order and nothing races).  Output: an order-preserving 64-bit key per
+//                  entry in the given order, the term's postings inside the tile are found by binary search and each
+//                  adds its contribution (a term touches a chunk at most once; a barrier separates the entries, so a
+//                  chunk's sum runs in entry order and nothing races).  Output: an order-preserving 64-bit key per
 //                  chunk, 0 where the chunk is unmatched or masked.
 //   select kernel  one CTA per query: MSB-first radix select over the 96-bit composite (key, ~chunk) -- unique per
 //                  chunk, so the k-th largest composite is the exact cut of (score desc, chunk asc) -- then the k
@@ -39,7 +36,7 @@ constexpr int kBm25MaxK = 4096;        // RL_MAX_SURVIVORS: the num_hits cap of 
 constexpr int kSelBins = 2048;        // 11-bit digits
 constexpr uint64_t kSign = 1ull << 63;
 
-// ---- corpus statistics -> BM25 weights (shared by the single-index and the sharded path, so both round alike) --------
+// ---- corpus statistics -> BM25 weights -----------------------------------------------------------------------------
 __device__ __forceinline__ double bm25_avgdl(double n, double sum_len) {
   return __ddiv_rn(sum_len, n);   // AVG(len); NaN for an empty corpus (nothing is scored then)
 }
@@ -75,12 +72,10 @@ __global__ void __launch_bounds__(1024) bm25_corpus_kernel(const int32_t* __rest
   }
 }
 
-__global__ void __launch_bounds__(256) bm25_idf_kernel(const int64_t* __restrict__ term_off, const int32_t* __restrict__ doc,
-                                                       const uint8_t* __restrict__ alive, int64_t n_terms,
-                                                       const double* __restrict__ corpus, int32_t* __restrict__ df_out,
-                                                       double* __restrict__ idf) {
+__global__ void __launch_bounds__(256) bm25_df_kernel(const int64_t* __restrict__ term_off, const int32_t* __restrict__ doc,
+                                                      const uint8_t* __restrict__ alive, int64_t n_terms,
+                                                      int32_t* __restrict__ df_out) {
   __shared__ int s_part[8];
-  const double N = corpus[0];
   for (int64_t t = blockIdx.x; t < n_terms; t += gridDim.x) {
     const int64_t p0 = term_off[t], p1 = term_off[t + 1];
     int cnt = 0;
@@ -91,31 +86,27 @@ __global__ void __launch_bounds__(256) bm25_idf_kernel(const int64_t* __restrict
     if (threadIdx.x == 0) {
       int df = 0;
       for (int w = 0; w < 8; ++w) df += s_part[w];
-      idf[t] = bm25_idf(N, (double)df);
-      if (df_out) df_out[t] = df;
+      df_out[t] = df;
     }
     __syncthreads();
   }
 }
 
-// ---- rl_bm25_topk / rl_bm25_topk_global: scores of one (query, tile) ---------------------------------------------------
-// kGlobal = false: idf[t] and corpus[2] from rl_bm25_stats.  kGlobal = true: the weights come from the corpus-wide
-// integers gstats = {N, sum of doc_len, df of entry 0, 1, ...} (rl_bm25_local_stats summed over the shards): avgdl once
-// per CTA, the idf of entry j where the term is met -- the same expressions rl_bm25_stats evaluates, so the same bits.
-// gstats is the last parameter so that the kGlobal = false instantiation keeps the parameter layout it always had.
-template <bool kGlobal>
+// ---- rl_bm25_topk_global: scores of one (query, tile) ------------------------------------------------------------------
+// The weights come from the integers stats = {N, sum of doc_len, df of entry 0, 1, ...}: avgdl once per CTA, the idf of
+// entry j where the term is met -- the expressions of DuckDB's stats / dict tables, rounded alike on every shard.
 __global__ void __launch_bounds__(kScoreThreads) bm25_score_kernel(
     const int64_t* __restrict__ term_off, const int32_t* __restrict__ doc, const int32_t* __restrict__ tf,
-    const int32_t* __restrict__ doc_len, const double* __restrict__ idf, const double* __restrict__ corpus, int64_t n_terms,
-    int64_t n_chunks, const uint8_t* __restrict__ mask, const int32_t* __restrict__ q_off, const int32_t* __restrict__ q_terms,
-    int q0, double k1, double b, uint64_t* __restrict__ keys, const int64_t* __restrict__ gstats) {
+    const int32_t* __restrict__ doc_len, const int64_t* __restrict__ stats, int64_t n_terms, int64_t n_chunks,
+    const uint8_t* __restrict__ mask, const int32_t* __restrict__ q_off, const int32_t* __restrict__ q_terms, int q0,
+    double k1, double b, uint64_t* __restrict__ keys) {
   __shared__ double acc[kTile];
   __shared__ int64_t range[2];
   const int q = q0 + (int)blockIdx.y;
   const int64_t c0 = (int64_t)blockIdx.x * kTile;
   const int n = (int)min((int64_t)kTile, n_chunks - c0);
   for (int i = threadIdx.x; i < n; i += blockDim.x) acc[i] = 0.0;
-  const double avgdl = kGlobal ? bm25_avgdl((double)gstats[0], (double)gstats[1]) : corpus[2];
+  const double avgdl = bm25_avgdl((double)stats[0], (double)stats[1]);
   const double k1p1 = __dadd_rn(k1, 1.0), one_minus_b = __dsub_rn(1.0, b);
   const int j0 = q_off[q], j1 = q_off[q + 1];
   for (int j = j0; j < j1; ++j) {
@@ -133,7 +124,7 @@ __global__ void __launch_bounds__(kScoreThreads) bm25_score_kernel(
     }
     __syncthreads();
     const int64_t p0 = range[0], p1 = range[1];
-    const double w = kGlobal ? bm25_idf((double)gstats[0], (double)gstats[2 + j]) : idf[t];
+    const double w = bm25_idf((double)stats[0], (double)stats[2 + j]);
     for (int64_t p = p0 + threadIdx.x; p < p1; p += blockDim.x) {
       const int c = doc[p];
       const double f = (double)tf[p];
@@ -151,7 +142,7 @@ __global__ void __launch_bounds__(kScoreThreads) bm25_score_kernel(
   }
 }
 
-// ---- rl_bm25_topk: top k of one query ------------------------------------------------------------------------------------
+// ---- rl_bm25_topk_global: top k of one query -----------------------------------------------------------------------------
 // Radix digits of the composite (key: bits 95..32, ~chunk: bits 31..0), most significant first.
 struct Digit {
   int8_t part;   // 1: key, 0: ~chunk
@@ -166,13 +157,12 @@ __device__ __forceinline__ bool ge_prefix(uint64_t key, uint32_t lo, uint64_t m_
   return a > p_hi || (a == p_hi && (lo & m_lo) >= p_lo);
 }
 
-// kGlobal: out_chunk holds chunk_base + chunk (the shard's global numbering).  chunk_base is the last parameter for the
-// reason given at the score kernel.  With n_chunks == 0 (an empty shard) nothing is read and every row comes out empty.
-template <bool kGlobal>
+// out_chunk holds chunk_base + chunk (the shard's global numbering).  With n_chunks == 0 (an empty shard) nothing is read
+// and every row comes out empty.
 __global__ void __launch_bounds__(kSelectThreads) bm25_select_kernel(const uint64_t* __restrict__ keys, int64_t n_chunks, int q0,
-                                                                     int k, int64_t* __restrict__ out_chunk,
-                                                                     double* __restrict__ out_score, int32_t* __restrict__ out_count,
-                                                                     int64_t chunk_base) {
+                                                                     int k, int64_t chunk_base, int64_t* __restrict__ out_chunk,
+                                                                     double* __restrict__ out_score,
+                                                                     int32_t* __restrict__ out_count) {
   extern __shared__ __align__(16) unsigned char smem[];
   uint64_t* s_key = reinterpret_cast<uint64_t*>(smem);              // [kBm25MaxK]
   int32_t* s_chunk = reinterpret_cast<int32_t*>(s_key + kBm25MaxK);  // [kBm25MaxK]
@@ -297,7 +287,7 @@ __global__ void __launch_bounds__(kSelectThreads) bm25_select_kernel(const uint6
   double* os = out_score + (int64_t)q * k;
   for (int i = tid; i < k; i += blockDim.x) {
     if (i < m) {
-      oc[i] = kGlobal ? chunk_base + s_chunk[i] : s_chunk[i];
+      oc[i] = chunk_base + s_chunk[i];
       os[i] = __longlong_as_double((long long)(s_key[i] & ~kSign));
     } else {
       oc[i] = -1;
@@ -305,57 +295,6 @@ __global__ void __launch_bounds__(kSelectThreads) bm25_select_kernel(const uint6
     }
   }
   if (tid == 0) out_count[q] = m;
-}
-
-// ---- rl_bm25_local_stats ---------------------------------------------------------------------------------------------
-// Block 0: this shard's live N and sum of doc_len; block 1 + i (grid-stride): the live df of entry i.  Integers only,
-// so the sum over the shards is exact whatever order the all-reduce adds them in.
-constexpr int kStatThreads = 256;
-__global__ void __launch_bounds__(kStatThreads) bm25_local_stats_kernel(
-    const int64_t* __restrict__ term_off, const int32_t* __restrict__ doc, const int32_t* __restrict__ doc_len,
-    const uint8_t* __restrict__ alive, int64_t n_terms, int64_t n_chunks, const int32_t* __restrict__ q_terms,
-    int64_t n_entries, int64_t* __restrict__ out) {
-  __shared__ long long s_a[kStatThreads / 32], s_b[kStatThreads / 32];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (blockIdx.x == 0) {
-    long long n = 0, len = 0;
-    for (int64_t c = threadIdx.x; c < n_chunks; c += blockDim.x) {
-      if (alive == nullptr || alive[c]) {
-        ++n;
-        len += doc_len[c];
-      }
-    }
-    for (int off = 16; off > 0; off >>= 1) {
-      n += __shfl_down_sync(0xffffffffu, n, off);
-      len += __shfl_down_sync(0xffffffffu, len, off);
-    }
-    if (lane == 0) { s_a[warp] = n; s_b[warp] = len; }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      long long tn = 0, tl = 0;
-      for (int w = 0; w < kStatThreads / 32; ++w) { tn += s_a[w]; tl += s_b[w]; }
-      out[0] = tn;
-      out[1] = tl;
-    }
-    return;
-  }
-  for (int64_t j = blockIdx.x - 1; j < n_entries; j += gridDim.x - 1) {
-    const int t = q_terms[j];
-    long long cnt = 0;
-    if (t >= 0 && (int64_t)t < n_terms) {   // uniform over the CTA
-      for (int64_t p = term_off[t] + threadIdx.x; p < term_off[t + 1]; p += blockDim.x)
-        cnt += (alive == nullptr || alive[doc[p]]) ? 1 : 0;
-    }
-    for (int off = 16; off > 0; off >>= 1) cnt += __shfl_down_sync(0xffffffffu, cnt, off);
-    if (lane == 0) s_a[warp] = cnt;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      long long df = 0;
-      for (int w = 0; w < kStatThreads / 32; ++w) df += s_a[w];
-      out[2 + j] = df;
-    }
-    __syncthreads();
-  }
 }
 
 // ---- rl_bm25_merge_packed ----------------------------------------------------------------------------------------------
@@ -482,15 +421,15 @@ __global__ void __launch_bounds__(kMergeThreads) bm25_merge_kernel(const unsigne
 using namespace rl;
 
 extern "C" int rl_bm25_stats(const int64_t* term_off, const int32_t* doc, const int32_t* doc_len, const uint8_t* chunk_alive,
-                             int64_t n_terms, int64_t n_chunks, int32_t* df, double* idf, double* corpus, void* stream) {
+                             int64_t n_terms, int64_t n_chunks, int32_t* df, double* corpus, void* stream) {
   RL_REQUIRE(n_terms >= 0 && n_chunks >= 0 && n_chunks <= INT32_MAX, RL_EINVAL, "rl_bm25_stats: bad sizes");
-  RL_REQUIRE(term_off && corpus && (n_chunks == 0 || doc_len) && (n_terms == 0 || (doc && idf)), RL_EINVAL,
+  RL_REQUIRE(term_off && corpus && (n_chunks == 0 || doc_len) && (n_terms == 0 || (doc && df)), RL_EINVAL,
              "rl_bm25_stats: null pointer");
   bm25_corpus_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(doc_len, chunk_alive, n_chunks, corpus);
   RL_CUDA_CHECK(cudaGetLastError());
   if (n_terms > 0) {
     const int grid = (int)std::min<int64_t>(n_terms, 1 << 16);
-    bm25_idf_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(term_off, doc, chunk_alive, n_terms, corpus, df, idf);
+    bm25_df_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(term_off, doc, chunk_alive, n_terms, df);
     RL_CUDA_CHECK(cudaGetLastError());
   }
   return RL_OK;
@@ -501,55 +440,6 @@ extern "C" size_t rl_bm25_workspace_bytes(int64_t n_chunks, int group) {
   return (size_t)group * (size_t)n_chunks * sizeof(uint64_t);
 }
 
-extern "C" int rl_bm25_topk(const int64_t* term_off, const int32_t* doc, const int32_t* tf, const int32_t* doc_len,
-                            const double* idf, const double* corpus, int64_t n_terms, int64_t n_chunks,
-                            const uint8_t* chunk_mask, const int32_t* q_off, const int32_t* q_terms, int B, int k, double k1,
-                            double b, int64_t* out_chunk, double* out_score, int32_t* out_count, void* workspace,
-                            size_t workspace_bytes, void* stream) {
-  RL_REQUIRE(B >= 0 && n_terms >= 0 && n_chunks >= 1 && n_chunks <= INT32_MAX, RL_EINVAL, "rl_bm25_topk: bad sizes");
-  RL_REQUIRE(k >= 1 && k <= kBm25MaxK, RL_EINVAL, "rl_bm25_topk: k=%d outside [1, %d]", k, kBm25MaxK);
-  RL_REQUIRE(k1 >= 0.0 && b >= 0.0 && b <= 1.0, RL_EINVAL, "rl_bm25_topk: k1 must be >= 0 and b in [0, 1]");
-  if (B == 0) return RL_OK;
-  RL_REQUIRE(term_off && doc_len && idf && corpus && q_off && out_chunk && out_score && out_count && workspace &&
-                 (n_terms == 0 || (doc && tf)),
-             RL_EINVAL, "rl_bm25_topk: null pointer");
-  RL_REQUIRE(((uintptr_t)workspace & 7) == 0, RL_EINVAL, "rl_bm25_topk: workspace must be 8-byte aligned");
-  const int64_t group64 = (int64_t)(workspace_bytes / ((size_t)n_chunks * sizeof(uint64_t)));
-  RL_REQUIRE(group64 >= 1, RL_ENOSPACE, "rl_bm25_topk: workspace of %zu bytes holds no query (needs %zu)", workspace_bytes,
-             rl_bm25_workspace_bytes(n_chunks, 1));
-  const int group = (int)std::min<int64_t>(std::min<int64_t>(group64, B), 65535);
-  const size_t sel_smem = (size_t)kBm25MaxK * (sizeof(uint64_t) + sizeof(int32_t)) + kSelBins * sizeof(uint32_t);
-  RL_CUDA_CHECK(cudaFuncSetAttribute(bm25_select_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sel_smem));
-  const unsigned n_tiles = (unsigned)((n_chunks + kTile - 1) / kTile);
-  uint64_t* keys = static_cast<uint64_t*>(workspace);
-  cudaStream_t st = (cudaStream_t)stream;
-  for (int q0 = 0; q0 < B; q0 += group) {
-    const int g = min(group, B - q0);
-    bm25_score_kernel<false><<<dim3(n_tiles, g), kScoreThreads, 0, st>>>(term_off, doc, tf, doc_len, idf, corpus, n_terms,
-                                                                         n_chunks, chunk_mask, q_off, q_terms, q0, k1, b, keys,
-                                                                         nullptr);
-    RL_CUDA_CHECK(cudaGetLastError());
-    bm25_select_kernel<false><<<g, kSelectThreads, sel_smem, st>>>(keys, n_chunks, q0, k, out_chunk, out_score, out_count, 0);
-    RL_CUDA_CHECK(cudaGetLastError());
-  }
-  return RL_OK;
-}
-
-// ---- the sharded path: rl_bm25_local_stats -> all-reduce -> rl_bm25_topk_global -> all-gather -> rl_bm25_merge_packed --
-extern "C" int rl_bm25_local_stats(const int64_t* term_off, const int32_t* doc, const int32_t* doc_len,
-                                   const uint8_t* chunk_alive, int64_t n_terms, int64_t n_chunks, const int32_t* q_terms,
-                                   int64_t n_entries, int64_t* out, void* stream) {
-  RL_REQUIRE(n_terms >= 0 && n_chunks >= 0 && n_chunks <= INT32_MAX && n_entries >= 0, RL_EINVAL,
-             "rl_bm25_local_stats: bad sizes");
-  RL_REQUIRE(term_off && out && (n_chunks == 0 || doc_len) && (n_entries == 0 || q_terms) && (n_terms == 0 || n_chunks == 0 || doc),
-             RL_EINVAL, "rl_bm25_local_stats: null pointer");
-  const int grid = 1 + (int)std::min<int64_t>(n_entries, 1 << 16);
-  bm25_local_stats_kernel<<<grid, kStatThreads, 0, (cudaStream_t)stream>>>(term_off, doc, doc_len, chunk_alive, n_terms,
-                                                                            n_chunks, q_terms, n_entries, out);
-  RL_CUDA_CHECK(cudaGetLastError());
-  return RL_OK;
-}
-
 extern "C" size_t rl_bm25_packed_bytes(int B, int k) {
   if (B <= 0 || k <= 0) return 0;
   const size_t raw = (size_t)B * (size_t)k * 16 + (size_t)B * 4;
@@ -557,7 +447,7 @@ extern "C" size_t rl_bm25_packed_bytes(int B, int k) {
 }
 
 extern "C" int rl_bm25_topk_global(const int64_t* term_off, const int32_t* doc, const int32_t* tf, const int32_t* doc_len,
-                                   const int64_t* global_stats, int64_t n_terms, int64_t n_chunks, const uint8_t* chunk_mask,
+                                   const int64_t* stats, int64_t n_terms, int64_t n_chunks, const uint8_t* chunk_mask,
                                    const int32_t* q_off, const int32_t* q_terms, int B, int k, double k1, double b,
                                    int64_t chunk_base, void* out_packed, void* workspace, size_t workspace_bytes,
                                    void* stream) {
@@ -566,7 +456,7 @@ extern "C" int rl_bm25_topk_global(const int64_t* term_off, const int32_t* doc, 
   RL_REQUIRE(k >= 1 && k <= kBm25MaxK, RL_EINVAL, "rl_bm25_topk_global: k=%d outside [1, %d]", k, kBm25MaxK);
   RL_REQUIRE(k1 >= 0.0 && b >= 0.0 && b <= 1.0, RL_EINVAL, "rl_bm25_topk_global: k1 must be >= 0 and b in [0, 1]");
   if (B == 0) return RL_OK;
-  RL_REQUIRE(term_off && global_stats && q_off && out_packed && (n_chunks == 0 || (doc_len && workspace)) &&
+  RL_REQUIRE(term_off && stats && q_off && out_packed && (n_chunks == 0 || (doc_len && workspace)) &&
                  (n_terms == 0 || n_chunks == 0 || (doc && tf)),
              RL_EINVAL, "rl_bm25_topk_global: null pointer");
   RL_REQUIRE(((uintptr_t)out_packed & 15) == 0 && ((uintptr_t)workspace & 7) == 0, RL_EINVAL,
@@ -587,19 +477,18 @@ extern "C" int rl_bm25_topk_global(const int64_t* term_off, const int32_t* doc, 
   const size_t used = bk * 16 + (size_t)B * 4, total = rl_bm25_packed_bytes(B, k);
   if (total > used) RL_CUDA_CHECK(cudaMemsetAsync(out + used, 0, total - used, st));   // the padding travels too
   const size_t sel_smem = (size_t)kBm25MaxK * (sizeof(uint64_t) + sizeof(int32_t)) + kSelBins * sizeof(uint32_t);
-  RL_CUDA_CHECK(cudaFuncSetAttribute(bm25_select_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sel_smem));
+  RL_CUDA_CHECK(cudaFuncSetAttribute(bm25_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sel_smem));
   const unsigned n_tiles = (unsigned)((n_chunks + kTile - 1) / kTile);
   uint64_t* keys = static_cast<uint64_t*>(workspace);
   for (int q0 = 0; q0 < B; q0 += group) {
     const int g = min(group, B - q0);
     if (n_chunks > 0) {
-      bm25_score_kernel<true><<<dim3(n_tiles, g), kScoreThreads, 0, st>>>(term_off, doc, tf, doc_len, nullptr, nullptr,
-                                                                          n_terms, n_chunks, chunk_mask, q_off, q_terms, q0,
-                                                                          k1, b, keys, global_stats);
+      bm25_score_kernel<<<dim3(n_tiles, g), kScoreThreads, 0, st>>>(term_off, doc, tf, doc_len, stats, n_terms, n_chunks,
+                                                                    chunk_mask, q_off, q_terms, q0, k1, b, keys);
       RL_CUDA_CHECK(cudaGetLastError());
     }
-    bm25_select_kernel<true><<<g, kSelectThreads, sel_smem, st>>>(keys, n_chunks, q0, k, out_chunk, out_score, out_count,
-                                                                  chunk_base);
+    bm25_select_kernel<<<g, kSelectThreads, sel_smem, st>>>(keys, n_chunks, q0, k, chunk_base, out_chunk, out_score,
+                                                            out_count);
     RL_CUDA_CHECK(cudaGetLastError());
   }
   return RL_OK;

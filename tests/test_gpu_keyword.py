@@ -1,5 +1,6 @@
-"""BM25 keyword search on the device (``rl_bm25_stats`` / ``rl_bm25_topk`` behind ``keyword_search`` and
-``hybrid_search``) against the NumPy oracle of DuckDB's FTS tables and ``match_bm25`` (``tests/keyword_oracle.py``)."""
+"""BM25 keyword search on a ``CorpusIndex`` (``rl_bm25_stats`` / ``rl_bm25_topk_global`` behind ``keyword_search`` and
+``hybrid_search``, one shard: no collective, no merge) against the NumPy oracle of DuckDB's FTS tables and
+``match_bm25`` (``tests/keyword_oracle.py``)."""
 
 from __future__ import annotations
 

@@ -1,6 +1,7 @@
 """BM25 keyword search on a ``ShardedIndex``: R thread ranks on one GPU (``thread_group``) run the real host pipeline --
-``Analyzer.query_plan``, ``rl_bm25_local_stats``, one all-reduce, ``rl_bm25_topk_global``, one all-gather and
-``rl_bm25_merge_packed`` -- against the bare ``CorpusIndex`` and the NumPy oracle of ``match_bm25``.
+``Analyzer.query_plan`` and the entries' statistics, one all-reduce, ``rl_bm25_topk_global``, one all-gather and
+``rl_bm25_merge_packed`` (R = 1: neither collective nor the merge) -- against the bare ``CorpusIndex`` and the NumPy
+oracle of ``match_bm25``.
 
 * The merge kernel, bit for bit against a NumPy restatement, on synthetic packed buffers.
 * Exactness: on a corpus whose single-index term ids follow sorted-stem order (chunk 0 holds every word, one per stem,

@@ -115,21 +115,18 @@ def test_oracle_hand_computed_example():
     assert ix3.num_docs == 2.0 and ix3.avgdl == 3.0 and match_bm25(ix3, "dog").keys() == {1}
 
 
-def test_c_abi_refusals_before_any_cuda_call():
+def test_stats_abi_refusals_before_any_cuda_call():
     from raglite_b200 import _lib
 
     lib = _lib.load()
     dummy = ctypes.c_void_p(16)
-    args = [dummy] * 6 + [10, 100, None, dummy, dummy, 4]
-    out = [dummy, dummy, dummy, dummy, 1 << 20, None]
-    assert lib.rl_bm25_topk(*args, 0, 1.2, 0.75, *out) == -1                 # k = 0
-    assert lib.rl_bm25_topk(*args, 4097, 1.2, 0.75, *out) == -1              # k above the cap
-    assert lib.rl_bm25_topk(*args, 10, 1.2, 1.5, *out) == -1                 # b outside [0, 1]
-    small = [dummy, dummy, dummy, dummy, 799, None]                          # 100 chunks need 800 bytes per query
-    assert lib.rl_bm25_topk(*args, 10, 1.2, 0.75, *small) == -3
-    assert "holds no query" in lib.rl_last_error().decode()
     assert lib.rl_bm25_workspace_bytes(100, 3) == 2400 and lib.rl_bm25_workspace_bytes(0, 3) == 0
-    assert lib.rl_bm25_stats(None, None, None, None, 1, 1, None, None, None, None) == -1
+    # rl_bm25_stats(term_off, doc, doc_len, alive, n_terms, n_chunks, df, corpus, stream)
+    assert lib.rl_bm25_stats(None, None, None, None, 1, 1, None, None, None) == -1
+    assert lib.rl_bm25_stats(dummy, dummy, dummy, None, 10, 100, None, dummy, None) == -1      # df
+    assert lib.rl_bm25_stats(dummy, dummy, dummy, None, 10, 100, dummy, None, None) == -1      # corpus
+    assert lib.rl_bm25_stats(dummy, dummy, dummy, None, -1, 100, dummy, dummy, None) == -1     # n_terms < 0
+    assert "rl_bm25_stats" in lib.rl_last_error().decode()
 
 
 def test_keyword_search_refusals_without_a_device():

@@ -1,5 +1,5 @@
 """Sharded BM25 keyword search, host side: the query plan every rank builds (``Analyzer.query_plan``), the packed
-buffer's size, and the C-ABI refusals of the sharded entry points (no GPU needed)."""
+buffer's size, and the C-ABI refusals of the top-k and merge entry points (no GPU needed)."""
 
 from __future__ import annotations
 
@@ -61,19 +61,11 @@ def test_packed_bytes_of_nothing():
     assert lib.rl_bm25_packed_bytes(0, 10) == 0 and lib.rl_bm25_packed_bytes(10, 0) == 0 and lib.rl_bm25_packed_bytes(-1, 5) == 0
 
 
-def test_c_abi_refusals_before_any_cuda_call():
+def test_topk_and_merge_abi_refusals_before_any_cuda_call():
     from raglite_b200 import _lib
 
     lib = _lib.load()
     d = ctypes.c_void_p(16)
-    # rl_bm25_local_stats(term_off, doc, doc_len, alive, n_terms, n_chunks, q_terms, n_entries, out, stream)
-    assert lib.rl_bm25_local_stats(None, d, d, None, 10, 100, d, 3, d, None) == -1             # term_off
-    assert lib.rl_bm25_local_stats(d, d, d, None, 10, 100, d, 3, None, None) == -1             # out
-    assert lib.rl_bm25_local_stats(d, d, d, None, 10, 100, None, 3, d, None) == -1             # q_terms
-    assert lib.rl_bm25_local_stats(d, d, None, None, 10, 100, d, 3, d, None) == -1             # doc_len
-    assert lib.rl_bm25_local_stats(d, d, d, None, 10, 100, d, -1, d, None) == -1               # n_entries < 0
-    assert "rl_bm25_local_stats" in lib.rl_last_error().decode()
-
     # rl_bm25_topk_global(term_off, doc, tf, doc_len, stats, n_terms, n_chunks, mask, q_off, q_terms, B, k, k1, b,
     #                     chunk_base, out_packed, workspace, workspace_bytes, stream)
     def topk(k=10, b=0.75, base=0, out=d, stats=d, ws=d, ws_bytes=1 << 20, B=4):

@@ -1,17 +1,17 @@
-"""BM25 keyword search throughput (``keyword_search_batch``: ``rl_bm25_topk`` over the device postings) on one GPU, next
-to the NumPy port of DuckDB's FTS tables and ``match_bm25`` (tests/keyword_oracle.py) on the host cores.
+"""BM25 keyword search throughput (``keyword_search_batch``: ``rl_bm25_topk_global`` over the device postings) on one GPU,
+next to the NumPy port of DuckDB's FTS tables and ``match_bm25`` (tests/keyword_oracle.py) on the host cores.
 
 Corpus: seeded, ``--chunks`` bodies (default 1.25 M, the chunk count of the headline shard) of 0-600 words drawn from a
 Zipf distribution over a generated vocabulary.  Queries: ``--batch`` queries of 3-12 words from the same distribution,
 top ``--k`` (256 x top-64: what ``hybrid_search`` asks for under ``search_and_rerank_chunks``' defaults, 2 x 4 x 8).
 Prints one JSON line: index build time (host analysis / device postings / statistics), queries/s end to end, CUDA-event
-time of the top-k launches, per-kernel device times (torch.profiler), algorithmic bytes over kernel time against the
+time of the top-k launch, per-kernel device times (torch.profiler), algorithmic bytes over kernel time against the
 H100's 3.35 TB/s, the port's queries/s for ``--oracle-queries`` queries, and how many of those the device matched.
 At the default size the host stages dominate the run (generating 375 M words, analysing them for the index and again for
 the port): about ten minutes on a 16-thread host; ``--chunks 250000`` takes about three.
 ``--shards 1`` adds the sharded path on one GPU: ``ShardedIndex(group=None)`` over the same index against the bare index
-(per-batch medians, alternating), CUDA-event times of ``rl_bm25_local_stats``, ``rl_bm25_topk_global`` and
-``rl_bm25_merge_packed``, and the merge alone on synthetic full lists at R = 2, 8 and k = 64, 4096 (B = 256)."""
+(per-batch medians, alternating), and ``rl_bm25_merge_packed`` alone on synthetic full lists at R = 2, 8 and k = 64, 4096
+(B = 256)."""
 import argparse, json, operator, subprocess, sys, time
 from pathlib import Path
 ROOT = Path(__file__).resolve().parents[1]
@@ -31,7 +31,7 @@ ap.add_argument("--oracle-queries", type=int, default=16)
 ap.add_argument("--seed", type=int, default=0)
 ap.add_argument("--shards", type=int, default=0,
                 help="1: also time the sharded path (ShardedIndex(group=None)) against the bare index, alternating, "
-                     "its three kernels, and the merge alone at R = 2, 8 and k = 64, 4096")
+                     "and the merge alone at R = 2, 8 and k = 64, 4096")
 args = ap.parse_args()
 if args.shards not in (0, 1):
     sys.exit("--shards: only 1 (one GPU) is implemented; a multi-GPU run under torchrun is not")
@@ -87,27 +87,28 @@ for _ in range(args.reps):
     wall.append(time.perf_counter() - t0)
 
 stage("end-to-end timed")
-# device time of the launches alone: queries uploaded once, CUDA events around rl_bm25_topk
+# device time of the top-k launch alone: the plan and its statistics built as KeywordIndex.topk_to_host builds them for
+# a CorpusIndex and uploaded once, CUDA events around rl_bm25_topk_global
 from raglite_b200 import _lib
 from raglite_b200._keyword import B_PARAM, K1
 
 B, C, k = len(queries), kw.n_chunks, args.k
 qids = [kw.analyzer.query_ids(q) for q in queries]
 q_off = np.concatenate([[0], np.cumsum([len(x) for x in qids])]).astype(np.int32)
-qd = torch.from_numpy(np.concatenate([q_off, *qids]).astype(np.int32)).cuda()
+ids = np.concatenate(qids).astype(np.int32)
+stats_d = torch.from_numpy(np.concatenate([[kw.n_live, kw.sum_len], kw.df_host[ids]]).astype(np.int64)).cuda()
+qd = torch.from_numpy(np.concatenate([q_off, ids])).cuda()
 group = max(1, min(B, (1 << 30) // (8 * C)))
 need = int(kw.lib.rl_bm25_workspace_bytes(C, group))
 ws = torch.empty(need, dtype=torch.uint8, device="cuda")
-oc = torch.empty((B, k), dtype=torch.int64, device="cuda")
-osc = torch.empty((B, k), dtype=torch.float64, device="cuda")
-ocn = torch.empty(B, dtype=torch.int32, device="cuda")
+packed = torch.empty(int(kw.lib.rl_bm25_packed_bytes(B, k)), dtype=torch.uint8, device="cuda")
 
 
 def launch():
-    _lib.check(kw.lib.rl_bm25_topk(kw.term_off.data_ptr(), kw.doc.data_ptr(), kw.tf.data_ptr(), kw.doc_len.data_ptr(),
-                                   kw.idf.data_ptr(), kw.corpus.data_ptr(), kw.n_terms, C, None, qd.data_ptr(),
-                                   qd.data_ptr() + 4 * (B + 1), B, k, K1, B_PARAM, oc.data_ptr(), osc.data_ptr(), ocn.data_ptr(),
-                                   ws.data_ptr(), need, torch.cuda.current_stream().cuda_stream), "rl_bm25_topk")
+    _lib.check(kw.lib.rl_bm25_topk_global(kw.term_off.data_ptr(), kw.doc.data_ptr(), kw.tf.data_ptr(), kw.doc_len.data_ptr(),
+                                          stats_d.data_ptr(), kw.n_terms, C, None, qd.data_ptr(), qd.data_ptr() + 4 * (B + 1),
+                                          B, k, K1, B_PARAM, 0, packed.data_ptr(), ws.data_ptr(), need,
+                                          torch.cuda.current_stream().cuda_stream), "rl_bm25_topk_global")
 
 
 launch()
@@ -157,7 +158,6 @@ if args.shards == 1:
     sh = ShardedIndex(idx)
     s_ids, s_sc, s_cnt = rl.keyword_search_batch(queries, num_results=k, index=sh)
     sharded["sharded_same_counts"] = bool(np.array_equal(s_cnt, counts_))
-    # the sum runs over sorted stems instead of first-appearance ids: scores agree to the last bits, not bit for bit
     n_ok = [np.allclose(s_sc[b, :counts_[b]], scores_[b, :counts_[b]], rtol=1e-12, atol=0) for b in range(B)]
     sharded["sharded_scores_within_1e-12"] = f"{sum(n_ok)}/{B}"
     t_bare, t_sh = [], []
@@ -170,26 +170,7 @@ if args.shards == 1:
         t_sh.append(time.perf_counter() - t0)
     sharded["bare_batch_ms_median"] = 1e3 * float(np.median(t_bare))
     sharded["sharded_r1_batch_ms_median"] = 1e3 * float(np.median(t_sh))
-    # the three kernels of the sharded path alone, CUDA events around `reps` launches each
-    q_off_s, _, ids_s = kw.analyzer.query_plan(queries)
-    J = len(ids_s)
-    qs = torch.from_numpy(np.concatenate([q_off_s, ids_s]).astype(np.int32)).cuda()
     st = torch.cuda.current_stream().cuda_stream
-    gstats = torch.empty(2 + J, dtype=torch.int64, device="cuda")
-    nb = int(kw.lib.rl_bm25_packed_bytes(B, k))
-    packed = torch.empty(nb, dtype=torch.uint8, device="cuda")
-    merged = torch.empty(nb, dtype=torch.uint8, device="cuda")
-
-    def local_stats():
-        _lib.check(kw.lib.rl_bm25_local_stats(kw.term_off.data_ptr(), kw.doc.data_ptr(), kw.doc_len.data_ptr(), None,
-                                              kw.n_terms, C, qs.data_ptr() + 4 * (B + 1), J, gstats.data_ptr(), st),
-                   "rl_bm25_local_stats")
-
-    def topk_global():
-        _lib.check(kw.lib.rl_bm25_topk_global(kw.term_off.data_ptr(), kw.doc.data_ptr(), kw.tf.data_ptr(),
-                                              kw.doc_len.data_ptr(), gstats.data_ptr(), kw.n_terms, C, None, qs.data_ptr(),
-                                              qs.data_ptr() + 4 * (B + 1), B, k, K1, B_PARAM, 0, packed.data_ptr(),
-                                              ws.data_ptr(), need, st), "rl_bm25_topk_global")
 
     def merge(src, R, Bm, km, dst):
         _lib.check(kw.lib.rl_bm25_merge_packed(src.data_ptr(), R, Bm, km, dst.data_ptr(), dst.data_ptr() + Bm * km * 8,
@@ -205,9 +186,6 @@ if args.shards == 1:
         torch.cuda.synchronize()
         return e[0].elapsed_time(e[1]) / args.reps
 
-    sharded["local_stats_ms"] = event_ms(local_stats)
-    sharded["topk_global_ms"] = event_ms(topk_global)
-    sharded["merge_r1_ms"] = event_ms(lambda: merge(packed, 1, B, k, merged))
     # the merge alone on synthetic full lists: R shards x B queries x k entries, sorted, unique global chunks
     for R in (2, 8):
         for km in (64, 4096):
