@@ -34,6 +34,9 @@ extern "C" {
 #define RL_METRIC_COSINE 0 /* dist = 1 - <e,q>/sqrt(|e|^2 |q|^2)  (array_cosine_distance)        */
 #define RL_METRIC_DOT 1    /* dist = -<e,q>                        (array_negative_inner_product) */
 #define RL_METRIC_L2 2     /* dist = |e - q|_2                     (array_distance)               */
+#define RL_METRIC_L1 3     /* dist = sum_i |e_i - q_i|             (PostgreSQL only: pgvector `<+>`, HNSW
+                              index halfvec_l1_ops; _typing.py:110-120, _database.py:573-578).  Runs the
+                              CUDA-core L1 scan under RL_ALGO_AUTO and RL_ALGO_FP32; RL_ALGO_TCGEN05 is refused. */
 
 /* Scan kernel selection. */
 #define RL_ALGO_AUTO 0
@@ -50,6 +53,8 @@ extern "C" {
 #define RL_STATUS_CAND_OVERFLOW 1 /* candidate list overflowed: call again with REUSE_THRESHOLDS */
 #define RL_STATUS_TIE_OVERFLOW 2  /* reserved (never set since v101: more than RL_MAX_SURVIVORS rows inside the error
                                      band of the cut are rescored by a streaming pass over the candidate list) */
+#define RL_STATUS_QUERY_NONFINITE 4 /* RL_METRIC_L1 only: the query has an infinite or NaN element (pgvector refuses
+                                       such a halfvec); the hits of that query are meaningless */
 
 #define RL_MAX_SURVIVORS 4096
 
@@ -129,7 +134,8 @@ typedef struct rl_scan_params {
   int32_t sample_stride; /* 0 = auto */
   int32_t cand_cap;      /* 0 = auto */
   int32_t e_dtype;       /* storage of E: 0 = float32, 1 = float16 (E then points to IEEE binary16; needs
-                            RL_ALGO_TCGEN05, d % 8 == 0 and rows that need no per-row scaling) */
+                            d % 8 == 0, ld % 8 == 0 and 16-byte aligned E, and then RL_ALGO_TCGEN05 with rows that
+                            need no per-row scaling for cosine / dot / l2, the L1 scan for RL_METRIC_L1) */
   int32_t rows_unit_scale; /* 1: the caller guarantees (from the rl_row_stats statistics: max 1/|e| <= 2, max |e_ij| <= 1024,
                             no all-zero row -- true for normalised embeddings) that rows can enter the fp16 scan unscaled,
                             which lets the cosine scan use the two-tiles-per-query-slice kernel.  0: unknown (always valid) */
@@ -162,8 +168,9 @@ int rl_maxsim_stats(const rl_scan_params* p, const void* workspace, rl_scan_stat
  * of its num_hits filtered hits: every emission threshold the scan ever used lies at or below that hit's key, so
  * the rows counted against the thresholds (allowed ones = the candidate count, masked ones = the extra counter)
  * plus the whole sample are a superset.  bound <= 1 000 000 proves that the filter-first answer is also the
- * rank-then-filter answer, without the second pass over the corpus rl_maxsim_count_at_least needs.  Returns
- * RL_EUNSUPPORTED when the last call did not count (fp32 scan, flag not set).  An empty shard (p->n_rows == 0)
+ * rank-then-filter answer, without the second pass over the corpus rl_maxsim_count_at_least needs.  The
+ * tensor-core scan and the L1 scan count; bound[b] is -1 when the last call did not count (fp32 scan of cosine / dot /
+ * l2, flag not set).  An empty shard (p->n_rows == 0)
  * gets bound 0 without the workspace being read: rl_maxsim_topk writes nothing there for it. */
 int rl_maxsim_unfiltered_bound(const rl_scan_params* p, const void* workspace, int64_t* bound, void* stream);
 

@@ -78,7 +78,9 @@ class RAGLiteConfig:
     # Chunk config used to partition documents into chunks.
     chunk_max_size: int = 2048
     # Vector search config.
-    vector_search_distance_metric: Literal["cosine", "dot", "l2"] = "cosine"
+    # "l1" is not in the reference's annotation, but its PostgreSQL layer renders it (pgvector `<+>`,
+    # _typing.py:110-120; halfvec_l1_ops, _database.py:573-578), so PostgreSQL configs may carry it.
+    vector_search_distance_metric: Literal["cosine", "dot", "l2", "l1"] = "cosine"
     vector_search_multivector: bool = True
     vector_search_query_adapter: bool = True
     # Reranking config: anything with ``.rank(query=, docs=)`` -> ``.results[i].doc_id``.

@@ -32,8 +32,8 @@ import torch
 import torch.distributed as dist
 
 from . import _lib
-from ._lib import (RL_ALGO, RL_FLAG_COUNT_UNFILTERED, RL_FLAG_REUSE_THRESHOLDS, RL_METRIC, RL_STATUS_CAND_OVERFLOW, ScanParams,
-                   ScanStats, check)
+from ._lib import (RL_ALGO, RL_FLAG_COUNT_UNFILTERED, RL_FLAG_REUSE_THRESHOLDS, RL_METRIC, RL_STATUS_CAND_OVERFLOW,
+                   RL_STATUS_QUERY_NONFINITE, ScanParams, ScanStats, check)
 from ._typing import ChunkId
 
 
@@ -859,6 +859,14 @@ class CorpusIndex:
 MAX_SCAN_RUNS = 16
 
 
+def raise_if_query_nonfinite(status: Any) -> None:
+    """``RL_STATUS_QUERY_NONFINITE`` in any status word (an int or an int tensor) -> ``ValueError``: an ``l1`` query
+    with an infinite or NaN element, which pgvector refuses as a ``halfvec``."""
+    bad = status & RL_STATUS_QUERY_NONFINITE
+    if bool(bad.any()) if isinstance(bad, torch.Tensor) else bad:
+        raise ValueError("a query element is not finite in float16: pgvector refuses such a halfvec")
+
+
 def run_until_no_overflow(local: "CorpusIndex", run: Callable[[int, int], Any], *, flags: int = 0,
                           cand_cap: int = 0) -> None:
     """The candidate-overflow policy of every search.  ``run(flags, cand_cap)`` enqueues one search and returns its
@@ -871,7 +879,9 @@ def run_until_no_overflow(local: "CorpusIndex", run: Callable[[int, int], Any], 
     gathered status, stop together; running out of runs raises ``RagliteB200Error``."""
     cap, fl = cand_cap, flags
     for n_run in range(1, MAX_SCAN_RUNS + 1):
-        overflow = run(fl, cap) & RL_STATUS_CAND_OVERFLOW
+        st = run(fl, cap)
+        raise_if_query_nonfinite(st)   # (a non-finite l1 query can overflow every list: never retried)
+        overflow = st & RL_STATUS_CAND_OVERFLOW
         if not (bool(overflow.any()) if isinstance(overflow, torch.Tensor) else overflow):   # (a tensor synchronises)
             return
         if n_run % 2 == 1:
@@ -937,8 +947,8 @@ def search_to_host(  # noqa: PLR0913
                 neg = index.sum_over_shards((local.unfiltered_bound() < 0).to(torch.int64))   # any shard that did not count
                 ids, sims, counts, st, ub = local.to_host(sim, chunk, count, status, torch.where(neg > 0, -1, bound))
                 out = ids, sims, counts
-                if st & RL_STATUS_CAND_OVERFLOW or (ub.min() >= 0 and ub.max() <= rank_first_limit):
-                    return st
+                if st & (RL_STATUS_CAND_OVERFLOW | RL_STATUS_QUERY_NONFINITE) or (ub.min() >= 0 and ub.max() <= rank_first_limit):
+                    return st   # (a non-finite query raises in the caller; it never reaches the counting passes)
                 fused = False       # not provable from the counters: run the explicit rank probe
             ids, sims, counts, st = local.to_host(*index.search_pipeline(Q, **kw, flags=flags, cand_cap=cand_cap,
                                                                          rank_first_limit=rank_first_limit))
@@ -975,6 +985,9 @@ class PendingSearch:
             slot = self._slot
             self._event.synchronize()
             ids, sims, counts, st = CorpusIndex._parse_result(slot.host.numpy(), self._B, self._k)
+            if st & RL_STATUS_QUERY_NONFINITE:
+                slot.busy = False
+                raise_if_query_nonfinite(st)
             if st & RL_STATUS_CAND_OVERFLOW:
                 with torch.cuda.stream(slot.stream):
                     ids, sims, counts = search_to_host(self._index, self._Q, **self._kw)

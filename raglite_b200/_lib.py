@@ -12,13 +12,14 @@ import threading
 
 from . import _build
 
-RL_METRIC = {"cosine": 0, "dot": 1, "l2": 2}
+RL_METRIC = {"cosine": 0, "dot": 1, "l2": 2, "l1": 3}
 RL_ALGO = {"auto": 0, "fp32": 1, "tcgen05": 2}
 RL_FLAG_REUSE_THRESHOLDS = 1
 RL_FLAG_TIME_KERNELS = 2
 RL_FLAG_COUNT_UNFILTERED = 4
 RL_STATUS_CAND_OVERFLOW = 1
 RL_STATUS_TIE_OVERFLOW = 2
+RL_STATUS_QUERY_NONFINITE = 4
 RL_MAX_SURVIVORS = 4096   # finalize window (include/raglite_b200.h)
 
 EXPORTS = [

@@ -49,13 +49,34 @@ def _filter_on_device(index: Any, metadata_filter: dict[str, list[Any]] | None) 
     return local.filter_chunks(metadata_filter)
 
 
+def halfvec_round(Q: torch.Tensor) -> torch.Tensor:
+    """The query as pgvector's ``halfvec`` holds it, as float32.  ``PostgresHalfVec.bind_processor``
+    (``_typing.py:157-163``) binds each element as the text ``str(x)``; pgvector parses it with ``strtof`` and rounds it to
+    binary16, to nearest even.  float32 and float16 elements are therefore rounded once (float16: not at all); float64
+    elements twice, to float32 and then to binary16.  An element beyond the binary16 range becomes +-inf here; pgvector
+    refuses it."""
+    return Q.to(torch.float32).to(torch.float16).to(torch.float32)
+
+
+def _check_metric(config: RAGLiteConfig) -> None:
+    """``l1`` exists on PostgreSQL only (pgvector's ``<+>``); the reference's DuckDB branch has no L1 function
+    (``_typing.py:125-129``)."""
+    if config.vector_search_distance_metric == "l1" and not str(config.db_url).startswith("postgresql"):
+        raise ValueError(f"vector_search_distance_metric='l1' needs a PostgreSQL db_url (pgvector's <+> operator); "
+                         f"db_url={config.db_url!r} has no L1 distance")
+
+
 def _plan_search(  # noqa: PLR0913
     queries: Any, *, num_results: int, oversample: int, metadata_filter: MetadataFilter | None, config: RAGLiteConfig | None,
     index: Any | None, exact_maxsim: bool, queries_are_fp16: bool,
 ) -> tuple[Any, torch.Tensor, tuple | None, dict[str, Any], Any]:
     """Argument handling shared by the synchronous and the asynchronous batched search: returns
-    ``(index, Q (as given, not yet on the device), empty result or None, search kwargs, prepare(Q_device))``."""
+    ``(index, Q (as given, not yet on the device), empty result or None, search kwargs, prepare(Q_device))``.
+    Under ``l1`` (PostgreSQL only) ``prepare`` rounds the adapted query to ``halfvec`` (``halfvec_round``).  A host
+    query that no adapter changes is range-checked here; any other query reports a non-finite element through the
+    result status (``RL_STATUS_QUERY_NONFINITE``) and the search raises after its one download."""
     config = config or RAGLiteConfig()
+    _check_metric(config)
     index = index if index is not None else get_index(config)
     if index is None:
         raise ValueError(f"No index registered for db_url={config.db_url!r}; use raglite_b200.register_index")
@@ -64,6 +85,10 @@ def _plan_search(  # noqa: PLR0913
     queries_are_fp16 = queries_are_fp16 or Q.dtype == torch.float16
     if Q.ndim != 2:
         raise ValueError("queries must be [B, d]")
+    halfvec = config.vector_search_distance_metric == "l1"
+    adapt = config.vector_search_query_adapter and local.query_adapter is not None
+    if halfvec and not adapt and Q.device.type == "cpu" and not bool(torch.isfinite(halfvec_round(Q)).all()):
+        raise ValueError("a query element is not finite in float16: pgvector refuses such a halfvec")
     k = int(num_results)
     B = int(Q.shape[0])
     sharded = hasattr(index, "group")
@@ -74,9 +99,12 @@ def _plan_search(  # noqa: PLR0913
     if not exact_maxsim and num_hits == 0:  # round(oversample * size / 2048) == 0 -> LIMIT 0
         return index, Q, empty, {}, None
     prepare = None
-    if config.vector_search_query_adapter and local.query_adapter is not None:
+    if adapt and not halfvec:
         def prepare(Qd: torch.Tensor) -> torch.Tensor:  # (A @ q).astype(q.dtype), _search.py:58-62
             return local.apply_adapter(Qd, round_fp16=queries_are_fp16)
+    elif halfvec:
+        def prepare(Qd: torch.Tensor) -> torch.Tensor:  # [adapter], then the query is bound as a halfvec
+            return halfvec_round(local.apply_adapter(Qd, round_fp16=queries_are_fp16) if adapt else Qd)
     chunk_ok, n_match = _filter_on_device(index, _adapt_metadata(metadata_filter))
     metric = config.vector_search_distance_metric
     # Which metadata branch the reference would take (_search.py:96-143): many matching rows in a corpus
@@ -160,6 +188,7 @@ def vector_search(
     (``_search.py:36-153``): embed / ravel the query, apply the query adapter, keep the
     ``num_hits`` nearest vectors, group by chunk with ``max(sim)``, return the best ``num_results``."""
     config = config or RAGLiteConfig()
+    _check_metric(config)
     index = get_index(config)
     if index is None:
         raise ValueError(f"No index registered for db_url={config.db_url!r}; use raglite_b200.register_index")

@@ -64,7 +64,7 @@ int make_layout(const rl_scan_params* p, int sm_count, Layout* L) {
   RL_REQUIRE(p->B >= 0 && p->B <= 65535, RL_EINVAL, "bad B");
   RL_REQUIRE(p->k > 0, RL_EINVAL, "k must be positive");
   RL_REQUIRE(p->num_hits >= 0, RL_EINVAL, "num_hits must be >= 0");
-  RL_REQUIRE(p->metric >= RL_METRIC_COSINE && p->metric <= RL_METRIC_L2, RL_EINVAL, "unknown metric %d", p->metric);
+  RL_REQUIRE(p->metric >= RL_METRIC_COSINE && p->metric <= RL_METRIC_L1, RL_EINVAL, "unknown metric %d", p->metric);
   RL_REQUIRE(p->max_vecs_per_chunk >= 1, RL_EINVAL, "max_vecs_per_chunk must be >= 1");
   RL_REQUIRE(p->e_dtype == 0 || p->e_dtype == 1, RL_EINVAL, "e_dtype must be 0 (float32) or 1 (float16)");
   memset(L, 0, sizeof(*L));
@@ -78,16 +78,26 @@ int make_layout(const rl_scan_params* p, int sm_count, Layout* L) {
   L->n_blocks = (p->n_rows + kBlockRows - 1) / kBlockRows;
 
   int algo = p->algo;
-  const bool tc_ok = wgmma_scan_supported(p);
-  if (algo == RL_ALGO_AUTO) algo = tc_ok ? RL_ALGO_TCGEN05 : RL_ALGO_FP32;
-  RL_REQUIRE(algo == RL_ALGO_FP32 || algo == RL_ALGO_TCGEN05, RL_EINVAL, "unknown algo %d", p->algo);
   // An empty shard (a sharded corpus with fewer chunks than ranks, or emptied by compact) scans nothing: every
   // entry point returns before its first launch, so it takes any storage and algo.
   const bool empty = p->n_rows == 0;
-  RL_REQUIRE(empty || p->e_dtype == 0 || algo == RL_ALGO_TCGEN05, RL_EUNSUPPORTED,
-             "float16 storage needs the tensor-core scan (d %% 8 == 0, ld %% 8 == 0, 16-byte aligned E)");
-  RL_REQUIRE(empty || algo != RL_ALGO_TCGEN05 || tc_ok, RL_EUNSUPPORTED,
-             "RL_ALGO_TCGEN05 needs d %% 4 == 0, ld %% 4 == 0, 16-byte aligned E and a supported metric");
+  if (p->metric == RL_METRIC_L1) {
+    // L1 has no GEMM form: AUTO and FP32 both run the CUDA-core L1 scan (scan_l1.cu), on either storage.
+    RL_REQUIRE(algo != RL_ALGO_TCGEN05, RL_EUNSUPPORTED, "the l1 metric has no tensor-core scan: use RL_ALGO_AUTO or RL_ALGO_FP32");
+    if (algo == RL_ALGO_AUTO) algo = RL_ALGO_FP32;
+    RL_REQUIRE(algo == RL_ALGO_FP32, RL_EINVAL, "unknown algo %d", p->algo);
+    RL_REQUIRE(empty || p->e_dtype == 0 ||
+                   (p->d % 8 == 0 && p->ld % 8 == 0 && (reinterpret_cast<uintptr_t>(p->E) & 15) == 0),
+               RL_EUNSUPPORTED, "float16 storage needs d %% 8 == 0, ld %% 8 == 0 and 16-byte aligned E");
+  } else {
+    const bool tc_ok = wgmma_scan_supported(p);
+    if (algo == RL_ALGO_AUTO) algo = tc_ok ? RL_ALGO_TCGEN05 : RL_ALGO_FP32;
+    RL_REQUIRE(algo == RL_ALGO_FP32 || algo == RL_ALGO_TCGEN05, RL_EINVAL, "unknown algo %d", p->algo);
+    RL_REQUIRE(empty || p->e_dtype == 0 || algo == RL_ALGO_TCGEN05, RL_EUNSUPPORTED,
+               "float16 storage needs the tensor-core scan (d %% 8 == 0, ld %% 8 == 0, 16-byte aligned E)");
+    RL_REQUIRE(empty || algo != RL_ALGO_TCGEN05 || tc_ok, RL_EUNSUPPORTED,
+               "RL_ALGO_TCGEN05 needs d %% 4 == 0, ld %% 4 == 0, 16-byte aligned E and a supported metric");
+  }
   L->algo = algo;
 
   int S = p->sample_stride;
@@ -155,7 +165,7 @@ static int device_sm_count(int* out) {
 
 using namespace rl;
 
-extern "C" int rl_version(void) { return 103; }
+extern "C" int rl_version(void) { return 104; }
 extern "C" const char* rl_last_error(void) { return g_err; }
 
 extern "C" int rl_device_info(int* sm_count, int* cc_major, int* cc_minor, size_t* l2_bytes) {
@@ -195,6 +205,7 @@ extern "C" int rl_maxsim_topk(const rl_scan_params* p, float* hit_sim, int64_t* 
     return RL_OK;
   }
   RL_REQUIRE(p->E && p->inv_norm && p->sq_norm && p->row_chunk, RL_EINVAL, "rl_maxsim_topk: null index pointer");
+  RL_REQUIRE(p->metric != RL_METRIC_L1 || p->row_stats, RL_EINVAL, "rl_maxsim_topk: the l1 metric needs row_stats");
   RL_REQUIRE(workspace != nullptr && workspace_bytes >= L.total, RL_ENOSPACE,
              "rl_maxsim_topk: workspace %zu < required %zu", workspace_bytes, L.total);
   RL_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 255) == 0, RL_EINVAL, "workspace must be 256-byte aligned");
@@ -215,7 +226,8 @@ extern "C" int rl_maxsim_topk(const rl_scan_params* p, float* hit_sim, int64_t* 
   float* dump = reinterpret_cast<float*>(ws + L.off_dump);
   Cand* cand = reinterpret_cast<Cand*>(ws + L.off_cand);
   const bool reuse = (p->flags & RL_FLAG_REUSE_THRESHOLDS) != 0;
-  const bool count_unf = (p->flags & RL_FLAG_COUNT_UNFILTERED) != 0 && p->row_allowed != nullptr && L.algo == RL_ALGO_TCGEN05;
+  const bool count_unf = (p->flags & RL_FLAG_COUNT_UNFILTERED) != 0 && p->row_allowed != nullptr &&
+                         (L.algo == RL_ALGO_TCGEN05 || p->metric == RL_METRIC_L1);
   int launches = 0;
   cudaEvent_t* se = (p->flags & RL_FLAG_TIME_KERNELS) ? stage_events_for(workspace) : nullptr;
   auto mark = [&](int i) { if (se) cudaEventRecord(se[i], stream); };
@@ -249,6 +261,7 @@ extern "C" int rl_maxsim_topk(const rl_scan_params* p, float* hit_sim, int64_t* 
     a.n_mode_blocks = n_mode_blocks;
     ++launches;
     if (L.algo == RL_ALGO_TCGEN05) return launch_scan_wgmma(a, p, q_scale, qimg, sms, stream);
+    if (p->metric == RL_METRIC_L1) return launch_scan_l1(a, p->e_dtype == 1, stream);
     return launch_scan_fp32(a, stream);
   };
 
@@ -302,6 +315,7 @@ extern "C" int rl_maxsim_count_at_least(const rl_scan_params* p, const float* si
     return RL_OK;
   }
   RL_REQUIRE(p->E && p->inv_norm && p->sq_norm, RL_EINVAL, "rl_maxsim_count_at_least: null index pointer");
+  RL_REQUIRE(p->metric != RL_METRIC_L1 || p->row_stats, RL_EINVAL, "rl_maxsim_count_at_least: the l1 metric needs row_stats");
   RL_REQUIRE(workspace != nullptr && workspace_bytes >= L.total, RL_ENOSPACE,
              "rl_maxsim_count_at_least: workspace %zu < required %zu", workspace_bytes, L.total);
   RL_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 255) == 0, RL_EINVAL, "workspace must be 256-byte aligned");
@@ -340,7 +354,9 @@ extern "C" int rl_maxsim_count_at_least(const rl_scan_params* p, const float* si
   a.sel_count = 0x7fffffff;
   a.dump_mode = 0;
   a.n_mode_blocks = L.n_blocks;
-  rc = L.algo == RL_ALGO_TCGEN05 ? launch_scan_wgmma(a, p, q_scale, qimg, sms, stream) : launch_scan_fp32(a, stream);
+  rc = L.algo == RL_ALGO_TCGEN05     ? launch_scan_wgmma(a, p, q_scale, qimg, sms, stream)
+       : p->metric == RL_METRIC_L1 ? launch_scan_l1(a, p->e_dtype == 1, stream)
+                                   : launch_scan_fp32(a, stream);
   if (rc != RL_OK) return rc;
   RL_CUDA_CHECK(cudaMemcpyAsync(counts, cand_cnt, (size_t)p->B * 4, cudaMemcpyDeviceToDevice, stream));
   return RL_OK;

@@ -37,5 +37,7 @@ __device__ __forceinline__ void emit_candidate(const ScanArgs& a, int col, float
 }
 
 int launch_scan_fp32(const ScanArgs& a, cudaStream_t stream);
+// RL_METRIC_L1 (scan_l1.cu): float32 or float16 rows (e_f16), key = -sum |e - q|.
+int launch_scan_l1(const ScanArgs& a, bool e_f16, cudaStream_t stream);
 
 }  // namespace rl

@@ -186,16 +186,30 @@ __global__ void __launch_bounds__(128) query_prep_kernel(const float* __restrict
                                                          int algo, const float* __restrict__ row_stats,
                                                          double* __restrict__ q_sq, float* __restrict__ q_inv,
                                                          float* __restrict__ eps) {
-  __shared__ double red[4];
+  __shared__ double red[4], red1[4];
   const int b = blockIdx.x;
-  double s = 0.0;
+  double s = 0.0, s1 = 0.0;
   for (int c = threadIdx.x; c < d; c += blockDim.x) {
     const double v = Q[(size_t)b * d + c];
     s += v * v;
+    s1 += fabs(v);
   }
   s = warp_sum_d(s);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
+  s1 = warp_sum_d(s1);
+  if ((threadIdx.x & 31) == 0) { red[threadIdx.x >> 5] = s; red1[threadIdx.x >> 5] = s1; }
   __syncthreads();
+  if (threadIdx.x == 0 && metric == RL_METRIC_L1) {
+    // L1 scan: each key is -fl(sum_i |fl(e_i - q_i)|), summed sequentially in float32 (scan_l1.cu), so
+    // |key + sum |e - q|| <= gamma_d * sum |e - q| <= d u (1 + O(d u)) (sum |e| + sum |q|), u = 2^-24; the fp16 -> fp32
+    // row conversion is exact.  sum |e| <= min(sqrt(d) max |e|_2, d max |e_ij|) from row_stats.  The same
+    // (d + 8) 2^-23 factor as the fp32 scan leaves a factor 2 of slack.
+    const double sum_q = red1[0] + red1[1] + red1[2] + red1[3];
+    const double sum_e = fmin(sqrt((double)d) * (double)row_stats[0], (double)d * (double)row_stats[1]);
+    q_sq[b] = red[0] + red[1] + red[2] + red[3];
+    q_inv[b] = 0.f;
+    eps[b] = (float)((double)(d + 8) * 1.1920928955078125e-7 * (sum_q + sum_e));
+    return;
+  }
   if (threadIdx.x == 0) {
     const double nq = red[0] + red[1] + red[2] + red[3];
     q_sq[b] = nq;
@@ -394,8 +408,9 @@ __global__ void __launch_bounds__(kSelThreads) select_kernel(const SelectArgs a)
 
 // ---- finalize --------------------------------------------------------------------------------------
 // d2 = sum (e - q)^2, accumulated directly: ne + nq - 2 dot cancels to its rounding error for a row that (nearly)
-// duplicates a query of large norm.
+// duplicates a query of large norm.  For l1 the last argument is d1 = sum |e - q| instead.
 __device__ __forceinline__ float exact_sim(int metric, double dot, double ne, double nq, double d2) {
+  if (metric == RL_METRIC_L1) return 1.0f - (float)d2;   // the FLOAT the SQL returns, then sim = 1 - dist
   if (metric == RL_METRIC_COSINE) {
     double s = dot / sqrt(ne * nq);
     s = fmin(1.0, fmax(-1.0, s));
@@ -477,6 +492,7 @@ __global__ void __launch_bounds__(kSelThreads) finalize_kernel(const FinalizeArg
   const int cnt = f.cand_cnt[b];
   const int n = min(cnt, f.cap);
   int st = cnt > f.cap ? RL_STATUS_CAND_OVERFLOW : 0;
+  if (f.metric == RL_METRIC_L1 && !isfinite(f.q_sq[b])) st |= RL_STATUS_QUERY_NONFINITE;   // (q_sq is finite for finite q)
   const Cand* cand = f.cand + (size_t)b * f.cap;
 
   __shared__ int s_coll;
@@ -547,9 +563,35 @@ __global__ void __launch_bounds__(kSelThreads) finalize_kernel(const FinalizeArg
   // l2 needs only d2 = sum (e - q)^2, cosine and dot only dot and ne: one loop each, chosen once per row (the metric
   // is uniform per launch), so the cosine / dot loop is the one it always was.
   const bool l2 = f.metric == RL_METRIC_L2;
+  const bool l1 = f.metric == RL_METRIC_L1;
   auto exact_row_sim = [&](int32_t row) -> float {   // all 32 lanes call it; every lane gets the result
     const float* e = f.E + (int64_t)row * f.ld;
     double dot = 0.0, ne = 0.0, d2 = 0.0;
+    if (l1) {   // d1 = sum |e - q| in float64, the loop layout of the l2 one
+      double d1 = 0.0;
+      if (f.e_f16) {
+        const __half* eh = reinterpret_cast<const __half*>(f.E) + (int64_t)row * f.ld;
+        for (int c = lane * 8; c < f.d; c += 256) {
+          const uint4 v = __ldg(reinterpret_cast<const uint4*>(eh + c));
+          const __half2* h = reinterpret_cast<const __half2*>(&v);
+#pragma unroll
+          for (int k2 = 0; k2 < 4; ++k2) {
+            const float2 ev = __half22float2(h[k2]);
+            d1 += fabs((double)ev.x - qv[c + 2 * k2]) + fabs((double)ev.y - qv[c + 2 * k2 + 1]);
+          }
+        }
+      } else if (vec) {
+        for (int c = lane * 4; c < f.d; c += 128) {
+          const float4 ev = __ldg(reinterpret_cast<const float4*>(e + c));
+          const float4 qq = *reinterpret_cast<const float4*>(qv + c);
+          d1 += fabs((double)ev.x - qq.x) + fabs((double)ev.y - qq.y) + fabs((double)ev.z - qq.z) + fabs((double)ev.w - qq.w);
+        }
+      } else {
+        for (int c = lane; c < f.d; c += 32) d1 += fabs((double)__ldg(e + c) - qv[c]);
+      }
+      d1 = warp_sum_d(d1);
+      return exact_sim(f.metric, dot, ne, nq, d1);
+    }
     if (l2) {
       if (f.e_f16) {
         const __half* eh = reinterpret_cast<const __half*>(f.E) + (int64_t)row * f.ld;
@@ -764,7 +806,7 @@ __global__ void __launch_bounds__(kSelThreads) merge_kernel(const MergeArgs m) {
 
 // ---- launchers ---------------------------------------------------------------------------------------
 // ---- similarity floor -> key threshold (rl_maxsim_count_at_least) ------------------------------------
-// The scan compares approximate keys: cosine -> the similarity itself, dot -> <e,q> = sim - 1,
+// The scan compares approximate keys: cosine -> the similarity itself, dot -> <e,q> = sim - 1, l1 -> -sum |e - q| = sim - 1,
 // l2 -> 2<e,q> - |e|^2 = |q|^2 - dist^2 with dist = 1 - sim.  `bound` moves the threshold by the key's
 // error bound so that the count brackets the exact one (+1: no exact match is missed, -1: none is extra).
 __global__ void sim_floor_to_thr_kernel(const float* __restrict__ sim_floor, const double* __restrict__ q_sq,
@@ -775,7 +817,7 @@ __global__ void sim_floor_to_thr_kernel(const float* __restrict__ sim_floor, con
   const float f = sim_floor[b];
   float key;
   if (metric == RL_METRIC_COSINE) key = f;
-  else if (metric == RL_METRIC_DOT) key = f - 1.f;
+  else if (metric == RL_METRIC_DOT || metric == RL_METRIC_L1) key = f - 1.f;   // l1: -sum |e - q| = sim - 1
   else {
     const double dist = 1.0 - (double)f;
     key = dist < 0.0 ? __builtin_huge_valf() : (float)(q_sq[b] - dist * dist);
