@@ -103,6 +103,89 @@ def keyword_search(ix: FTSIndex, query: str, *, num_results: int, allowed: Seque
     return docs[top].tolist(), scores[top].tolist()
 
 
+# ---- the device kernels' arithmetic over the postings CSR ------------------------------------------------------------
+# ``rl_bm25_topk_global`` restated on the arrays it reads (include/raglite_b200.h): term_off int64 [V + 1], doc / tf
+# int32 [P] sorted by chunk within each term, doc_len int32 [C], stats int64 [2 + J] = {N, sum of doc_len, df of each
+# entry}, q_off int32 [B + 1], q_terms int32 [J] (-1: an entry this index does not hold).
+def bm25_csr_scores(term_off, doc, tf, doc_len, stats, q_off, q_terms, k1, b, idf=None):
+    """Per query, a dense float64 score per chunk and the mask of chunks holding one of its entries' terms: ``(score
+    [B, C], matched bool [B, C])``.  Every step is the kernel's expression in its order (that of ``match_bm25_arrays``):
+    avgdl = sum / N; idf = log10(((N - df) + 0.5) / (df + 0.5) + 1); norm = (1 - b) + b * (len / avgdl); sub = idf *
+    ((f * (k1 + 1)) / (f + k1 * norm)); each chunk's sum runs in entry order.  ``idf`` (float64 [J]) replaces NumPy's
+    log10 per entry, so that a device's own log10 can be fed in."""
+    term_off, q_off, q_terms = np.asarray(term_off, np.int64), np.asarray(q_off, np.int64), np.asarray(q_terms, np.int64)
+    doc, tf, doc_len, stats = np.asarray(doc), np.asarray(tf), np.asarray(doc_len), np.asarray(stats, np.int64)
+    V, B, C = len(term_off) - 1, len(q_off) - 1, len(doc_len)
+    N = np.float64(stats[0])
+    with np.errstate(invalid="ignore", divide="ignore"):
+        avgdl = np.float64(stats[1]) / N
+        if idf is None:
+            df = stats[2:].astype(np.float64)
+            idf = np.log10(((N - df) + 0.5) / (df + 0.5) + 1.0)
+    idf = np.asarray(idf, np.float64)
+    scores = np.zeros((B, C), np.float64)
+    matched = np.zeros((B, C), bool)
+    for q in range(B):
+        for j in range(q_off[q], q_off[q + 1]):
+            t = q_terms[j]
+            if t < 0 or t >= V:
+                continue
+            p0, p1 = term_off[t], term_off[t + 1]
+            d = doc[p0:p1].astype(np.int64)
+            f = tf[p0:p1].astype(np.float64)
+            length = doc_len[d].astype(np.float64)
+            sub = idf[j] * ((f * (k1 + 1.0)) / (f + k1 * ((1.0 - b) + b * (length / avgdl))))
+            scores[q, d] += sub                  # a term holds a chunk at most once: no repeated index
+            matched[q, d] = True
+    return scores, matched
+
+
+def bm25_topk(scores, matched, mask, k, chunk_base=0):
+    """The exact top k of each query by (score desc, chunk asc) over the matched chunks that ``mask`` (bool [C] or None)
+    allows, laid out as ``rl_bm25_packed_bytes`` describes: ``(chunk int64 [B, k] (-1 padded, chunk_base added), score
+    float64 [B, k] (-inf padded), count int32 [B])``."""
+    B = len(scores)
+    ids = np.full((B, k), -1, np.int64)
+    out = np.full((B, k), -np.inf, np.float64)
+    count = np.zeros(B, np.int32)
+    for q in range(B):
+        keep = matched[q] if mask is None else matched[q] & np.asarray(mask, bool)
+        cand = np.flatnonzero(keep)
+        top = cand[np.lexsort((cand, -scores[q][cand]))[:k]]
+        n = len(top)
+        ids[q, :n], out[q, :n], count[q] = top + chunk_base, scores[q][top], n
+    return ids, out, count
+
+
+def csr_from_postings(postings, doc_len):
+    """The CSR of ``postings`` (per term, ``(chunks, tfs)``; chunks distinct) sorted by chunk within each term:
+    ``(term_off int64 [V + 1], doc int32 [P], tf int32 [P], doc_len int32 [C])``.  No text analysis: any tf, doc_len
+    and corpus size can be built directly."""
+    docs, tfs, counts = [], [], []
+    for chunks, tf in postings:
+        chunks = np.asarray(chunks, np.int64)
+        tf = np.broadcast_to(np.asarray(tf, np.int64), chunks.shape)
+        order = np.argsort(chunks, kind="stable")
+        assert len(np.unique(chunks)) == len(chunks), "a term holds a chunk at most once"
+        docs.append(chunks[order])
+        tfs.append(tf[order])
+        counts.append(len(chunks))
+    term_off = np.concatenate([[0], np.cumsum(counts, dtype=np.int64)]).astype(np.int64)
+    doc = np.concatenate([np.zeros(0, np.int64), *docs]).astype(np.int32)
+    tf = np.concatenate([np.zeros(0, np.int64), *tfs]).astype(np.int32)
+    doc_len = np.asarray(doc_len, np.int32)
+    assert doc.size == 0 or (doc.min() >= 0 and doc.max() < len(doc_len))
+    return term_off, doc, tf, doc_len
+
+
+def csr_from_fts(ix: FTSIndex):
+    """The postings CSR of an ``FTSIndex``'s terms table (term ids = the index's own termids)."""
+    pairs, tf = np.unique((ix.term_id << 32) | ix.term_doc, return_counts=True)
+    term = pairs >> 32
+    term_off = np.concatenate([[0], np.cumsum(np.bincount(term, minlength=len(ix.dict)))]).astype(np.int64)
+    return term_off, (pairs & 0xFFFFFFFF).astype(np.int32), tf.astype(np.int32), ix.doc_len.astype(np.int32)
+
+
 # ---- seeded corpora ---------------------------------------------------------------------------------------------------
 EVERYWHERE = "omnia"   # a word every non-empty synthetic body holds
 

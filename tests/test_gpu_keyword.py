@@ -31,7 +31,10 @@ def _index(bodies, *, seed=0, metadata=None, ids=None):
 
 def _check(got_ids, got_scores, count, want_ids, want_scores, all_scores, *, allowed=None):
     """Scores within REL of the oracle; ids identical wherever the oracle's neighbouring scores are more than REL apart
-    (and otherwise every returned chunk carries the oracle score it is listed with)."""
+    (and otherwise every returned chunk carries the oracle score it is listed with).  Exactly, whatever the ties: the ids
+    are distinct and in (score desc, chunk asc) order by the returned scores, and a full list (count = k) leaves out no
+    chunk whose oracle score is more than 2 REL above that of its last entry."""
+    k = len(got_ids)
     n = int(count)
     assert n == len(want_ids), (n, len(want_ids))
     got_ids, got_scores = [int(x) for x in got_ids[:n]], [float(x) for x in got_scores[:n]]
@@ -43,6 +46,16 @@ def _check(got_ids, got_scores, count, want_ids, want_scores, all_scores, *, all
     for d, s in zip(got_ids, got_scores, strict=True):
         assert d in all_scores and abs(all_scores[d] - s) <= REL * abs(s)
         assert allowed is None or allowed[d]
+    assert len(set(got_ids)) == n, "ids must be distinct"
+    for i in range(n - 1):
+        s0, s1 = got_scores[i], got_scores[i + 1]
+        assert s1 < s0 or (s1 == s0 and got_ids[i + 1] > got_ids[i]), ("order", i, got_ids[i: i + 2], s0, s1)
+    if n == k and n:
+        last = all_scores[got_ids[-1]]
+        kept = set(got_ids)
+        missed = [d for d, s in all_scores.items() if s > last * (1 + 2 * REL) and (allowed is None or allowed[d])
+                  and d not in kept]
+        assert not missed, ("left out above the cut", missed[:5])
 
 
 def _queries(seed, corpus_seed, vocab, n):

@@ -115,6 +115,44 @@ def test_oracle_hand_computed_example():
     assert ix3.num_docs == 2.0 and ix3.avgdl == 3.0 and match_bm25(ix3, "dog").keys() == {1}
 
 
+def test_csr_restatement_matches_the_fts_oracle_bit_for_bit():
+    """``bm25_csr_scores`` over the CSR of ``create_fts_index``'s tables (what the device kernels read) equals
+    ``match_bm25_arrays`` bit for bit, and ``bm25_topk`` equals ``keyword_search``, with and without a filter."""
+    import keyword_oracle as ko
+
+    bodies = make_bodies(3000, seed=5, vocab=600, empty=0.03, dup=0.05)
+    live = np.random.default_rng(5).random(len(bodies)) > 0.1
+    ix = create_fts_index(bodies, live=live)
+    term_off, doc, tf, doc_len = ko.csr_from_fts(ix)
+    allowed = np.arange(len(bodies)) % 3 != 1
+    queries = ko.make_queries(60, 6, corpus_seed=5, vocab=600) + [ko.EVERYWHERE, "qqqzzzx", bodies[7], bodies[8]]
+    compared = 0
+    for q in queries:
+        qids = sorted({ix.dict[t] for t in _fts.query_terms(q) if t in ix.dict})
+        stats = np.concatenate([[ix.num_docs, ix.doc_len.sum()], ix.df[qids]]).astype(np.int64)
+        scores, matched = ko.bm25_csr_scores(term_off, doc, tf, doc_len, stats, [0, len(qids)], qids, 1.2, 0.75)
+        docs, want = ko.match_bm25_arrays(ix, q)
+        assert np.array_equal(np.flatnonzero(matched[0]), docs)
+        assert np.array_equal(scores[0][docs].view(np.int64), want.view(np.int64))
+        assert (scores[0][~matched[0]] == 0).all()
+        for k, mask in ((1, None), (17, None), (4096, None), (50, allowed)):
+            ids, sc, cnt = ko.bm25_topk(scores, matched, mask, k)
+            w_ids, w_sc = keyword_search(ix, q, num_results=k, allowed=mask)
+            assert cnt[0] == len(w_ids) and ids[0, :cnt[0]].tolist() == w_ids
+            assert np.array_equal(sc[0, :cnt[0]].view(np.int64), np.asarray(w_sc, np.float64).view(np.int64))
+            assert (ids[0, cnt[0]:] == -1).all() and np.isneginf(sc[0, cnt[0]:]).all()
+        compared += len(docs)
+    assert compared > 10_000
+    # k1 = 0: every posting of a term scores its idf exactly, so the top k is the term's chunks in ascending order
+    stats = np.array([ix.num_docs, ix.doc_len.sum(), ix.df[0]], np.int64)
+    scores, matched = ko.bm25_csr_scores(term_off, doc, tf, doc_len, stats, [0, 1], [0], 0.0, 0.75)
+    ids, sc, cnt = ko.bm25_topk(scores, matched, None, 4096, chunk_base=1 << 40)
+    n = min(int(ix.df[0]), 4096)
+    assert cnt[0] == n and np.array_equal(ids[0, :n], (1 << 40) + doc[term_off[0]:term_off[1]][:n].astype(np.int64))
+    assert (sc[0, :n] == sc[0, 0]).all()
+    assert sc[0, 0] == pytest.approx(math.log10((ix.num_docs - ix.df[0] + 0.5) / (ix.df[0] + 0.5) + 1), rel=1e-15)
+
+
 def test_stats_abi_refusals_before_any_cuda_call():
     from raglite_b200 import _lib
 
