@@ -404,6 +404,25 @@ int rl_bm25_topk_global(const int64_t* term_off, const int32_t* doc, const int32
 int rl_bm25_merge_packed(const void* gathered, int R, int B, int k, int64_t* out_chunk, double* out_score,
                          int32_t* out_count, void* stream);
 
+/* ---- ts_rank keyword search: _search.py:176-201 (PostgreSQL, ts_rank over to_tsvector('simple', body)) -------------
+ * rl_tsrank_topk_global: the top k of B queries by PostgreSQL's ts_rank(tsvector, tsquery) at the default weights and
+ * normalization 0, every position of weight D.  Index: term_off int64 [n_terms + 1], a lexeme-major CSR whose doc int32
+ * [P] is sorted by chunk within each lexeme and npos int32 [P] is the number of positions the chunk's tsvector lists for
+ * it (1 for a lexeme without positions; values outside [1, 256] are clamped to it).  Query b = the entries q_off[b] ..
+ * q_off[b+1] (device int32): its distinct lexemes in ascending UTF-8 byte order, q_terms[j] the lexeme id of entry j or -1
+ * (a lexeme this index does not hold: it matches nothing but still counts in the divisor).  Per chunk, in entry order,
+ * res = (float)((double)res + c[npos]) with c[n] = (double)((0.1f + sum_{j<n} 0.1f / (float)((j+1)^2)) - 0.1f) /
+ * 1.64493406685 (float steps, ascending j), then score = res / (float)(number of entries): calc_rank_or, every step
+ * rounded to nearest in its C type, no contraction.  A chunk is a result when it holds an entry and chunk_mask allows it.
+ * Output as rl_bm25_topk_global: one rl_bm25_packed_bytes(B, k) buffer, best first by (score desc, chunk asc), the
+ * float32 score widened to double, chunk_base added, -1 / -inf padded, padding zeroed; 1 <= k <= 4096; workspace sized by
+ * rl_bm25_workspace_bytes (query groups, RL_ENOSPACE below one query); n_chunks == 0 valid.  The table c[1..256] is
+ * computed on the device by the first call on each device, which waits for it once. */
+int rl_tsrank_topk_global(const int64_t* term_off, const int32_t* doc, const int32_t* npos, int64_t n_terms,
+                          int64_t n_chunks, const uint8_t* chunk_mask, const int32_t* q_off, const int32_t* q_terms, int B,
+                          int k, int64_t chunk_base, void* out_packed, void* workspace, size_t workspace_bytes,
+                          void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -99,6 +99,12 @@ class ShardedIndex:
                 f"the next shard's range starting at {nxt}; build the shards with spaced bases (ShardedIndex.shard_bases) "
                 "to let them follow inserts")
 
+    def add_tsvector_rows(self, rows: Any) -> int:
+        """``CorpusIndex.add_tsvector_rows`` for this rank's shard, not a collective: of the ``(chunk_id, text)`` rows it
+        keeps those of the chunks this shard holds and ignores the rest, so every rank can be handed the whole result
+        set of ``SELECT id, to_tsvector('simple', body)::text FROM chunk``.  Returns the number of rows kept."""
+        return self.local._add_tsvector_rows(rows, others_ok=True)
+
     def search_pipeline(self, Q: torch.Tensor, **kw: Any) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]:
         """``scan_gather_merge`` over the shards of the group; ``last_status`` keeps the gathered status words."""
         out = scan_gather_merge(self, Q, **kw)

@@ -192,6 +192,7 @@ class CorpusIndex:
         self._meta_inv_chunks = 0                      # chunks covered by _meta_inv
         self._filter_cache: dict[Any, tuple[torch.Tensor, int]] = {}      # filter -> (chunk_ok uint8 [C], matching live rows)
         self._keyword: Any | None = None               # BM25 postings of the chunk bodies (keyword_index), built on demand
+        self._tsrank: Any | None = None                # ts_rank postings of PostgreSQL tsvectors (add_tsvector_rows)
         self._pinned: dict[Any, torch.Tensor] = {}     # result staging buffers (pinned host memory) by (size, stream)
         self._slots: list[Any] = []                    # streams + pinned buffers of the asynchronous searches (search_async)
         self.last_params: ScanParams | None = None
@@ -472,6 +473,8 @@ class CorpusIndex:
             self.max_vecs = int(counts.max()) if len(counts) else 1
             if self._keyword is not None:
                 self._keyword.compact(keep)
+            if self._tsrank is not None:
+                self._tsrank.compact(keep)
             self._chunk_alive = np.ones(self.n_chunks, dtype=bool)
             self._chunk_pos, self._alive = None, None
             for name in self._ROW_ARRAYS:
@@ -573,6 +576,8 @@ class CorpusIndex:
         self._span_tables = None
         if self._keyword is not None:
             self._keyword.stale = True
+        if self._tsrank is not None:
+            self._tsrank.stale = True
 
     def keyword_index(self) -> Any:
         """The BM25 index over ``chunks[i].body`` (``_keyword.KeywordIndex``), brought up to date with the table:
@@ -591,6 +596,48 @@ class CorpusIndex:
             if kw.stale:
                 kw.refresh(self._chunk_alive)
             return kw
+
+    def add_tsvector_rows(self, rows: Any) -> int:
+        """Index the tsvectors PostgreSQL computes for a ``postgresql`` keyword search (``ts_rank``, ``_search.py:176-201``):
+        ``(chunk_id, text)`` rows of ``SELECT id, to_tsvector('simple', body)::text FROM chunk``, in any order.  Call it
+        once after building the index and again after each ``append`` for the new chunks.  A chunk id the index does not
+        hold, a chunk given a second time, or a tsvector that ``to_tsvector`` does not print (weights, more than 256
+        positions per lexeme, malformed text) raises ``ValueError`` and leaves the index unchanged.  Returns the number
+        of rows indexed."""
+        return self._add_tsvector_rows(rows, others_ok=False)
+
+    def _add_tsvector_rows(self, rows: Any, *, others_ok: bool) -> int:
+        """``add_tsvector_rows``; ``others_ok``: skip the rows of chunk ids this index does not hold (a shard's share)."""
+        import time
+
+        from . import _pgfts
+        from ._keyword import TsRankIndex
+
+        if self.chunk_ids is None:
+            raise ValueError("the index holds no chunk ids: tsvector rows cannot be matched to chunks")
+        t0 = time.perf_counter()
+        with self._lock:
+            pos = self._positions()
+            have = self._tsrank.has_tsvector if self._tsrank is not None else np.zeros(0, dtype=bool)
+            chunks: list[int] = []
+            parsed = []
+            seen: set[int] = set()
+            for cid, text in rows:
+                p = pos.get(cid)
+                if p is None:
+                    if others_ok:
+                        continue
+                    raise ValueError(f"chunk_id {cid!r} is not in the index")
+                if p in seen or (p < len(have) and have[p]):
+                    raise ValueError(f"chunk_id {cid!r} already has a tsvector (a chunk's body never changes)")
+                seen.add(p)
+                chunks.append(p)
+                parsed.append(_pgfts.parse_tsvector(text, cid))
+            with torch.cuda.device(self.device):
+                if self._tsrank is None:
+                    self._tsrank = TsRankIndex(self.device)
+                self._tsrank.add(np.asarray(chunks, dtype=np.int64), parsed, time.perf_counter() - t0)
+        return len(chunks)
 
     def span_tables(self) -> dict[str, torch.Tensor]:
         """Device tables ``rl_span_collate`` needs (built once per index change from the ``Chunk`` records):

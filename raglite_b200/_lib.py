@@ -28,7 +28,7 @@ EXPORTS = [
     "rl_segment_mean_pool", "rl_xenc_linear_image_bytes", "rl_xenc_pack_linear", "rl_xenc_linear",
     "rl_xenc_workspace_bytes", "rl_xenc_score", "rl_xenc_attention", "rl_xenc_encode", "rl_xenc_encode_attention",
     "rl_xenc_embed_ln", "rl_xenc_add_ln", "rl_xenc_cls_head", "rl_bm25_stats", "rl_bm25_workspace_bytes",
-    "rl_bm25_packed_bytes", "rl_bm25_topk_global", "rl_bm25_merge_packed",
+    "rl_bm25_packed_bytes", "rl_bm25_topk_global", "rl_bm25_merge_packed", "rl_tsrank_topk_global",
 ]
 
 
@@ -122,6 +122,7 @@ def _declare(lib: C.CDLL) -> None:
     lib.rl_bm25_topk_global.argtypes = [vp, vp, vp, vp, vp, i64, i64, vp, vp, vp, i32, i32, C.c_double, C.c_double, i64, vp,
                                         vp, C.c_size_t, vp]
     lib.rl_bm25_merge_packed.argtypes = [vp, i32, i32, i32, vp, vp, vp, vp]
+    lib.rl_tsrank_topk_global.argtypes = [vp, vp, vp, i64, i64, vp, vp, vp, i32, i32, i64, vp, vp, C.c_size_t, vp]
     for name in EXPORTS:
         if name not in ("rl_last_error", "rl_maxsim_workspace_bytes", "rl_xenc_linear_image_bytes", "rl_xenc_workspace_bytes",
                         "rl_hits_packed_bytes", "rl_bm25_workspace_bytes", "rl_bm25_packed_bytes"):

@@ -259,7 +259,7 @@ def rerank_chunks(
     return chunks
 
 
-# ---- BM25 keyword search: the DuckDB branch of _search.py:156-230 ------------------------------------------------
+# ---- keyword search: BM25 (the DuckDB branch of _search.py:156-230) and ts_rank (its PostgreSQL branch) -----------
 def keyword_search_batch(
     queries: Sequence[str],
     *,
@@ -268,8 +268,14 @@ def keyword_search_batch(
     config: RAGLiteConfig | None = None,
     index: Any | None = None,
 ) -> tuple[np.ndarray, np.ndarray, np.ndarray]:
-    """Batched ``keyword_search``: BM25 as DuckDB's ``fts_main_chunk.match_bm25(id, query)`` computes it at its
-    defaults, over the ``Chunk`` bodies of the index (``CorpusIndex.keyword_index``; ``_fts`` has the text analysis).
+    """Batched ``keyword_search``.  With a DuckDB (or any non-PostgreSQL) ``db_url``: BM25 as DuckDB's
+    ``fts_main_chunk.match_bm25(id, query)`` computes it at its defaults, over the ``Chunk`` bodies of the index
+    (``CorpusIndex.keyword_index``; ``_fts`` has the text analysis).  With a ``postgresql`` ``db_url``: PostgreSQL's
+    ``ts_rank(to_tsvector('simple', body), to_tsquery('simple', q))`` over the tsvectors given to
+    ``CorpusIndex.add_tsvector_rows`` / ``ShardedIndex.add_tsvector_rows`` (``_pgfts`` has the query analysis); scores
+    are the float32 ``ts_rank`` widened to float64, ties by ascending chunk index (PostgreSQL leaves their order
+    unspecified).  It raises ``NotImplementedError`` when no index is registered or no shard has received tsvectors, and
+    for a query operand PostgreSQL would make a phrase; ``ValueError`` when a live chunk has no tsvector.
 
     Returns host arrays ``(chunk_index [B, k] int64 (-1 padded), score [B, k] float64 (-inf padded), count [B])``,
     ordered by descending score, ties by ascending chunk index.  The metadata filter only decides which chunks can be
@@ -282,13 +288,14 @@ def keyword_search_batch(
     (one all-reduce), each shard ranks its own chunks with those corpus-wide statistics, and the per-shard top k are
     merged after one all-gather; the returned chunk indices are GLOBAL (``chunk_base`` of the owning shard + local
     index), identical on every rank and for every shard layout of the same corpus (DESIGN.md section 3.7).  The
-    metadata filter is applied by each rank to its own chunks."""
+    metadata filter is applied by each rank to its own chunks.  ``ts_rank`` needs no statistics; its collectives are one
+    all-reduce of each shard's count of live chunks without a tsvector, then the all-gather and merge (section 3.9)."""
     from ._keyword import MAX_RESULTS
 
     config = config or RAGLiteConfig()
     if str(config.db_url).startswith("postgresql"):
-        raise NotImplementedError("keyword_search on PostgreSQL ranks with ts_rank over to_tsvector('simple', body), "
-                                  "a different formula; only the DuckDB branch (match_bm25) is implemented")
+        return _ts_rank_search_batch(queries, num_results=num_results, metadata_filter=metadata_filter, config=config,
+                                     index=index)
     index = index if index is not None else get_index(config)
     if index is None:
         raise ValueError(f"No index registered for db_url={config.db_url!r}; use raglite_b200.register_index")
@@ -308,6 +315,56 @@ def keyword_search_batch(
         return kw.topk_to_host(queries, k=k, chunk_mask=chunk_ok if chunk_ok is not None else kw.alive, index=index)
 
 
+_TS_RANK_NEEDS_TSVECTORS = ("keyword_search on PostgreSQL ranks with ts_rank over the database's own to_tsvector('simple', "
+                            "body); give the index those tsvectors with add_tsvector_rows(rows), rows = {select}")
+
+
+def _ts_rank_search_batch(
+    queries: Sequence[str], *, num_results: int, metadata_filter: MetadataFilter | None, config: RAGLiteConfig,
+    index: Any | None,
+) -> tuple[np.ndarray, np.ndarray, np.ndarray]:
+    """The PostgreSQL branch of ``keyword_search_batch`` (``_search.py:176-201``): ``ts_rank`` on the device over the
+    tsvectors given to ``add_tsvector_rows`` (``_keyword.TsRankIndex``).  Whether the search can run depends on every
+    shard (no tsvectors anywhere: ``NotImplementedError``; a live chunk without one: ``ValueError``), so on a
+    ``ShardedIndex`` both are decided after one all-reduce of each shard's count, and every rank raises alike."""
+    from . import _pgfts
+    from ._keyword import MAX_RESULTS, TsRankIndex, tsrank_plan
+
+    hint = _TS_RANK_NEEDS_TSVECTORS.format(select=_pgfts.TSVECTOR_SELECT)
+    index = index if index is not None else get_index(config)
+    if index is None:
+        raise NotImplementedError(f"No index registered for db_url={config.db_url!r}. {hint}")
+    sharded = hasattr(index, "group")
+    local: CorpusIndex = getattr(index, "local", index)
+    queries = list(queries)
+    k = int(num_results)
+    if k < 0 or k > MAX_RESULTS:
+        raise ValueError(f"num_results={k} is outside [0, {MAX_RESULTS}]")
+    B = len(queries)
+    empty = (np.full((B, k), -1, np.int64), np.full((B, k), -np.inf, np.float64), np.zeros(B, np.int32))
+    if B == 0 or k == 0:
+        return empty
+    with local._lock:
+        ts = local._tsrank
+        q_off, q_terms = tsrank_plan(queries, ts.lexeme_ids if ts is not None else {})
+        chunk_ok, _ = _filter_on_device(local, _adapt_metadata(metadata_filter))
+        state = [ts.missing(local._chunk_alive) if ts is not None else local.n_live_chunks, int(ts is None)]
+        if sharded:
+            state = index.sum_over_shards(torch.tensor(state, dtype=torch.int64, device=local.device)).tolist()
+        missing, without = state
+        if without == (index.world if sharded else 1):
+            raise NotImplementedError(f"The index has no tsvectors. {hint}")
+        if missing:
+            raise ValueError(f"{missing} live chunks have no tsvector: ts_rank cannot score them; pass their rows of "
+                             f"{_pgfts.TSVECTOR_SELECT} to add_tsvector_rows")
+        if local.n_live_chunks == 0 and not sharded:
+            return empty
+        if ts is None:   # a shard that never received tsvectors and holds no live chunk: it matches nothing
+            ts = TsRankIndex(local.device)
+        mask = chunk_ok if chunk_ok is not None else ts.alive_mask(local._chunk_alive)
+        return ts.topk_to_host(q_off, q_terms, k=k, n_chunks=local.n_chunks, chunk_mask=mask, index=index)
+
+
 def keyword_search(
     query: str,
     *,
@@ -315,9 +372,11 @@ def keyword_search(
     metadata_filter: MetadataFilter | None = None,
     config: RAGLiteConfig | None = None,
 ) -> tuple[list[ChunkId], list[float]]:
-    """Search chunks with BM25 keyword search -- drop-in for ``raglite.keyword_search`` (``_search.py:156-230``, the
-    DuckDB branch): the chunks that contain at least one query term, best ``num_results`` first.  On a registered
-    ``ShardedIndex`` a collective (see ``keyword_search_batch``) that returns the ids of chunks owned by every rank."""
+    """Search chunks with keyword search -- drop-in for ``raglite.keyword_search`` (``_search.py:156-230``): the chunks
+    that contain at least one query term, best ``num_results`` first, ranked by BM25 (DuckDB ``db_url``) or by
+    ``ts_rank`` (``postgresql`` ``db_url``; the score as pg8000 hands a ``float4`` over, its shortest round-trip digits:
+    see ``keyword_search_batch``).  On a registered ``ShardedIndex`` a collective (see ``keyword_search_batch``) that
+    returns the ids of chunks owned by every rank."""
     config = config or RAGLiteConfig()
     if config.self_query and isinstance(query, str):
         raise NotImplementedError("self_query needs an LLM and is outside the accelerated hot path")
@@ -326,7 +385,11 @@ def keyword_search(
                                                config=config, index=index)
     n = int(counts[0])
     base = 0 if hasattr(index, "group") else index.chunk_base   # a ShardedIndex returns global indices
-    return ([index.chunk_id_of(base + int(c)) for c in ids[0, :n]], [float(s) for s in scores[0, :n]])
+    if str(config.db_url).startswith("postgresql"):   # pg8000 reads a float4 as its shortest round-trip text
+        values = [float(str(np.float32(s))) for s in scores[0, :n]]
+    else:
+        values = [float(s) for s in scores[0, :n]]
+    return [index.chunk_id_of(base + int(c)) for c in ids[0, :n]], values
 
 
 # ---- the steps right after the hot path (SURVEY.md section 8f-3) ------------------------------------------
@@ -359,7 +422,9 @@ _KEYWORD_SEARCH: dict[str, Any] = {}
 def register_keyword_search(config_or_url: Any, fn: Any) -> None:
     """Replace the keyword search ``hybrid_search`` uses for a database (by default the device ``keyword_search``):
     any callable with ``keyword_search``'s signature ``(query, *, num_results, metadata_filter, config) ->
-    (chunk_ids, scores)`` -- e.g. one that queries PostgreSQL, whose ``ts_rank`` branch is not implemented here."""
+    (chunk_ids, scores)`` -- e.g. one that queries the database itself.  Both of the reference's branches run on the
+    device without one: BM25 for DuckDB, ``ts_rank`` for PostgreSQL once the index holds the database's tsvectors
+    (``CorpusIndex.add_tsvector_rows``)."""
     _KEYWORD_SEARCH[str(getattr(config_or_url, "db_url", config_or_url))] = fn
 
 
@@ -419,8 +484,8 @@ def hybrid_search(  # noqa: PLR0913
     keyword_search_weight: float = 0.25, metadata_filter: MetadataFilter | None = None, config: RAGLiteConfig | None = None,
 ) -> tuple[list[ChunkId], list[float]]:
     """Drop-in ``hybrid_search`` (``_search.py:257-280``): vector search on the device index, keyword search -- the
-    callable registered with ``register_keyword_search`` if there is one, the device ``keyword_search`` otherwise --
-    and Reciprocal Rank Fusion of the two rankings on the device."""
+    callable registered with ``register_keyword_search`` if there is one, the device ``keyword_search`` otherwise (BM25
+    or, for a ``postgresql`` ``db_url``, ``ts_rank``) -- and Reciprocal Rank Fusion of the two rankings on the device."""
     config = config or RAGLiteConfig()
     ks = _KEYWORD_SEARCH.get(str(config.db_url), keyword_search)
     vs_ids, _ = vector_search(query, num_results=oversample * num_results, metadata_filter=metadata_filter, config=config)

@@ -20,9 +20,14 @@
 //                  chunk, so the k-th largest composite is the exact cut of (score desc, chunk asc) -- then the k
 //                  survivors are sorted in shared memory.
 // Nothing depends on launch order and no global atomics are used; the shared-memory histogram counts are integers.
+//
+// rl_tsrank_topk_global ranks the same way by PostgreSQL's ts_rank (calc_rank_or at the default weights, normalization 0)
+// over a lexeme-major CSR whose value is npos, the number of positions a chunk's tsvector lists for the lexeme: its own
+// score kernel (float32 accumulators, DESIGN.md section 3.9), then the select kernel above, unchanged.
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <mutex>
 
 #include "common.cuh"
 
@@ -139,6 +144,79 @@ __global__ void __launch_bounds__(kScoreThreads) bm25_score_kernel(
     const double s = acc[i];
     const bool ok = s > 0.0 && (mask == nullptr || mask[c0 + i]);
     out[i] = ok ? ((uint64_t)__double_as_longlong(s) | kSign) : 0ull;   // positive doubles order as their bits
+  }
+}
+
+// ---- rl_tsrank_topk_global: ts_rank of one (query, tile) --------------------------------------------------------------
+// tsrank.c's calc_rank_or with every position of weight D (w = 0.1f, so the maximum weight is at j = 0): an entry held
+// n times adds contrib[n - 1] = (double)t / 1.64493406685 with t = (0.1f + resj) - 0.1f / 1 and resj = sum over j < n of
+// 0.1f / (float)((j + 1)^2), float sums in ascending j -- the C expressions in their own types.  The 256 values (npos is
+// capped at MAXNUMPOS = 256) are built once per device by tsrank_table_kernel.
+constexpr int kTsMaxPos = 256;
+
+__device__ double g_tsrank_contrib[kTsMaxPos];
+
+__global__ void __launch_bounds__(kTsMaxPos) tsrank_table_kernel() {
+  __shared__ float term[kTsMaxPos], resj[kTsMaxPos];
+  const int j = threadIdx.x;
+  term[j] = __fdiv_rn(0.1f, (float)((j + 1) * (j + 1)));
+  __syncthreads();
+  if (j == 0) {   // a sequential float sum: its rounding depends on the order
+    float r = 0.0f;
+    for (int i = 0; i < kTsMaxPos; ++i) {
+      r = __fadd_rn(r, term[i]);
+      resj[i] = r;
+    }
+  }
+  __syncthreads();
+  const float t = __fsub_rn(__fadd_rn(0.1f, resj[j]), __fdiv_rn(0.1f, 1.0f));
+  g_tsrank_contrib[j] = __ddiv_rn((double)t, 1.64493406685);
+}
+
+// Per chunk res = (float)((double)res + contrib) over the query's entries in the given order (the plan's byte order, that
+// of SortAndUniqItems), then res / (float)size with size = every entry of the query, known to this index or not.  A
+// chunk matches when it holds an entry (every contribution is > 0, so exactly when res > 0).
+__global__ void __launch_bounds__(kScoreThreads) tsrank_score_kernel(
+    const int64_t* __restrict__ term_off, const int32_t* __restrict__ doc, const int32_t* __restrict__ npos,
+    int64_t n_terms, int64_t n_chunks, const uint8_t* __restrict__ mask, const int32_t* __restrict__ q_off,
+    const int32_t* __restrict__ q_terms, int q0, uint64_t* __restrict__ keys) {
+  __shared__ float acc[kTile];
+  __shared__ double contrib[kTsMaxPos];
+  __shared__ int64_t range[2];
+  const int q = q0 + (int)blockIdx.y;
+  const int64_t c0 = (int64_t)blockIdx.x * kTile;
+  const int n = (int)min((int64_t)kTile, n_chunks - c0);
+  for (int i = threadIdx.x; i < n; i += blockDim.x) acc[i] = 0.0f;
+  for (int i = threadIdx.x; i < kTsMaxPos; i += blockDim.x) contrib[i] = g_tsrank_contrib[i];
+  const int j0 = q_off[q], j1 = q_off[q + 1];
+  for (int j = j0; j < j1; ++j) {
+    const int t = q_terms[j];
+    if (t < 0 || (int64_t)t >= n_terms) continue;   // uniform over the CTA; still counted in size
+    __syncthreads();   // the previous entry's additions (and the zeroing, the table) are done; range[] is free
+    if (threadIdx.x < 2) {
+      int64_t lo = term_off[t], hi = term_off[t + 1];
+      const int64_t target = c0 + (threadIdx.x ? n : 0);
+      while (lo < hi) {
+        const int64_t mid = (lo + hi) >> 1;
+        if ((int64_t)doc[mid] < target) lo = mid + 1; else hi = mid;
+      }
+      range[threadIdx.x] = lo;
+    }
+    __syncthreads();
+    const int64_t p0 = range[0], p1 = range[1];
+    for (int64_t p = p0 + threadIdx.x; p < p1; p += blockDim.x) {
+      const int c = doc[p];
+      const int np = min(max(npos[p], 1), kTsMaxPos);
+      acc[c - c0] = __double2float_rn(__dadd_rn((double)acc[c - c0], contrib[np - 1]));
+    }
+  }
+  __syncthreads();
+  const float size = (float)(j1 - j0);
+  uint64_t* out = keys + (int64_t)blockIdx.y * n_chunks + c0;
+  for (int i = threadIdx.x; i < n; i += blockDim.x) {
+    const float s = acc[i];
+    const bool ok = s > 0.0f && (mask == nullptr || mask[c0 + i]);
+    out[i] = ok ? ((uint64_t)__double_as_longlong((double)__fdiv_rn(s, size)) | kSign) : 0ull;
   }
 }
 
@@ -415,6 +493,64 @@ __global__ void __launch_bounds__(kMergeThreads) bm25_merge_kernel(const unsigne
   if (tid == 0) out_count[q] = want;
 }
 
+// ---- the query-group loop shared by rl_bm25_topk_global and rl_tsrank_topk_global ---------------------------------------
+// Called once the arguments are checked and B > 0: the queries are scored in groups of as many as the workspace holds
+// (G * n_chunks keys), each group by score(q0, g, keys) and then the select kernel into the packed output.  prepare()
+// runs first when there is a chunk to score.
+template <typename Prepare, typename ScoreLaunch>
+int topk_by_groups(const char* who, int B, int k, int64_t n_chunks, int64_t chunk_base, void* out_packed, void* workspace,
+                   size_t workspace_bytes, cudaStream_t st, Prepare prepare, ScoreLaunch score) {
+  int group = std::min(B, 65535);
+  if (n_chunks > 0) {
+    const int64_t group64 = (int64_t)(workspace_bytes / ((size_t)n_chunks * sizeof(uint64_t)));
+    RL_REQUIRE(group64 >= 1, RL_ENOSPACE, "%s: workspace of %zu bytes holds no query (needs %zu)", who, workspace_bytes,
+               (size_t)n_chunks * sizeof(uint64_t));
+    group = (int)std::min<int64_t>(group64, group);
+    const int rc = prepare();
+    if (rc != RL_OK) return rc;
+  }
+  unsigned char* out = static_cast<unsigned char*>(out_packed);
+  const size_t bk = (size_t)B * k;
+  int64_t* out_chunk = reinterpret_cast<int64_t*>(out);
+  double* out_score = reinterpret_cast<double*>(out + bk * 8);
+  int32_t* out_count = reinterpret_cast<int32_t*>(out + bk * 16);
+  const size_t used = bk * 16 + (size_t)B * 4, total = ((used + 15) & ~(size_t)15);
+  if (total > used) RL_CUDA_CHECK(cudaMemsetAsync(out + used, 0, total - used, st));   // the padding travels too
+  const size_t sel_smem = (size_t)kBm25MaxK * (sizeof(uint64_t) + sizeof(int32_t)) + kSelBins * sizeof(uint32_t);
+  RL_CUDA_CHECK(cudaFuncSetAttribute(bm25_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sel_smem));
+  uint64_t* keys = static_cast<uint64_t*>(workspace);
+  for (int q0 = 0; q0 < B; q0 += group) {
+    const int g = min(group, B - q0);
+    if (n_chunks > 0) {
+      score(q0, g, keys);
+      RL_CUDA_CHECK(cudaGetLastError());
+    }
+    bm25_select_kernel<<<g, kSelectThreads, sel_smem, st>>>(keys, n_chunks, q0, k, chunk_base, out_chunk, out_score,
+                                                            out_count);
+    RL_CUDA_CHECK(cudaGetLastError());
+  }
+  return RL_OK;
+}
+
+// g_tsrank_contrib of the current device, built on the first call that needs it.  That call waits for the table kernel
+// (once per device and process), so every later call on any stream finds the table complete.
+int ensure_tsrank_table(cudaStream_t st) {
+  constexpr int kMaxDevices = 256;
+  static std::mutex mu;
+  static bool built[kMaxDevices] = {};
+  int dev = 0;
+  RL_CUDA_CHECK(cudaGetDevice(&dev));
+  RL_REQUIRE(dev >= 0 && dev < kMaxDevices, RL_EINVAL, "rl_tsrank_topk_global: device %d out of range", dev);
+  std::lock_guard<std::mutex> lock(mu);
+  if (!built[dev]) {
+    tsrank_table_kernel<<<1, kTsMaxPos, 0, st>>>();
+    RL_CUDA_CHECK(cudaGetLastError());
+    RL_CUDA_CHECK(cudaStreamSynchronize(st));
+    built[dev] = true;
+  }
+  return RL_OK;
+}
+
 }  // namespace
 }  // namespace rl
 
@@ -461,37 +597,36 @@ extern "C" int rl_bm25_topk_global(const int64_t* term_off, const int32_t* doc, 
              RL_EINVAL, "rl_bm25_topk_global: null pointer");
   RL_REQUIRE(((uintptr_t)out_packed & 15) == 0 && ((uintptr_t)workspace & 7) == 0, RL_EINVAL,
              "rl_bm25_topk_global: out_packed must be 16-byte and workspace 8-byte aligned");
-  int group = std::min(B, 65535);
-  if (n_chunks > 0) {
-    const int64_t group64 = (int64_t)(workspace_bytes / ((size_t)n_chunks * sizeof(uint64_t)));
-    RL_REQUIRE(group64 >= 1, RL_ENOSPACE, "rl_bm25_topk_global: workspace of %zu bytes holds no query (needs %zu)",
-               workspace_bytes, rl_bm25_workspace_bytes(n_chunks, 1));
-    group = (int)std::min<int64_t>(group64, group);
-  }
-  unsigned char* out = static_cast<unsigned char*>(out_packed);
-  const size_t bk = (size_t)B * k;
-  int64_t* out_chunk = reinterpret_cast<int64_t*>(out);
-  double* out_score = reinterpret_cast<double*>(out + bk * 8);
-  int32_t* out_count = reinterpret_cast<int32_t*>(out + bk * 16);
   cudaStream_t st = (cudaStream_t)stream;
-  const size_t used = bk * 16 + (size_t)B * 4, total = rl_bm25_packed_bytes(B, k);
-  if (total > used) RL_CUDA_CHECK(cudaMemsetAsync(out + used, 0, total - used, st));   // the padding travels too
-  const size_t sel_smem = (size_t)kBm25MaxK * (sizeof(uint64_t) + sizeof(int32_t)) + kSelBins * sizeof(uint32_t);
-  RL_CUDA_CHECK(cudaFuncSetAttribute(bm25_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sel_smem));
   const unsigned n_tiles = (unsigned)((n_chunks + kTile - 1) / kTile);
-  uint64_t* keys = static_cast<uint64_t*>(workspace);
-  for (int q0 = 0; q0 < B; q0 += group) {
-    const int g = min(group, B - q0);
-    if (n_chunks > 0) {
-      bm25_score_kernel<<<dim3(n_tiles, g), kScoreThreads, 0, st>>>(term_off, doc, tf, doc_len, stats, n_terms, n_chunks,
-                                                                    chunk_mask, q_off, q_terms, q0, k1, b, keys);
-      RL_CUDA_CHECK(cudaGetLastError());
-    }
-    bm25_select_kernel<<<g, kSelectThreads, sel_smem, st>>>(keys, n_chunks, q0, k, chunk_base, out_chunk, out_score,
-                                                            out_count);
-    RL_CUDA_CHECK(cudaGetLastError());
-  }
-  return RL_OK;
+  return topk_by_groups("rl_bm25_topk_global", B, k, n_chunks, chunk_base, out_packed, workspace, workspace_bytes, st,
+                        [] { return (int)RL_OK; }, [&](int q0, int g, uint64_t* keys) {
+                          bm25_score_kernel<<<dim3(n_tiles, g), kScoreThreads, 0, st>>>(
+                              term_off, doc, tf, doc_len, stats, n_terms, n_chunks, chunk_mask, q_off, q_terms, q0, k1, b,
+                              keys);
+                        });
+}
+
+extern "C" int rl_tsrank_topk_global(const int64_t* term_off, const int32_t* doc, const int32_t* npos, int64_t n_terms,
+                                     int64_t n_chunks, const uint8_t* chunk_mask, const int32_t* q_off,
+                                     const int32_t* q_terms, int B, int k, int64_t chunk_base, void* out_packed,
+                                     void* workspace, size_t workspace_bytes, void* stream) {
+  RL_REQUIRE(B >= 0 && n_terms >= 0 && n_chunks >= 0 && n_chunks <= INT32_MAX && chunk_base >= 0, RL_EINVAL,
+             "rl_tsrank_topk_global: bad sizes");
+  RL_REQUIRE(k >= 1 && k <= kBm25MaxK, RL_EINVAL, "rl_tsrank_topk_global: k=%d outside [1, %d]", k, kBm25MaxK);
+  if (B == 0) return RL_OK;
+  RL_REQUIRE(term_off && q_off && out_packed && (n_chunks == 0 || workspace) &&
+                 (n_terms == 0 || n_chunks == 0 || (doc && npos)),
+             RL_EINVAL, "rl_tsrank_topk_global: null pointer");
+  RL_REQUIRE(((uintptr_t)out_packed & 15) == 0 && ((uintptr_t)workspace & 7) == 0, RL_EINVAL,
+             "rl_tsrank_topk_global: out_packed must be 16-byte and workspace 8-byte aligned");
+  cudaStream_t st = (cudaStream_t)stream;
+  const unsigned n_tiles = (unsigned)((n_chunks + kTile - 1) / kTile);
+  return topk_by_groups("rl_tsrank_topk_global", B, k, n_chunks, chunk_base, out_packed, workspace, workspace_bytes, st,
+                        [&] { return ensure_tsrank_table(st); }, [&](int q0, int g, uint64_t* keys) {
+                          tsrank_score_kernel<<<dim3(n_tiles, g), kScoreThreads, 0, st>>>(
+                              term_off, doc, npos, n_terms, n_chunks, chunk_mask, q_off, q_terms, q0, keys);
+                        });
 }
 
 extern "C" int rl_bm25_merge_packed(const void* gathered, int R, int B, int k, int64_t* out_chunk, double* out_score,

@@ -11,7 +11,12 @@ At the default size the host stages dominate the run (generating 375 M words, an
 the port): about ten minutes on a 16-thread host; ``--chunks 250000`` takes about three.
 ``--shards 1`` adds the sharded path on one GPU: ``ShardedIndex(group=None)`` over the same index against the bare index
 (per-batch medians, alternating), and ``rl_bm25_merge_packed`` alone on synthetic full lists at R = 2, 8 and k = 64, 4096
-(B = 256)."""
+(B = 256).
+``--dialect postgresql`` measures the PostgreSQL branch instead (``ts_rank``, ``rl_tsrank_topk_global``): the same corpus
+and queries, each body's ``to_tsvector('simple', body)::text`` synthesised on the host (the ``simple`` configuration keeps
+every word, lower-cased, with its positions: the bodies here are lower-case words separated by spaces), the index built
+from that text with ``add_tsvector_rows``, then the batch end to end, the kernels, and the NumPy port of ``calc_rank_or``
+(tests/tsrank_oracle.py) on ``--oracle-queries`` queries, checked bit for bit."""
 import argparse, json, operator, subprocess, sys, time
 from pathlib import Path
 ROOT = Path(__file__).resolve().parents[1]
@@ -32,6 +37,8 @@ ap.add_argument("--seed", type=int, default=0)
 ap.add_argument("--shards", type=int, default=0,
                 help="1: also time the sharded path (ShardedIndex(group=None)) against the bare index, alternating, "
                      "and the merge alone at R = 2, 8 and k = 64, 4096")
+ap.add_argument("--dialect", choices=["duckdb", "postgresql"], default="duckdb",
+                help="postgresql: ts_rank over synthesised tsvectors instead of BM25")
 args = ap.parse_args()
 if args.shards not in (0, 1):
     sys.exit("--shards: only 1 (one GPU) is implemented; a multi-GPU run under torchrun is not")
@@ -64,6 +71,109 @@ for c0 in range(0, args.chunks, step):
 gen_s = time.perf_counter() - t0
 stage("corpus generated")
 queries = [" ".join(vocab[i] for i in rng.choice(len(vocab), size=int(rng.integers(3, 13)), p=p)) for _ in range(args.batch)]
+
+
+def card_name():
+    try:
+        return subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
+                              text=True, timeout=30, check=False).stdout.strip().splitlines()[0]
+    except Exception:  # noqa: BLE001
+        return torch.cuda.get_device_name()
+
+
+def postgresql_bench():
+    import tsrank_oracle as to
+    from raglite_b200 import _lib
+
+    t0 = time.perf_counter()
+    rows = []
+    for c, body in enumerate(bodies):
+        held: dict[str, list[int]] = {}
+        for i, w in enumerate(body.split(), 1):
+            held.setdefault(w, []).append(min(i, 16383))
+        rows.append((str(c), " ".join(f"'{w}':" + ",".join(map(str, ps[:256])) for w, ps in sorted(held.items()))))
+    tsv_s = time.perf_counter() - t0
+    stage("tsvector text synthesised")
+    E, off = make_corpus(args.chunks, 1, 16, seed=args.seed)
+    idx = rl.CorpusIndex(E, off, chunk_ids=[str(c) for c in range(args.chunks)])
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    idx.add_tsvector_rows(rows)
+    build_s = time.perf_counter() - t0
+    ts = idx._tsrank
+    stage("ts_rank index built")
+    cfg = rl.RAGLiteConfig(db_url="postgresql://bench/raglite")
+    for _ in range(2):
+        rl.keyword_search_batch(queries, num_results=args.k, config=cfg, index=idx)
+    wall = []
+    for _ in range(args.reps):
+        t0 = time.perf_counter()
+        ids_, scores_, counts_ = rl.keyword_search_batch(queries, num_results=args.k, config=cfg, index=idx)
+        wall.append(time.perf_counter() - t0)
+    stage("end-to-end timed")
+    from raglite_b200._keyword import tsrank_plan
+
+    B, C, k = len(queries), args.chunks, args.k
+    q_off, q_terms = tsrank_plan(queries, ts.lexeme_ids)
+    qd = torch.from_numpy(np.concatenate([q_off, q_terms])).cuda()
+    group = max(1, min(B, (1 << 30) // (8 * C)))
+    need = int(ts.lib.rl_bm25_workspace_bytes(C, group))
+    ws = torch.empty(need, dtype=torch.uint8, device="cuda")
+    packed = torch.empty(int(ts.lib.rl_bm25_packed_bytes(B, k)), dtype=torch.uint8, device="cuda")
+
+    def launch():
+        _lib.check(ts.lib.rl_tsrank_topk_global(ts.term_off.data_ptr(), ts.doc.data_ptr(), ts.npos.data_ptr(), ts.n_terms, C,
+                                                None, qd.data_ptr(), qd.data_ptr() + 4 * (B + 1), B, k, 0, packed.data_ptr(),
+                                                ws.data_ptr(), need, torch.cuda.current_stream().cuda_stream),
+                   "rl_tsrank_topk_global")
+
+    launch()
+    ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
+    ev[0].record()
+    for _ in range(args.reps):
+        launch()
+    ev[1].record()
+    torch.cuda.synchronize()
+    kernel_ms = ev[0].elapsed_time(ev[1]) / args.reps
+    per_kernel = {}
+    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+        launch()
+        torch.cuda.synchronize()
+    for e in prof.key_averages():
+        if "tsrank_score" in e.key or "bm25_select" in e.key:
+            name = "score" if "score" in e.key else "select"
+            per_kernel[name] = per_kernel.get(name, 0.0) + getattr(e, "device_time_total", getattr(e, "cuda_time_total", 0.0)) / 1e3
+    stage("kernels timed")
+    df = np.diff(ts.term_off.cpu().numpy())
+    postings = int(sum(int(df[t]) for t in q_terms if t >= 0))
+    alg_bytes = postings * 8 + B * C * 8 * 2   # postings (doc, npos) + dense keys written and read once
+    # the NumPy port on the host cores over the same CSR: calc_rank_or per query, then the (score desc, chunk asc) top k
+    nq = min(args.oracle_queries, B)
+    csr = (ts.term_off.cpu().numpy(), ts.doc.cpu().numpy(), ts.npos.cpu().numpy())
+    t0 = time.perf_counter()
+    scores, matched = to.tsrank_csr_scores(*csr, q_off[: nq + 1], q_terms[: q_off[nq]], C)
+    w_ids, w_sc, w_cnt = to.tsrank_topk(scores, matched, None, k)
+    port_s = time.perf_counter() - t0
+    ok = sum(int(np.array_equal(ids_[b], w_ids[b]) and np.array_equal(scores_[b].view(np.int64), w_sc[b].view(np.int64))
+                 and counts_[b] == w_cnt[b]) for b in range(nq))
+    print(json.dumps({
+        "metric": f"ts_rank keyword_search queries/sec ({B} queries x top-{k}, {C} chunks)", "card": card_name(),
+        "chunks": C, "tokens": int(lens.sum()), "lexemes": ts.n_terms, "postings": int(ts.doc.numel()),
+        "corpus_gen_s": gen_s, "tsvector_text_s": tsv_s, "build_from_tsvector_text_s": build_s,
+        "build_parse_s": ts.build_seconds["parse"], "build_device_postings_s": ts.build_seconds["postings"],
+        "queries_per_s": B / float(np.median(wall)), "batch_wall_ms_median": 1e3 * float(np.median(wall)),
+        "batch_wall_ms_min": 1e3 * float(np.min(wall)), "topk_kernel_ms": kernel_ms, "kernel_ms": per_kernel,
+        "query_groups": -(-B // group), "algorithmic_gb": alg_bytes / 1e9,
+        "algorithmic_tb_per_s": alg_bytes / (kernel_ms * 1e-3) / 1e12,
+        "share_of_hbm": alg_bytes / (kernel_ms * 1e-3) / 1e12 / HBM_TBPS,
+        "port_numpy_queries_per_s": nq / port_s, "port_queries": nq, "cpu_threads": torch.get_num_threads(),
+        "oracle_match_bitwise": f"{ok}/{nq}",
+    }))
+
+
+if args.dialect == "postgresql":
+    postgresql_bench()
+    sys.exit(0)
 
 E, off = make_corpus(args.chunks, 1, 16, seed=args.seed)
 chunks = [rl.Chunk(id=str(c), body=b) for c, b in enumerate(bodies)]
