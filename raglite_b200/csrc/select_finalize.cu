@@ -240,9 +240,12 @@ __device__ __forceinline__ int32_t sample_row_of(int64_t p, int S) {
 // value that takes part in the order statistic -- v itself (SQL semantics) or, for exact MaxSim, the
 // max over the run of sample rows one chunk owns, reported once at the head of the run (-inf
 // elsewhere).  A warp owns 32 consecutive sample rows (coalesced loads of keys and owners, kU segments
-// in flight); the run max is a segmented suffix max over the warp (shuffles).  Runs are cut at
-// 32-row segment boundaries: the continuation is not a head, so no chunk is ever counted twice and a
-// partial max only lowers the statistic (it must be a lower bound).
+// in flight); the run max is a segmented suffix max over the warp (shuffles).  A sampled row is a head
+// exactly when it is the first row of its chunk, whether or not the row before it was sampled: with
+// S > 1 a chunk that spans two sampled blocks would otherwise be counted once in each and lift the
+// statistic above the shard's sel_k-th chunk maximum.  Runs are cut at 32-row segment and sampled
+// block boundaries; a continuation is not a head, so a chunk is counted at most once and a partial
+// max only lowers the statistic (it must be a lower bound).
 template <class CB>
 __device__ void for_each_sample(const SelectArgs& a, const float* __restrict__ dump, int64_t n, CB cb) {
   constexpr int kU = 4;
@@ -261,9 +264,8 @@ __device__ void for_each_sample(const SelectArgs& a, const float* __restrict__ d
         const int64_t row = sample_row_of(p, a.S);
         if (row < a.n_rows) {
           c[u] = a.row_chunk[row];
-          // Owner of the row before lane 0: inside the 128-row block, or across blocks when every
-          // block is sampled (S == 1).  Otherwise lane 0 starts a run.
-          if (lane == 0 && row > 0 && ((p % kBlockRows) != 0 || a.S == 1)) cprev0[u] = a.row_chunk[row - 1];
+          // Owner of the row before lane 0 (sampled or not): lane 0 is a head only at its chunk's first row.
+          if (lane == 0 && row > 0) cprev0[u] = a.row_chunk[row - 1];
         }
       }
     }
@@ -309,7 +311,7 @@ __global__ void __launch_bounds__(kSelThreads) select_kernel(const SelectArgs a)
     const int64_t row = sample_row_of(p, a.S);
     if (row >= a.n_rows) return kNegInf;
     const int32_t c = a.row_chunk[row];
-    if (row > 0 && (r_in != 0 || a.S == 1) && a.row_chunk[row - 1] == c) return kNegInf;  // not the head of its run
+    if (row > 0 && a.row_chunk[row - 1] == c) return kNegInf;  // not the first row of its chunk
     float m = dump[p];
     for (int j = 1; (r_in + j < kBlockRows || a.S == 1) && p + j < n && row + j < a.n_rows && a.row_chunk[row + j] == c; ++j)
       m = fmaxf(m, dump[p + j]);
