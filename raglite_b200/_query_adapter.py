@@ -127,8 +127,8 @@ def update_query_adapter(  # noqa: PLR0913
     ``evals`` are ``(question_embedding, relevant_chunk_indices)`` pairs -- what the reference reads from
     its ``Eval`` table and ``embed_strings`` (``_query_adapter.py:151-160``).
 
-    ``solver="device"`` (default on a single-GPU index) solves every eval's bounded least squares exactly on the
-    device (the unique projection; it satisfies the margin constraints to 1e-16).  ``solver="scipy"`` calls
+    ``solver="device"`` (default on a single-GPU index) solves every eval's bounded least squares on the
+    device (the projection to ~1e-15 relative; with examples 1e-7 apart or closer, to ~1e-8).  ``solver="scipy"`` calls
     ``scipy.optimize.lsq_linear`` per eval as the reference does: identical to the device answer to ~1e-8 on small
     instances, but SciPy's trust-region iteration stops up to ~1e-3 short of the optimum on the larger rank-deficient
     ones (20 x 20 positives x negatives), so choose it only to reproduce the reference's iterate.

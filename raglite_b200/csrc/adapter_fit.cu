@@ -138,7 +138,9 @@ __global__ void __launch_bounds__(kFitThreads) adapter_targets_kernel(const floa
   auto gent = [&](int j) -> double { return wq[j / N] - c * wq[P + j % N]; };   // <d_j, q>
   double gmax = 0.0;
   for (int j = 0; j < m; ++j) gmax = fmax(gmax, fabs(gent(j)));
-  const double tol = 1e-13 * (gmax + 1.0);
+  // Relative to the instance, like the pivot and fresh-column tests: scaling q by 2^a and the examples by 2^b scales
+  // every gradient by 2^(a+b) and t by 2^a exactly.  gmax = 0 makes every gradient 0, and nothing is picked.
+  const double tol = 1e-13 * gmax;
   const int max_iter = 6 * m + 64;
   while (true) {
     // w = -(g + H mu) over the generators outside the passive set; pick the largest
