@@ -205,6 +205,17 @@ int rl_maxsim_copy_dump(const rl_scan_params* p, const void* workspace, float* d
  * (float32 [B], key units: |approximate key - exact key| <= eps[b] for every row) into dst (device memory). */
 int rl_maxsim_copy_eps(const rl_scan_params* p, const void* workspace, float* dst, void* stream);
 
+/* Debug/test hook: copy the candidate list of the last call into device memory: key float32 [B, cap] and
+ * row int32 [B, cap] (the first min(cand_cnt[b], cap) entries of query b are the emitted candidates, in no
+ * particular order), cand_cnt int32 [B] (the number emitted, > cap on overflow), the emission threshold the
+ * select kernel handed to the main scan (thr float32 [B]) and the reciprocal bin width of the online
+ * refinement's histogram (hist_inv_w float32 [B]).  cap is the candidate capacity of the call
+ * (rl_maxsim_stats).  Any output pointer may be NULL.  When more than RL_MAX_SURVIVORS rows of a query survive,
+ * finalize rescores them in place: that query's keys then hold the order-preserving bits of exact similarities
+ * (0 for rows outside the band), not the emitted keys. */
+int rl_maxsim_copy_candidates(const rl_scan_params* p, const void* workspace, float* key, int32_t* row, int32_t* cand_cnt,
+                              float* thr, float* hist_inv_w, void* stream);
+
 /* ---- Shard merge + GROUP BY chunk + top-k: _search.py:143-150 --------------------------------
  * hit_*[R,B,H] are the per-shard outputs of rl_maxsim_topk (all-gathered).  num_hits > 0: keep
  * the num_hits best vectors overall, group by chunk (max sim), order desc, limit k.  num_hits == 0:

@@ -818,6 +818,23 @@ class CorpusIndex:
             check(self.lib.rl_maxsim_copy_eps(C.byref(p), _ptr(self.last_ws), _ptr(out), _stream()), "rl_maxsim_copy_eps")
         return out
 
+    def debug_candidates(self) -> dict[str, torch.Tensor]:
+        """Candidate list of the last scan (test hook): ``key`` float32 and ``row`` int32 ``[B, cap]`` (the first
+        ``min(cand_cnt[b], cap)`` entries of row b are valid), ``cand_cnt`` int32 ``[B]``, the select kernel's emission
+        threshold ``thr`` and the refinement histogram's ``hist_inv_w`` (float32 ``[B]``)."""
+        p = self.last_params
+        B, cap = int(p.B), self.scan_stats()["cand_cap"]
+        dev = self.device
+        out = {"key": torch.empty((B, cap), dtype=torch.float32, device=dev),
+               "row": torch.empty((B, cap), dtype=torch.int32, device=dev),
+               "cand_cnt": torch.empty(B, dtype=torch.int32, device=dev),
+               "thr": torch.empty(B, dtype=torch.float32, device=dev),
+               "hist_inv_w": torch.empty(B, dtype=torch.float32, device=dev)}
+        with torch.cuda.device(dev):
+            check(self.lib.rl_maxsim_copy_candidates(C.byref(p), _ptr(self.last_ws), *(_ptr(out[n]) for n in out), _stream()),
+                  "rl_maxsim_copy_candidates")
+        return out
+
     def kernel_times_ms(self) -> dict[str, float]:
         """Stage times of the last scan made with ``flags=RL_FLAG_TIME_KERNELS`` (synchronises)."""
         ms = (C.c_float * 5)()

@@ -24,7 +24,7 @@ RL_MAX_SURVIVORS = 4096   # finalize window (include/raglite_b200.h)
 
 EXPORTS = [
     "rl_version", "rl_last_error", "rl_device_info", "rl_row_stats", "rl_row_stats_f16", "rl_chunk_row_map", "rl_adapter_apply",
-    "rl_maxsim_workspace_bytes", "rl_maxsim_topk", "rl_maxsim_count_at_least", "rl_maxsim_unfiltered_bound", "rl_maxsim_stats", "rl_maxsim_kernel_times", "rl_maxsim_release", "rl_maxsim_copy_dump", "rl_maxsim_copy_eps", "rl_topk_merge", "rl_topk_merge_packed", "rl_hits_packed_bytes", "rl_row_mask", "rl_rrf_fuse", "rl_span_collate", "rl_best_vectors", "rl_adapter_targets",
+    "rl_maxsim_workspace_bytes", "rl_maxsim_topk", "rl_maxsim_count_at_least", "rl_maxsim_unfiltered_bound", "rl_maxsim_stats", "rl_maxsim_kernel_times", "rl_maxsim_release", "rl_maxsim_copy_dump", "rl_maxsim_copy_eps", "rl_maxsim_copy_candidates", "rl_topk_merge", "rl_topk_merge_packed", "rl_hits_packed_bytes", "rl_row_mask", "rl_rrf_fuse", "rl_span_collate", "rl_best_vectors", "rl_adapter_targets",
     "rl_segment_mean_pool", "rl_xenc_linear_image_bytes", "rl_xenc_pack_linear", "rl_xenc_linear",
     "rl_xenc_workspace_bytes", "rl_xenc_score", "rl_xenc_attention", "rl_xenc_encode", "rl_xenc_encode_attention",
     "rl_xenc_embed_ln", "rl_xenc_add_ln", "rl_xenc_cls_head", "rl_bm25_stats", "rl_bm25_workspace_bytes",
@@ -92,6 +92,7 @@ def _declare(lib: C.CDLL) -> None:
     lib.rl_row_mask.argtypes = [vp, vp, vp, i64, vp, vp]
     lib.rl_maxsim_copy_dump.argtypes = [C.POINTER(ScanParams), vp, vp, C.POINTER(C.c_int64), vp]
     lib.rl_maxsim_copy_eps.argtypes = [C.POINTER(ScanParams), vp, vp, vp]
+    lib.rl_maxsim_copy_candidates.argtypes = [C.POINTER(ScanParams), vp, vp, vp, vp, vp, vp, vp]
     lib.rl_topk_merge.argtypes = [vp, vp, vp, i32, i32, i32, i32, i32, vp, vp, vp, vp]
     lib.rl_hits_packed_bytes.argtypes = [i32, i32, i32]
     lib.rl_hits_packed_bytes.restype = C.c_size_t

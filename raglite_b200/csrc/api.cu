@@ -457,6 +457,30 @@ extern "C" int rl_maxsim_copy_eps(const rl_scan_params* p, const void* workspace
   return RL_OK;
 }
 
+extern "C" int rl_maxsim_copy_candidates(const rl_scan_params* p, const void* workspace, float* key, int32_t* row,
+                                         int32_t* cand_cnt, float* thr, float* hist_inv_w, void* stream_) {
+  RL_REQUIRE(p && workspace, RL_EINVAL, "rl_maxsim_copy_candidates: null pointer");
+  Layout L;
+  int rc = make_layout(p, 132, &L);
+  if (rc != RL_OK) return rc;
+  if (p->B == 0) return RL_OK;
+  cudaStream_t stream = (cudaStream_t)stream_;
+  const unsigned char* ws = static_cast<const unsigned char*>(workspace);
+  const size_t n = (size_t)p->B * L.cap;
+  // Cand is {key, row}: one strided 2D copy per field
+  if (key)
+    RL_CUDA_CHECK(cudaMemcpy2DAsync(key, 4, ws + L.off_cand + offsetof(Cand, key), sizeof(Cand), 4, n,
+                                    cudaMemcpyDeviceToDevice, stream));
+  if (row)
+    RL_CUDA_CHECK(cudaMemcpy2DAsync(row, 4, ws + L.off_cand + offsetof(Cand, row), sizeof(Cand), 4, n,
+                                    cudaMemcpyDeviceToDevice, stream));
+  const size_t per_query = (size_t)p->B * 4;
+  if (cand_cnt) RL_CUDA_CHECK(cudaMemcpyAsync(cand_cnt, ws + L.off_cnt, per_query, cudaMemcpyDeviceToDevice, stream));
+  if (thr) RL_CUDA_CHECK(cudaMemcpyAsync(thr, ws + L.off_thr, per_query, cudaMemcpyDeviceToDevice, stream));
+  if (hist_inv_w) RL_CUDA_CHECK(cudaMemcpyAsync(hist_inv_w, ws + L.off_histw, per_query, cudaMemcpyDeviceToDevice, stream));
+  return RL_OK;
+}
+
 extern "C" int rl_topk_merge(const float* hit_sim, const int64_t* hit_chunk, const int32_t* hit_count, int R, int B,
                              int H, int num_hits, int k, float* out_sim, int64_t* out_chunk, int32_t* out_count,
                              void* stream) {

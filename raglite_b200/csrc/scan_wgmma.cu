@@ -595,7 +595,6 @@ __global__ void __launch_bounds__(kThreads, 1) scan_wgmma_kernel(const __grid_co
             const int h = e >> 1, col = c + (e & 1);
             const float key = key_of(acc[4 * c8 + e], h, (e & 1) ? sc.y : sc.x);
             if (key >= ((e & 1) ? th.y : th.x)) {   // rare: a few hits per tile
-              if (masked_alive[h]) atomicAdd(a.cnt_all + col, 1);   // (only with RL_FLAG_COUNT_UNFILTERED on a filtered scan)
               if (valid[h]) {
                 // Stage the hit in shared memory (one returning atomic for the slot; the histogram update
                 // does not wait); per-query ranks and global slots are handed out in bulk at the flush.
@@ -610,6 +609,27 @@ __global__ void __launch_bounds__(kThreads, 1) scan_wgmma_kernel(const __grid_co
                   emit_candidate(a, col, key, (int32_t)row[h]);
                 }
               }
+            }
+          }
+        }
+        if (masked_alive[0] || masked_alive[1]) {
+          // Rows the filter masks out but that exist are counted against the threshold with their own key (the loop
+          // above keys them without the row's -|e|^2 or 1/|e|); only RL_FLAG_COUNT_UNFILTERED on a filtered scan gets here.
+          float mbias[2], mscale[2];
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            mbias[h] = (METRIC == RL_METRIC_L2 && masked_alive[h]) ? -a.sq_norm[row[h]] : 0.f;
+            mscale[h] = (METRIC == RL_METRIC_COSINE && cos_noscale && masked_alive[h]) ? __ldg(a.inv_norm + row[h]) : 1.f;
+          }
+#pragma unroll
+          for (int c8 = 0; c8 < NQ / 8; ++c8) {
+            if (8 * c8 >= nq) break;
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+              const int h = e >> 1, col = 8 * c8 + c_lane + (e & 1);
+              const float accv = acc[4 * c8 + e];
+              const float key = METRIC != RL_METRIC_COSINE ? fmaf(accv, s.cs[col], mbias[h]) : accv * mscale[h];
+              if (masked_alive[h] && key >= s.thr[col]) atomicAdd(a.cnt_all + col, 1);
             }
           }
         }
@@ -673,8 +693,14 @@ __global__ void __launch_bounds__(kThreads, 1) scan_wgmma_kernel(const __grid_co
               if (best < 0 && cum >= a.sel_count) best = bb;
             }
             if (best >= 1 && s.inv_w[col] > 0.f) {
-              // edge = thr0 + best * w; new emission threshold = edge - 2 eps
-              const float nt = s.thr0[col] + (float)best / s.inv_w[col] - 2.f * a.eps[col];
+              // edge = thr0 + best * w; new emission threshold = edge - 2 eps.  hist_bin rounds (key - thr0) * inv_w, so
+              // a key a few ulps under the rounded edge can still fall in bin `best`: any key it counts there is at
+              // least thr0 + g (1 - 2u) with g = best / inv_w, u = 2^-24, and the rounded edge exceeds thr0 + g by at most
+              // u (g + |edge|).  Lowering the edge by 8u (g + |edge|) covers both and this subtraction's own rounding.
+              const float g = (float)best / s.inv_w[col];
+              const float e0 = s.thr0[col] + g;
+              const float edge = e0 - (g + fabsf(e0)) * 0x1p-21f;
+              const float nt = edge - 2.f * a.eps[col];
               if (nt > s.thr[col]) s.thr[col] = nt;
             }
           }
