@@ -434,6 +434,43 @@ int rl_tsrank_topk_global(const int64_t* term_off, const int32_t* doc, const int
                           int k, int64_t chunk_base, void* out_packed, void* workspace, size_t workspace_bytes,
                           void* stream);
 
+/* ---- sentence splitting (SaT boundary probabilities + the reference's sentence partition) ---------------------------
+ * logits[r, l] = hidden[r, :] . W[l, :] + bias[l] for rows r < rows (float32; W [n_labels, hidden_size] row-major,
+ * 1 <= n_labels <= 16).  Runs on the output of rl_xenc_encode, one call at a time. */
+int rl_sat_token_logits(const float* hidden, int64_t rows, int hidden_size, const float* W, const float* bias,
+                        int n_labels, float* logits, void* stream);
+size_t rl_sat_workspace_bytes(int64_t n_tokens, int n_docs, int n_labels);
+/* One float32 probability per character of n_docs documents (probas [n_chars], document d at
+ * doc_char_off[d] .. doc_char_off[d + 1]; its tokens at doc_tok_off[d] .. doc_tok_off[d + 1]; both [n_docs + 1],
+ * ascending from 0).  Document d's blocks are blk_off[d] .. blk_off[d + 1]: each holds doc_block[d] = B tokens from
+ * document-relative token blk_start[b] (ascending), whose in-block position k is logits row blk_row[b] + k.
+ *  1. stitched[t, l] = sum_b hat[B (B - 1) / 2 + k] logits[blk_row[b] + k, l] / sum_b hat[..] over the blocks b that
+ *     cover token t, ascending b (k = t - blk_start[b]; float32, one rounding per operation);
+ *  2. every character of document d = min over its stitched logits (all tokens, all labels; -inf when it has none);
+ *  3. probas[tok_char[t]] = stitched[t, 0] for every token with tok_char[t] >= 0 (global character index, at most one
+ *     token per character);
+ *  4. probas = 1 / (1 + exp(-probas)); then, when known is not null, probas[c] = known[c] wherever known[c] is not NaN;
+ *  5. when is_space is not null: for each run of is_space characters inside a document, from the non-space character i
+ *     before it to the first non-space j after it, probas[i .. j-2] = min(probas[i .. j-1]), probas[j-1] = max(..).
+ * No atomics: results do not depend on the grouping of documents.  workspace >= rl_sat_workspace_bytes(n_tokens,
+ * n_docs, n_labels). */
+int rl_sat_char_probas(const float* logits, int n_labels, const int64_t* doc_tok_off, const int64_t* doc_char_off,
+                       const int32_t* doc_block, int n_docs, int64_t n_tokens, int64_t n_chars, const int64_t* blk_off,
+                       const int32_t* blk_start, const int64_t* blk_row, const float* hat, const int64_t* tok_char,
+                       const float* known, const uint8_t* is_space, float* probas, void* workspace,
+                       size_t workspace_bytes, void* stream);
+size_t rl_sentence_partition_workspace_bytes(int64_t n_chars);
+/* raglite's split_sentences partition per document d (probas[doc_off[d] .. + doc_len[d]], disjoint ranges inside
+ * [0, n_chars)): the dynamic program with no maximum length over the whole document, then, when max_len[d] > 0, the
+ * deque program with max_len[d] over every resulting sentence longer than max_len[d].  score = p - 0.25f in float32,
+ * dp in float64 (one rounded addition per step, strict comparisons).  Writes the partition indices (a sentence ends
+ * before each) ascending to cuts[doc_off[d] ..], their number to counts[d], and status[d] = 0, or 1 when no split
+ * satisfies the constraints (the reference's ValueError).  One thread per document; workspace >=
+ * rl_sentence_partition_workspace_bytes(n_chars) (dp, back, the deque's index ring and the stage-1 boundaries). */
+int rl_sentence_partition(const float* probas, const int64_t* doc_off, const int32_t* doc_len, const int32_t* min_len,
+                          const int32_t* max_len, int n_docs, int64_t n_chars, int32_t* cuts, int32_t* counts,
+                          int32_t* status, void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -4,7 +4,8 @@ Drop-in surface (reference ``raglite/__init__.py`` names for this path): ``RAGLi
 ``vector_search``, ``keyword_search``, ``hybrid_search``, ``rerank_chunks``, ``embed_strings``; plus the device-resident ``CorpusIndex`` /
 ``ShardedIndex`` that replace the database for this path and the batched ``vector_search_batch`` /
 ``keyword_search_batch``; and
-``TokenEmbedderEngine``, the embedding model's encoder on the GPU behind ``embed_strings`` / ``embed_queries``.
+``TokenEmbedderEngine``, the embedding model's encoder on the GPU behind ``embed_strings`` / ``embed_queries``; and
+``split_sentences`` with ``SaTEngine``, the sentence splitter's SaT model and partition on the GPU.
 """
 
 from ._config import RAGLiteConfig
@@ -29,6 +30,14 @@ from ._search import (
     vector_search_batch,
     vector_search_batch_async,
 )
+from ._sentences import (
+    SaTEngine,
+    markdown_sentence_boundaries,
+    register_sentence_splitter,
+    sentence_boundary_probas,
+    split_sentences,
+    split_sentences_batch,
+)
 from ._xenc import TokenEmbedderEngine
 
 __all__ = [
@@ -36,12 +45,15 @@ __all__ = [
     "ChunkSpan",
     "CorpusIndex",
     "RAGLiteConfig",
+    "SaTEngine",
     "TokenEmbedderEngine",
     "collate_spans_device",
     "hybrid_search",
     "keyword_search",
     "keyword_search_batch",
+    "markdown_sentence_boundaries",
     "register_keyword_search",
+    "register_sentence_splitter",
     "rrf_fuse_device",
     "embed_queries",
     "embed_strings",
@@ -55,6 +67,9 @@ __all__ = [
     "retrieve_chunks",
     "search_and_rerank_chunk_spans",
     "search_and_rerank_chunks",
+    "sentence_boundary_probas",
+    "split_sentences",
+    "split_sentences_batch",
     "unregister_index",
     "update_query_adapter",
     "vector_search",

@@ -29,6 +29,8 @@ EXPORTS = [
     "rl_xenc_workspace_bytes", "rl_xenc_score", "rl_xenc_attention", "rl_xenc_encode", "rl_xenc_encode_attention",
     "rl_xenc_embed_ln", "rl_xenc_add_ln", "rl_xenc_cls_head", "rl_bm25_stats", "rl_bm25_workspace_bytes",
     "rl_bm25_packed_bytes", "rl_bm25_topk_global", "rl_bm25_merge_packed", "rl_tsrank_topk_global",
+    "rl_sat_token_logits", "rl_sat_workspace_bytes", "rl_sat_char_probas", "rl_sentence_partition_workspace_bytes",
+    "rl_sentence_partition",
 ]
 
 
@@ -124,9 +126,18 @@ def _declare(lib: C.CDLL) -> None:
                                         vp, C.c_size_t, vp]
     lib.rl_bm25_merge_packed.argtypes = [vp, i32, i32, i32, vp, vp, vp, vp]
     lib.rl_tsrank_topk_global.argtypes = [vp, vp, vp, i64, i64, vp, vp, vp, i32, i32, i64, vp, vp, C.c_size_t, vp]
+    lib.rl_sat_token_logits.argtypes = [vp, i64, i32, vp, vp, i32, vp, vp]
+    lib.rl_sat_workspace_bytes.argtypes = [i64, i32, i32]
+    lib.rl_sat_workspace_bytes.restype = C.c_size_t
+    lib.rl_sat_char_probas.argtypes = [vp, i32, vp, vp, vp, i32, i64, i64, vp, vp, vp, vp, vp, vp, vp, vp, vp, C.c_size_t,
+                                       vp]
+    lib.rl_sentence_partition_workspace_bytes.argtypes = [i64]
+    lib.rl_sentence_partition_workspace_bytes.restype = C.c_size_t
+    lib.rl_sentence_partition.argtypes = [vp, vp, vp, vp, vp, i32, i64, vp, vp, vp, vp, C.c_size_t, vp]
     for name in EXPORTS:
         if name not in ("rl_last_error", "rl_maxsim_workspace_bytes", "rl_xenc_linear_image_bytes", "rl_xenc_workspace_bytes",
-                        "rl_hits_packed_bytes", "rl_bm25_workspace_bytes", "rl_bm25_packed_bytes"):
+                        "rl_hits_packed_bytes", "rl_bm25_workspace_bytes", "rl_bm25_packed_bytes",
+                        "rl_sat_workspace_bytes", "rl_sentence_partition_workspace_bytes"):
             getattr(lib, name).restype = C.c_int
 
 

@@ -11,7 +11,9 @@ installed), but two pieces of the hot path are pure NumPy/SciPy once their impor
   (token counting, segmenting, largest-remainder split, mean pool, normalise, fp16 cast);
 * ``raglite/_query_adapter.py`` -- ``_optimize_query_target``;
 * ``raglite/_typing.py`` -- the column processors of the ``chunk_embedding.embedding`` column
-  (DuckDB ``FLOAT[d]`` lists, PostgreSQL ``halfvec`` text, ``np.save`` blobs).
+  (DuckDB ``FLOAT[d]`` lists, PostgreSQL ``halfvec`` text, ``np.save`` blobs);
+* ``raglite/_split_sentences.py`` -- ``split_sentences`` and ``markdown_sentence_boundaries``, with wtpsplit-lite's
+  ``SaT`` replaced by a fake that returns seeded float32 probabilities.
 
 This script loads those two files *unmodified from where they lie* under a synthetic ``raglite``
 package whose heavy dependencies are replaced by stubs, and whose embedder is
@@ -227,6 +229,93 @@ def golden_rrf() -> None:
     print("rrf", len(cases), "cases")
 
 
+class _FakeSaT:
+    """wtpsplit-lite's ``SaT`` for the golden run: seeded float32 probabilities, one per character, a function of the
+    document alone (so the fixture can store them and a test can replay them)."""
+
+    def __init__(self, name: str) -> None:
+        self.name = name
+
+    @staticmethod
+    def probas(doc: str) -> np.ndarray:
+        import zlib
+
+        rng = np.random.default_rng(zlib.crc32(doc.encode()))
+        p = rng.beta(0.6, 2.0, size=len(doc))
+        ends = np.array([c in ".!?。\n" for c in doc], dtype=bool)
+        p[ends] = np.maximum(p[ends], rng.uniform(0.5, 1.0, size=int(ends.sum())))
+        return p.astype(np.float32)
+
+    def predict_proba(self, doc: str, **kw) -> np.ndarray:  # noqa: ANN003
+        assert kw == {"stride": 128, "block_size": 256, "weighting": "hat"}, kw
+        return self.probas(doc)
+
+
+def golden_split_sentences() -> None:
+    """``split_sentences`` (``_split_sentences.py:146-219``) and ``markdown_sentence_boundaries`` run unmodified on
+    Markdown headings, whitespace runs, multi-byte text, the length edges and several (min_len, max_len) pairs, with the
+    fake SaT's probabilities and with fully finite known probabilities; the infeasible case records its error."""
+    for name in ("raglite", "raglite._typing", "wtpsplit_lite"):
+        sys.modules.pop(name, None)
+    pkg = types.ModuleType("raglite")
+    pkg.__path__ = []
+    sys.modules["raglite"] = pkg
+    _stub("raglite._typing", FloatVector=np.ndarray)
+    _stub("wtpsplit_lite", SaT=_FakeSaT)
+    mod = _load("raglite._split_sentences", REF / "_split_sentences.py")
+    rng = np.random.default_rng(31)
+    words = "alpha beta gamma delta light clock rod frame event time of the observer velocity".split()
+
+    def prose(n: int) -> str:
+        out = []
+        while sum(len(w) + 1 for w in out) < n:
+            w = str(rng.choice(words))
+            out.append(w + ("." if rng.random() < 0.12 else ""))
+        return " ".join(out)
+
+    docs = {
+        "headings": "# Title\n\nSome text. More text here!\n\n## Section two\nBody of section. Another one.\n"
+                    "### Third level\n- item one\n- item two\n#### Four\nTail text without end",
+        "setext": "Heading one\n===========\n\nParagraph. Second sentence.\n\nHeading two\n-----------\nLast words here.",
+        "spaces": "Alpha beta.   Gamma\tdelta.\t\tEpsilon\n\nzeta eta.\u3000\u3000Theta iota.  \n\n  Kappa.  ",
+        "leading": "   \n  Leading whitespace. Then text.\t \t",
+        "multibyte": "Ünïcödé tëxt — ça va? 日本語の文です。次の文。 Emoji 😀 here.\u3000Done. Ω≈ç√∫ end.",
+        "len4": "abcd", "len5": "abcde", "len8": "abcdefgh", "len9": "ab cd. ef",
+        "prose": prose(600),
+        "long_run": "x" * 70 + " " + "y" * 150 + ". " + prose(200),
+    }
+    pairs = [(4, None), (4, 8), (4, 64), (4, 2048), (1, 8), (10, 2048), (3, 64)]
+    cases, arrays = [], {}
+
+    def run(name: str, doc: str, min_len: int, max_len: int | None, known: np.ndarray | None) -> None:
+        i = len(cases)
+        arrays[f"pred{i}"] = _FakeSaT.probas(doc)
+        arrays[f"md{i}"] = mod.markdown_sentence_boundaries(doc)
+        if known is not None:
+            arrays[f"known{i}"] = known
+        try:
+            kw = {} if known is None else {"boundary_probas": known}
+            out, err = mod.split_sentences(doc, min_len=min_len, max_len=max_len, **kw), None
+        except ValueError as e:
+            out, err = None, str(e)
+        cases.append({"name": name, "doc": doc, "min_len": min_len, "max_len": max_len, "known": known is not None,
+                      "sentences": out, "error": err})
+
+    for name, doc in docs.items():
+        for min_len, max_len in pairs:
+            run(name, doc, min_len, max_len, None)
+    for name in ("prose", "multibyte", "spaces", "long_run"):           # known probabilities override the model entirely
+        doc = docs[name]
+        for min_len, max_len in [(4, None), (4, 8), (4, 64), (1, 8)]:
+            run(name + "_known", doc, min_len, max_len, rng.beta(0.5, 1.5, size=len(doc)))
+    # no split can satisfy (5, 6) on 13 characters kept whole by stage 1 (every score is -0.25)
+    run("infeasible", "abcdefghijklm", 5, 6, np.zeros(13))
+    run("short13", "abcdefghijklm", 5, 6, None)
+    np.savez_compressed(GOLDEN / "split_sentences.npz", cases=np.frombuffer(json.dumps(cases).encode(), dtype=np.uint8),
+                        **arrays)
+    print("split_sentences", len(cases), "cases,", sum(c["error"] is not None for c in cases), "errors")
+
+
 if __name__ == "__main__":
     GOLDEN.mkdir(parents=True, exist_ok=True)
     golden_rrf()
@@ -234,3 +323,4 @@ if __name__ == "__main__":
     golden_pool(embed_mod)
     golden_adapter(qa_mod)
     golden_table_rows(load_reference_typing())
+    golden_split_sentences()
