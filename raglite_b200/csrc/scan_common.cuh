@@ -1,4 +1,4 @@
-// Arguments shared by the two scan kernels (fp32 CUDA-core and tensor-core wgmma) and their epilogues.
+// Arguments shared by the three scan kernels (fp32 CUDA-core, tensor-core wgmma and L1) and their epilogues.
 #pragma once
 #include "common.cuh"
 
