@@ -5,6 +5,9 @@
   ``XLMRobertaForTokenClassification`` run block by block in float64.  Every rule is written again here as a loop.
 * ``split_sentences_post``: the reference's post-processing (``_split_sentences.py:183-219`` and ``:56-143``) step by
   step: the override, the whitespace-run propagation, the two dynamic programs with NumPy float32 scores and float64 dp.
+* The device kernels of ``csrc/sentences.cu`` restated in their own float32 order, for bit-exact checks at the C-ABI:
+  ``fmaf`` and ``sat_head`` (``rl_sat_token_logits``), ``sat_char_logits`` and ``propagate_runs``
+  (``rl_sat_char_probas`` up to and after its sigmoid), ``partition_cuts`` (``rl_sentence_partition``).
 """
 
 from __future__ import annotations
@@ -187,6 +190,127 @@ def split_sentences_post(doc: str, predicted: np.ndarray, *, min_len: int = 4, m
     for s in sentences:
         out.extend([s] if len(s) <= max_len else _cut(s, _partition(p[pos:pos + len(s)], len(s), min_len, max_len)))
         pos += len(s)
+    return out
+
+
+def partition_cuts(p: np.ndarray, n: int, min_len: int, max_len: int | None) -> list[int]:
+    """The cut indices (sentence starts after the first) that ``rl_sentence_partition`` writes for one document of n
+    characters with final probabilities ``p``: stage 1 with no maximum, then stage 2 on every stage-1 sentence longer
+    than ``max_len`` (None or 0: none), as ``split_sentences_post`` runs them.  Raises the reference's ValueError."""
+    cuts = [b + 1 for b in _partition(p, n, min_len, None) or []]
+    if not max_len:
+        return cuts
+    out = []
+    for s, (a, e) in enumerate(zip([0, *cuts], [*cuts, n], strict=True)):
+        if e - a > max_len:
+            out += [a + b + 1 for b in _partition(p[a:e], e - a, min_len, max_len) or []]
+        if s < len(cuts):
+            out.append(e)
+    return out
+
+
+# ---- the device kernels, in their own float32 order --------------------------------------------------------------------
+def fmaf(a, b, c) -> np.ndarray:  # noqa: ANN001
+    """IEEE ``fmaf(a, b, c)`` of float32 arrays: a b + c rounded once.  The float64 product of two float32 values is
+    exact; TwoSum gives s + e = a b + c exactly; s rounded to float32 is the answer except when s lies exactly halfway
+    between two float32 values and e != 0, where the exact sum is on e's side of the midpoint."""
+    a, b, c = (np.asarray(x, np.float32).astype(np.float64) for x in (a, b, c))
+    p = a * b
+    s = p + c
+    bp = s - c
+    e = (p - bp) + (c - (s - bp))
+    r = s.astype(np.float32)
+    r64 = r.astype(np.float64)
+    with np.errstate(over="ignore", invalid="ignore"):
+        other = np.nextafter(r, np.where(r64 < s, np.float32(np.inf), np.float32(-np.inf)))
+        mid = (r64 != s) & ((r64 + other.astype(np.float64)) / 2 == s)
+    toward = mid & (e != 0) & ((e > 0) == (s > r64))
+    return np.where(toward, other, r).astype(np.float32)
+
+
+def sat_head(hidden: np.ndarray, W: np.ndarray, bias: np.ndarray) -> np.ndarray:
+    """``sat_head_kernel``: lane l of a row's warp runs ``acc = fmaf(h[k], w[k], acc)`` over k = l, l + 32, ...; the
+    butterfly adds lane l ^ o for o = 16 ... 1; lane 0 adds the bias.  float32 [rows, NL]."""
+    R, H = hidden.shape
+    out = np.empty((R, len(bias)), np.float32)
+    lanes = np.arange(32)
+    for lab in range(len(bias)):
+        acc = np.zeros((R, 32), np.float32)
+        for k0 in range(0, H, 32):
+            k = (k0 + lanes)[k0 + lanes < H]
+            acc[:, :len(k)] = fmaf(hidden[:, k], W[lab, k][None, :], acc[:, :len(k)])
+        for o in (16, 8, 4, 2, 1):
+            acc = acc + acc[:, lanes ^ o]
+        out[:, lab] = acc[:, 0] + bias[lab]
+    return out
+
+
+def sat_char_logits(logits: np.ndarray, doc_tok_off: np.ndarray, doc_char_off: np.ndarray, doc_block: np.ndarray,
+                    blk_off: np.ndarray, blk_start: np.ndarray, blk_row: np.ndarray, hat: np.ndarray,
+                    tok_char: np.ndarray) -> tuple[np.ndarray, np.ndarray]:
+    """``rl_sat_char_probas`` before its sigmoid: (the logit of every character, the stitched logits [T, NL]).
+
+    A token t of document d takes the blocks b of d with start <= t < start + B in ascending order, and sums
+    fl(w_k lg) and w_k in float32 (k = t - start, w_k = hat[B (B - 1) / 2 + k]), then divides once.  A document's
+    characters get the minimum stitched logit over its tokens and labels (-inf without tokens); each token with
+    ``tok_char >= 0`` then writes its label-0 logit there."""
+    NL, D = logits.shape[1], len(doc_block)
+    T, N = int(doc_tok_off[-1]), int(doc_char_off[-1])
+    tok_doc = np.repeat(np.arange(D), np.diff(doc_tok_off))
+    t = np.arange(T, dtype=np.int64) - doc_tok_off[tok_doc]
+    B = doc_block[tok_doc].astype(np.int64)
+    blk_doc = np.repeat(np.arange(D), np.diff(blk_off))
+    starts = blk_start.astype(np.int64)
+    key = (blk_doc.astype(np.int64) << 32) + starts + 1024            # ascending: documents in order, starts within
+    b = np.searchsorted(key, (tok_doc.astype(np.int64) << 32) + t - B + 1024, side="right")   # first start > t - B
+    end = blk_off[tok_doc + 1]
+    num, den = np.zeros((T, NL), np.float32), np.zeros(T, np.float32)
+    live = np.nonzero(b < end)[0]
+    live = live[starts[b[live]] <= t[live]]
+    while len(live):
+        bb = b[live]
+        k = t[live] - starts[bb]
+        wk = hat[B[live] * (B[live] - 1) // 2 + k]
+        num[live] = num[live] + wk[:, None] * logits[blk_row[bb] + k]
+        den[live] = den[live] + wk
+        b[live] += 1
+        live = live[b[live] < end[live]]
+        live = live[starts[b[live]] <= t[live]]
+    with np.errstate(divide="ignore", invalid="ignore"):
+        stitched = num / den[:, None]
+    dmin = np.full(D, -np.inf, np.float32)
+    has = np.diff(doc_tok_off) > 0
+    if has.any():
+        dmin[has] = np.minimum.reduceat(stitched.min(axis=1), doc_tok_off[:-1][has])
+    char_doc = np.searchsorted(doc_char_off, np.arange(N), side="right") - 1
+    out = dmin[char_doc]
+    hit = tok_char >= 0
+    out[tok_char[hit]] = stitched[hit, 0]
+    return out, stitched
+
+
+def propagate_runs(p: np.ndarray, is_space: np.ndarray, doc_char_off: np.ndarray) -> np.ndarray:
+    """``propagate`` over a batch at once, from the whitespace flags: for each run of spaces after a non-space character
+    i and before the first non-space j of the same document, p[i .. j-2] = min(p[i .. j-1]), p[j-1] = max(...)."""
+    N = len(p)
+    sp = np.asarray(is_space, dtype=bool)
+    out = p.copy()
+    i = np.nonzero(~sp[:-1] & sp[1:])[0]
+    ns = np.nonzero(~sp)[0]
+    at = np.searchsorted(ns, i + 1)
+    j = np.where(at < len(ns), ns[np.minimum(at, len(ns) - 1)], N)
+    doc_end = doc_char_off[np.searchsorted(doc_char_off, i, side="right")]
+    keep = j < doc_end
+    i, j = i[keep], j[keep]
+    if not len(i):
+        return out
+    ext = np.append(p, p.dtype.type(0))
+    idx = np.ravel(np.column_stack([i, j]))
+    mn, mx = np.minimum.reduceat(ext, idx)[::2], np.maximum.reduceat(ext, idx)[::2]
+    L = j - i - 1                                                       # p[i .. j-2] takes the minimum
+    pos = np.repeat(i, L) + (np.arange(L.sum()) - np.repeat(np.cumsum(L) - L, L))
+    out[pos] = np.repeat(mn, L)
+    out[j - 1] = mx
     return out
 
 
