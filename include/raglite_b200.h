@@ -471,6 +471,47 @@ int rl_sentence_partition(const float* probas, const int64_t* doc_off, const int
                           const int32_t* max_len, int n_docs, int64_t n_chars, int32_t* cuts, int32_t* counts,
                           int32_t* status, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- chunklets and chunks (the reference's split_chunklets dynamic program and split_chunks' partition) -------------
+ * Both partitions are one windowed dynamic program, one warp per document: dp[0] = 0 and, for i = 1 .. n,
+ * dp[i] = min over j of dp[j] + cost(j, i) (one rounded float64 addition) over the window j = i-1, i-2, ... while
+ * lens[j] + .. + lens[i-1] <= max_size[d]; the minimum of (dp[j] + cost, j) lexicographically (the smallest j of the
+ * smallest cost, inf included), dp[i] = inf and back[i] = -1 when the window is empty.  The cuts are read back from
+ * back[n] down to the first back <= 0 and written ascending to cuts[doc_off[d] ..] (the first item of each piece but the
+ * first), their number to counts[d].  Document d owns items doc_off[d] .. doc_off[d + 1] (doc_off [n_docs + 1], ascending
+ * from 0).  The workspace holds n + 1 entries per document of dp, back and the prefix sums. */
+size_t rl_chunklet_partition_workspace_bytes(int64_t n_sentences, int n_docs);
+/* split_chunklets with its default costs, per sentence: the Markdown boundary probability, the statement count (both
+ * float64, as markdown_chunklet_boundaries / compute_num_statements give them) and the length in characters.
+ * cost(j, i) = ((1 - p[j]) + (PB[i] - PB[j+1])) + (s - 3)(s - 3) / sqrt(max(s, 1e-6)) / 2, s = PS[i] - PS[j], every
+ * step one rounded float64 operation, PB / PS the sequential prefix sums from 0.  status[d] = 0, or 1 for a document
+ * without sentences (the reference refuses it).  A sentence longer than max_size[d] is kept as the reference keeps it:
+ * dp stays inf past it and later windows take their smallest j. */
+int rl_chunklet_partition(const double* boundary_probas, const double* num_statements, const int32_t* lens,
+                          const int64_t* doc_off, const int32_t* max_size, int n_docs, int64_t n_sentences,
+                          int32_t* cuts, int32_t* counts, int32_t* status, void* workspace, size_t workspace_bytes,
+                          void* stream);
+size_t rl_chunk_similarities_workspace_bytes(int64_t n_rows);
+/* split_chunks' cut costs, one CTA per document: rows doc_off[d] .. doc_off[d + 1] of X (x_dtype 0: float32,
+ * 1: float16; row stride ld elements, 1 <= dim <= 8192) are normalised in float32; the mean of the rows nonoutlying[]
+ * selects, normalised, is the discourse vector (float64, from the float32 normalised rows); when some row is selected
+ * and no row's projection x - (x . disc) disc has norm <= FLT_EPSILON (x . disc and the norm in float64), the
+ * normalised projections replace the rows (float32, x . disc, the norm and disc rounded to float32).
+ * costs[doc_off[d] + i] = max((x_i . x_{i+1} + 1) / 2, sqrt(FLT_EPSILON)) in float32 for i < n - 1; then, i ascending
+ * over i < n - 1 with the first chunklet counted as preceded by a heading, a heading i (is_heading[]) sets
+ * costs[i] = 1 and divides costs[i - 1] by 4 when chunklet i - 1 is not a heading.  The slot of each document's last
+ * row is not written.  status[d] = 0, or 1 when a row has zero norm (then no cost of d is written).  A documented
+ * bound from float64, not the reference's bits. */
+int rl_chunk_similarities(const void* X, int x_dtype, int64_t ld, int dim, const int64_t* doc_off, int n_docs,
+                          int64_t n_rows, const uint8_t* nonoutlying, const uint8_t* is_heading, float* costs,
+                          int32_t* status, void* workspace, size_t workspace_bytes, void* stream);
+size_t rl_chunk_partition_workspace_bytes(int64_t n_chunklets, int n_docs);
+/* split_chunks' partition: cost(j, i) = costs[doc_off[d] + j - 1] widened to float64 for j > 0, 0 for j = 0 (a chunk
+ * starting at j pays for the cut before it), lens the chunklet lengths.  This is the optimum of the reference's integer
+ * program.  status[d] = 0, or 1 when a chunklet is longer than max_size[d] (no partition; counts[d] = 0). */
+int rl_chunk_partition(const float* costs, const int32_t* lens, const int64_t* doc_off, const int32_t* max_size,
+                       int n_docs, int64_t n_chunklets, int32_t* cuts, int32_t* counts, int32_t* status,
+                       void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -5,9 +5,19 @@ Drop-in surface (reference ``raglite/__init__.py`` names for this path): ``RAGLi
 ``ShardedIndex`` that replace the database for this path and the batched ``vector_search_batch`` /
 ``keyword_search_batch``; and
 ``TokenEmbedderEngine``, the embedding model's encoder on the GPU behind ``embed_strings`` / ``embed_queries``; and
-``split_sentences`` with ``SaTEngine``, the sentence splitter's SaT model and partition on the GPU.
+``split_sentences`` with ``SaTEngine``, the sentence splitter's SaT model and partition on the GPU; and
+``split_chunklets`` / ``split_chunks`` / ``split_documents``, the chunklet and chunk partitions on the GPU.
 """
 
+from ._chunks import (
+    embed_strings_batch,
+    markdown_chunklet_boundaries,
+    split_chunklets,
+    split_chunklets_batch,
+    split_chunks,
+    split_chunks_batch,
+    split_documents,
+)
 from ._config import RAGLiteConfig
 from ._embed import embed_queries, embed_strings, register_token_embedder
 from ._index import Chunk, CorpusIndex, get_index, merge_hits, register_index, unregister_index
@@ -57,6 +67,13 @@ __all__ = [
     "rrf_fuse_device",
     "embed_queries",
     "embed_strings",
+    "embed_strings_batch",
+    "markdown_chunklet_boundaries",
+    "split_chunklets",
+    "split_chunklets_batch",
+    "split_chunks",
+    "split_chunks_batch",
+    "split_documents",
     "get_index",
     "merge_hits",
     "register_index",

@@ -30,7 +30,9 @@ EXPORTS = [
     "rl_xenc_embed_ln", "rl_xenc_add_ln", "rl_xenc_cls_head", "rl_bm25_stats", "rl_bm25_workspace_bytes",
     "rl_bm25_packed_bytes", "rl_bm25_topk_global", "rl_bm25_merge_packed", "rl_tsrank_topk_global",
     "rl_sat_token_logits", "rl_sat_workspace_bytes", "rl_sat_char_probas", "rl_sentence_partition_workspace_bytes",
-    "rl_sentence_partition",
+    "rl_sentence_partition", "rl_chunklet_partition_workspace_bytes", "rl_chunklet_partition",
+    "rl_chunk_similarities_workspace_bytes", "rl_chunk_similarities", "rl_chunk_partition_workspace_bytes",
+    "rl_chunk_partition",
 ]
 
 
@@ -134,10 +136,21 @@ def _declare(lib: C.CDLL) -> None:
     lib.rl_sentence_partition_workspace_bytes.argtypes = [i64]
     lib.rl_sentence_partition_workspace_bytes.restype = C.c_size_t
     lib.rl_sentence_partition.argtypes = [vp, vp, vp, vp, vp, i32, i64, vp, vp, vp, vp, C.c_size_t, vp]
+    lib.rl_chunklet_partition_workspace_bytes.argtypes = [i64, i32]
+    lib.rl_chunklet_partition.argtypes = [vp, vp, vp, vp, vp, i32, i64, vp, vp, vp, vp, C.c_size_t, vp]
+    lib.rl_chunk_similarities_workspace_bytes.argtypes = [i64]
+    lib.rl_chunk_similarities.argtypes = [vp, i32, i64, i32, vp, i32, i64, vp, vp, vp, vp, vp, C.c_size_t, vp]
+    lib.rl_chunk_partition_workspace_bytes.argtypes = [i64, i32]
+    lib.rl_chunk_partition.argtypes = [vp, vp, vp, vp, i32, i64, vp, vp, vp, vp, C.c_size_t, vp]
+    for name in ("rl_chunklet_partition_workspace_bytes", "rl_chunk_similarities_workspace_bytes",
+                 "rl_chunk_partition_workspace_bytes"):
+        getattr(lib, name).restype = C.c_size_t
     for name in EXPORTS:
         if name not in ("rl_last_error", "rl_maxsim_workspace_bytes", "rl_xenc_linear_image_bytes", "rl_xenc_workspace_bytes",
                         "rl_hits_packed_bytes", "rl_bm25_workspace_bytes", "rl_bm25_packed_bytes",
-                        "rl_sat_workspace_bytes", "rl_sentence_partition_workspace_bytes"):
+                        "rl_sat_workspace_bytes", "rl_sentence_partition_workspace_bytes",
+                        "rl_chunklet_partition_workspace_bytes", "rl_chunk_similarities_workspace_bytes",
+                        "rl_chunk_partition_workspace_bytes"):
             getattr(lib, name).restype = C.c_int
 
 

@@ -105,14 +105,14 @@ def whitespace_flags(text: str) -> np.ndarray:
     return np.isin(code_points(text), _SPACE_CODEPOINTS)
 
 
-def markdown_sentence_boundaries(doc: str) -> np.ndarray:
+def markdown_sentence_boundaries(doc: str, tokens: list[Any] | None = None) -> np.ndarray:
     """Known boundary probabilities from the Markdown headings (``_split_sentences.py:23-53``): for each heading the
     character before it gets 1, its body 0 and its last character 1 (its line span, counted over ``str.splitlines``);
-    NaN elsewhere."""
+    NaN elsewhere.  ``tokens`` is markdown-it's parse of ``doc`` when the caller already has it."""
     from markdown_it import MarkdownIt
 
     out = np.full(len(doc), np.nan)
-    spans = [t.map for t in MarkdownIt().parse(doc) if t.type == "heading_open"]
+    spans = [t.map for t in (MarkdownIt().parse(doc) if tokens is None else tokens) if t.type == "heading_open"]
     if not spans:
         return out
     line_start = np.zeros(1, np.int64)

@@ -13,7 +13,9 @@ installed), but two pieces of the hot path are pure NumPy/SciPy once their impor
 * ``raglite/_typing.py`` -- the column processors of the ``chunk_embedding.embedding`` column
   (DuckDB ``FLOAT[d]`` lists, PostgreSQL ``halfvec`` text, ``np.save`` blobs);
 * ``raglite/_split_sentences.py`` -- ``split_sentences`` and ``markdown_sentence_boundaries``, with wtpsplit-lite's
-  ``SaT`` replaced by a fake that returns seeded float32 probabilities.
+  ``SaT`` replaced by a fake that returns seeded float32 probabilities;
+* ``raglite/_split_chunklets.py`` and ``raglite/_split_chunks.py`` -- ``split_chunklets`` (with its Markdown boundaries
+  and statement counts) and ``split_chunks`` (with the cost vector it hands to ``linprog``).
 
 This script loads those two files *unmodified from where they lie* under a synthetic ``raglite``
 package whose heavy dependencies are replaced by stubs, and whose embedder is
@@ -316,6 +318,129 @@ def golden_split_sentences() -> None:
     print("split_sentences", len(cases), "cases,", sum(c["error"] is not None for c in cases), "errors")
 
 
+def _sentences_of(doc: str) -> list[str]:
+    """A document cut after every '. ', '? ', '! ' and newline (the pieces join back to the document)."""
+    import re
+
+    return [s for s in re.split(r"(?<=[.?!] )|(?<=\n)", doc) if s]
+
+
+def _chunk_docs(seed: int) -> dict[str, str]:
+    rng = np.random.default_rng(seed)
+    words = "alpha beta gamma delta light clock rod frame event time of the observer velocity".split()
+
+    def para(n: int) -> str:
+        return " ".join(" ".join(str(w) for w in rng.choice(words, size=int(rng.integers(3, 14)))) + "."
+                        for _ in range(n))
+
+    return {
+        "atx": f"# Title\n\n{para(3)}\n\n## Section\n\n{para(4)}\n\n### Deeper\n{para(2)}\n",
+        "setext": f"Heading one\n===========\n\n{para(3)}\n\nHeading two\n-----------\n{para(3)}\n",
+        "lists": f"{para(2)}\n\n- {para(1)}\n- {para(2)}\n- item\n\n1. first {para(1)}\n2. second\n\n{para(2)}\n",
+        "quotes": f"{para(2)}\n\n> {para(2)}\n> {para(1)}\n\n{para(3)}\n",
+        "consecutive": f"# A\n## B\n### C\n- x\n- y\n> q\n\n{para(2)}\n# D\n\n{para(5)}\n",
+        "whitespace": f"{para(2)}\n\n   \n\t\n\n{para(3)}\n  \n",
+        "prose": para(40),
+    }
+
+
+def golden_split_chunklets() -> None:
+    """``split_chunklets`` and ``markdown_chunklet_boundaries`` (``_split_chunklets.py``) run unmodified on Markdown
+    headings (ATX and setext), lists, block quotes, consecutive boundaries, whitespace-only sentences, a sentence longer
+    than max_size and one sentence, at several max_size values; the empty document records its error."""
+    for name in ("raglite", "raglite._typing"):
+        sys.modules.pop(name, None)
+    pkg = types.ModuleType("raglite")
+    pkg.__path__ = []
+    sys.modules["raglite"] = pkg
+    _stub("raglite._typing", FloatVector=np.ndarray)
+    mod = _load("raglite._split_chunklets", REF / "_split_chunklets.py")
+    docs = {k: _sentences_of(v) for k, v in _chunk_docs(41).items()}
+    docs["long_middle"] = ["a b. "] * 5 + ["x" * 50] + ["c d. "] * 5
+    docs["long_first"] = ["x" * 50] + ["a b. "] * 5 + ["c d. "] * 5
+    docs["long_first_short"] = ["x" * 50] + ["c d. "] * 5
+    docs["one"] = ["Just one sentence."]
+    docs["spaces_only"] = ["   ", "\n", " \t "]
+    cases = []
+    for name, sents in docs.items():
+        for max_size in (20, 64, 256, 2048):
+            out = mod.split_chunklets(sents, max_size=max_size)
+            cases.append({"name": name, "sentences": sents, "max_size": max_size, "chunklets": out, "error": None,
+                          "md": mod.markdown_chunklet_boundaries(sents).tolist(),
+                          "statements": mod.compute_num_statements(sents).tolist()})
+    try:
+        mod.split_chunklets([])
+    except ValueError as e:
+        cases.append({"name": "empty", "sentences": [], "max_size": 2048, "chunklets": None, "error": str(e)})
+    np.savez_compressed(GOLDEN / "split_chunklets.npz", cases=np.frombuffer(json.dumps(cases).encode(), dtype=np.uint8))
+    print("split_chunklets", len(cases), "cases")
+
+
+def golden_split_chunks() -> None:
+    """``split_chunks`` (``_split_chunks.py``) run unmodified on seeded fp16 and fp32 chunklet embeddings: Markdown
+    headings, several max_size values, identical rows (the projection is skipped), and the long-chunklet and zero-norm
+    errors.  Each solved case also stores the float32 cost vector the reference hands to ``linprog``."""
+    for name in ("raglite", "raglite._typing"):
+        sys.modules.pop(name, None)
+    pkg = types.ModuleType("raglite")
+    pkg.__path__ = []
+    sys.modules["raglite"] = pkg
+    _stub("raglite._typing", FloatMatrix=np.ndarray)
+    mod = _load("raglite._split_chunks", REF / "_split_chunks.py")
+    seen: list[np.ndarray] = []
+    real_linprog = mod.linprog
+
+    def spy(c, **kw):  # noqa: ANN001, ANN003, ANN202
+        seen.append(np.array(c, copy=True))
+        return real_linprog(c, **kw)
+
+    mod.linprog = spy
+    rng = np.random.default_rng(43)
+    cases, arrays = [], {}
+
+    def run(name: str, chunklets: list[str], emb: np.ndarray, max_size: int) -> None:
+        i = len(cases)
+        arrays[f"emb{i}"] = emb
+        seen.clear()
+        try:
+            chunks, _ = mod.split_chunks(chunklets, emb, max_size=max_size)
+            err = None
+        except ValueError as e:
+            chunks, err = None, str(e)
+        if seen:
+            arrays[f"cost{i}"] = seen[0]
+        cases.append({"name": name, "chunklets": chunklets, "max_size": max_size, "chunks": chunks, "error": err,
+                      "solved": bool(seen)})
+
+    def rows(n: int, d: int, dtype: type, topics: int = 4) -> np.ndarray:
+        centers = rng.standard_normal((topics, d))
+        which = np.sort(rng.integers(0, topics, size=n))
+        return (centers[which] + 0.8 * rng.standard_normal((n, d))).astype(dtype)
+
+    words = "alpha beta gamma delta light clock rod frame event time of the observer velocity".split()
+    for k in range(24):
+        n = int(rng.integers(3, 80))
+        chunklets = []
+        for _ in range(n):
+            body = " ".join(str(w) for w in rng.choice(words, size=int(rng.integers(3, 90)))) + ". "
+            chunklets.append(("# " + body[:30] + "\n") if rng.random() < 0.2 else body)
+        emb = rows(n, int(rng.choice([16, 48, 64])), np.float16 if k % 3 else np.float32)
+        for max_size in (600, 2048):
+            run(f"doc{k}", chunklets, emb, max_size)
+    same = ["alpha beta gamma. " * 3] * 12
+    run("identical_rows", same, np.tile(rng.standard_normal((1, 32)).astype(np.float16), (12, 1)), 128)
+    run("identical_rows_f32", same, np.tile(rng.standard_normal((1, 32)).astype(np.float32), (12, 1)), 200)
+    run("one_chunklet", ["# Only\n"], rows(1, 16, np.float16), 64)
+    run("fits", ["a. ", "b. ", "c. "], rows(3, 16, np.float16), 64)
+    run("too_long", ["a" * 70, "b. "], rows(2, 16, np.float16), 64)
+    zero = rows(4, 16, np.float16)
+    zero[2] = 0
+    run("zero_norm", ["a. " * 10, "b. " * 10, "c. " * 10, "d. " * 10], zero, 40)
+    np.savez_compressed(GOLDEN / "split_chunks.npz", cases=np.frombuffer(json.dumps(cases).encode(), dtype=np.uint8),
+                        **arrays)
+    print("split_chunks", len(cases), "cases,", sum(c["solved"] for c in cases), "solved")
+
+
 if __name__ == "__main__":
     GOLDEN.mkdir(parents=True, exist_ok=True)
     golden_rrf()
@@ -324,3 +449,5 @@ if __name__ == "__main__":
     golden_adapter(qa_mod)
     golden_table_rows(load_reference_typing())
     golden_split_sentences()
+    golden_split_chunklets()
+    golden_split_chunks()
