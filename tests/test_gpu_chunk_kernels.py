@@ -1,6 +1,7 @@
 """The chunk kernels at the C-ABI: ``rl_chunklet_partition`` and ``rl_chunk_partition`` bit for bit against the
 restated loops of ``chunks_oracle`` (one launch of thousands of documents, each with its own max_size, dyadic costs
-that tie everywhere, infinite windows, windows wider than 32 and 512 items, documents past the grid stride), and
+that tie everywhere, infinite windows, windows wider than 32 and 512 items, documents past the grid stride; seeded
+non-dyadic costs; statement counts of 0; length prefixes past 2^31), and
 ``rl_chunk_similarities`` within ``chunks_oracle.chunk_cost_bound`` of float64.  Sentinels guard every output slice.
 The largest similarity error as a fraction of the bound goes to ``chunk_errors.jsonl`` in the temporary directory."""
 
@@ -234,3 +235,74 @@ def test_chunk_similarities_skip_exact_zero_projection(dtype):
     assert got[:5].tolist() == [1.0, 0.25, 1.0, 1.0, 1.0]        # the cut before the heading divided by 4
     want, info = co.chunk_costs_f64(other, np.ones(5, bool), np.zeros(5, bool))
     assert info["proj"] and (np.abs(got[6:10] - want) <= co.chunk_cost_bound(dim, 5, info)).all()
+
+
+def test_chunk_partition_non_dyadic_costs():
+    """Seeded float32 costs that round in the sums: random values, sqrt(eps), 1.0, the quarters the heading rule makes
+    and values repeated across different cuts of a document, in one launch of 9000 documents."""
+    rng = np.random.default_rng(3)
+    docs = _docs(rng, 9000)
+    special = np.float32([co.SQRT_EPS32, co.SQRT_EPS32 / 4, 1.0, 0.25])
+    costs = []
+    for lens, _ in docs:
+        c = rng.random(len(lens)).astype(np.float32) * np.float32(0.999) + co.SQRT_EPS32
+        c = np.where(rng.random(len(c)) < 0.2, c / np.float32(4), c)
+        c = np.where(rng.random(len(c)) < 0.15, rng.choice(special, size=len(c)), c)
+        c = np.where(rng.random(len(c)) < 0.2, c[0], c)                  # equal costs at different j
+        c[-1] = np.nan
+        costs.append(c.astype(np.float32))
+    off, h, counts, status = _run_partition("chunk", docs, [np.concatenate(costs)])
+    nontrivial = 0
+    for i, (lens, mx) in enumerate(docs):
+        if (lens > mx).any():
+            assert status[i] == 1 and counts[i] == 0, i
+            continue
+        assert status[i] == 0, i
+        want = co.chunk_cuts(costs[i][:-1], lens, mx)
+        assert h[off[i]:off[i] + counts[i]].tolist() == want, i
+        assert (h[off[i] + counts[i]:off[i] + len(lens)] == SENT).all(), i
+        nontrivial += len(want) > 1
+    assert nontrivial > 1000
+
+
+def test_chunklet_partition_zero_statements():
+    """Statement counts of 0 in every document, so a window of no statements takes sqrt(max(s, 1e-6)); non-dyadic
+    probabilities."""
+    rng = np.random.default_rng(4)
+    docs = _docs(rng, 2000)
+    p = [rng.random(len(x)) for x, _ in docs]
+    st = [np.where(rng.random(len(x)) < 0.5, 0.0, rng.choice([0.5, 1.0, 2.0, 3.0], size=len(x))) for x, _ in docs]
+    off, h, counts, status = _run_partition("chunklet", docs, [np.concatenate(p), np.concatenate(st)])
+    assert (status == 0).all()
+    empty_windows = 0
+    for i, (lens, mx) in enumerate(docs):
+        want = co.chunklet_cuts(p[i], st[i], lens, mx)
+        assert h[off[i]:off[i] + counts[i]].tolist() == want, i
+        edges = [0, *want, len(lens)]
+        empty_windows += sum(st[i][a:b].sum() == 0 for a, b in zip(edges[:-1], edges[1:]))
+    assert empty_windows > 100                              # chunklets without statements are chosen, not only tried
+
+
+def test_partitions_past_2_31_characters():
+    """Documents of lengths near 2^30 with max_size near 2^31 - 1: the length prefixes pass 2^31 (a 32-bit prefix
+    wraps), and a window holds one to three items."""
+    rng = np.random.default_rng(5)
+    docs = []
+    for _ in range(64):
+        n = int(rng.integers(6, 24))
+        lens = rng.integers(2**28, 2**30 + 1, size=n).astype(np.int32)
+        docs.append((lens, int(rng.integers(2**31 - 2**28, 2**31))))
+    assert max(int(x.astype(np.int64).sum()) for x, _ in docs) > 2**33
+    costs = [rng.random(len(x)).astype(np.float32) for x, _ in docs]
+    off, h, counts, status = _run_partition("chunk", docs, [np.concatenate(costs)])
+    p = [rng.random(len(x)) for x, _ in docs]
+    st = [rng.choice([0.0, 1.0, 2.0, 4.0], size=len(x)) for x, _ in docs]
+    off2, h2, counts2, status2 = _run_partition("chunklet", docs, [np.concatenate(p), np.concatenate(st)])
+    assert (status == 0).all() and (status2 == 0).all()
+    multi = 0
+    for i, (lens, mx) in enumerate(docs):
+        want = co.chunk_cuts(costs[i][:-1], lens, mx)
+        assert h[off[i]:off[i] + counts[i]].tolist() == want, i
+        assert h2[off2[i]:off2[i] + counts2[i]].tolist() == co.chunklet_cuts(p[i], st[i], lens, mx), i
+        multi += len(want) < len(lens) - 1                  # some chunk holds more than one item
+    assert multi > 10

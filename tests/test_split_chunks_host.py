@@ -1,6 +1,8 @@
 """``split_chunklets`` / ``split_chunks`` on the host: the restatements against the reference's own outputs
 (``tests/golden/split_chunklets.npz`` and ``split_chunks.npz``), the windowed dynamic program against ``linprog``, the
-``pow`` against ``d * d`` difference, and every refusal before any CUDA call."""
+``pow`` against ``d * d`` difference, every refusal before any CUDA call, and the restatement of
+``rl_chunk_similarities`` that ``test_gpu_chunk_similarity_exact.py`` relies on (``fma64`` against exact fractions, the
+restatement against float64 and the reference's costs, the planted rows of the projection test's edge)."""
 
 from __future__ import annotations
 
@@ -227,3 +229,101 @@ def test_similarities_refusals():
         assert sim(**{k: None}) == RL_EINVAL, k
     assert sim(ws_bytes=need - 1) == RL_ENOSPACE
     assert sim(D=0, ws_bytes=0, **{k: None for k in names}) == 0
+
+
+# ---- the lane-exact restatement of rl_chunk_similarities -------------------------------------------------------------
+def _fma_exact64(a, b, c) -> np.ndarray:
+    """a b + c in exact rational arithmetic, rounded once (``float`` of a Fraction is correctly rounded, ties to even)."""
+    return np.array([float(Fraction(float(x)) * Fraction(float(y)) + Fraction(float(z)))
+                     for x, y, z in zip(a, b, c, strict=True)])
+
+
+def test_fma64_against_fractions():
+    """``chunks_oracle.fma64`` is a correctly rounded a b + c: random triples with magnitudes from 2^-60 to 2^60, c
+    close to -a b (cancellation), and planted triples whose exact value is a float64 midpoint, or one ulp of the
+    product's error term off it."""
+    rng = np.random.default_rng(11)
+    n = 6000
+    a, b, c = (rng.standard_normal(n) * 2.0 ** rng.integers(-60, 61, n) for _ in range(3))
+    near = rng.random(n) < 0.4
+    c[near] = -(a[near] * b[near]) * (1 + rng.standard_normal(near.sum()) * 2.0 ** rng.integers(-52, -20, near.sum()))
+    np.testing.assert_array_equal(co.fma64(a, b, c), _fma_exact64(a, b, c))
+    # midpoints: a b within a rounding of half an ulp of c, a with a 26-bit significand, so a (h / a) = h (1 + delta)
+    # with |delta| <= 2^-53: exactly on the midpoint (a a power of two) or just off it, on either side
+    c = rng.standard_normal(n) * 2.0 ** rng.integers(-40, 41, n)
+    h = (np.nextafter(np.abs(c), np.inf) - np.abs(c)) / 2 * np.where(rng.random(n) < 0.5, -1.0, 1.0)
+    a = np.ldexp(rng.integers(2**25, 2**26, n).astype(np.float64), -25) * 2.0 ** rng.integers(-20, 21, n)
+    a[: n // 4] = 2.0 ** rng.integers(-20, 21, n // 4)
+    b = h / a
+    step = rng.integers(-1, 2, n)
+    b = np.where(step > 0, np.nextafter(b, np.inf), np.where(step < 0, np.nextafter(b, -np.inf), b))
+    want = _fma_exact64(a, b, c)
+    np.testing.assert_array_equal(co.fma64(a, b, c), want)
+    assert ((a * b + c) != want).sum() > n // 20               # the two-rounding answer is often wrong here
+    # an exact zero: +0 but for (-0) + (-0), as IEEE round-to-nearest gives
+    z = co.fma64([2.0, -0.0, 0.0, 3.0], [3.0, 1.0, -1.0, 2.0**-30], [-6.0, -0.0, -0.0, -3.0 * 2.0**-30])
+    assert z.view(np.uint64).tolist() == [0, 1 << 63, 1 << 63, 0]
+
+
+def _random_doc(rng, n: int, dim: int, dtype):
+    centers = rng.standard_normal((3, dim))
+    X = centers[rng.integers(0, 3, size=n)] + rng.standard_normal((n, dim))
+    return (X * 2.0 ** rng.integers(-6, 7, size=(n, 1))).astype(dtype)
+
+
+def test_chunk_costs_device_within_float64_bound():
+    """The restatement computes the cost formula: within ``chunk_cost_bound`` of ``chunk_costs_f64`` per document (the
+    rows of each document at their own scale), fp16 and fp32 rows, widths off and on the multiples of 32 and 256."""
+    rng = np.random.default_rng(12)
+    for dtype in (np.float16, np.float32):
+        for dim in (2, 31, 33, 257, 1000):
+            docs = [_random_doc(rng, int(n), dim, dtype) for n in rng.integers(2, 40, size=12)]
+            keeps = [rng.random(len(X)) < 0.7 for X in docs]
+            heads = [rng.random(len(X)) < 0.2 for X in docs]
+            off = np.concatenate([[0], np.cumsum([len(X) for X in docs])])
+            got, status, proj = co.chunk_costs_device(np.concatenate(docs), dim, off, np.concatenate(keeps),
+                                                      np.concatenate(heads))
+            assert (status == 0).all()
+            for i, (X, keep, head) in enumerate(zip(docs, keeps, heads, strict=True)):
+                want, info = co.chunk_costs_f64(X, keep, head)
+                g = got[off[i]:off[i + 1]]
+                assert np.isnan(g[-1]) and proj[i] == info["proj"], (dtype, dim, i)
+                err = np.abs(g[:-1] - want)
+                assert (err <= co.chunk_cost_bound(dim, int(keep.sum()), info)).all(), (dtype, dim, i)
+
+
+def test_chunk_costs_device_on_golden_cases(golden_dir):
+    """On the reference's own cases, the restatement's costs are within the bound of the reference's float32 costs
+    wherever both take the same projection decision (every case but those where a row's exact projection is zero)."""
+    cases, z = _cases(golden_dir, "split_chunks.npz")
+    checked = 0
+    for i, c in enumerate(cases):
+        if not c["solved"]:
+            continue
+        X = z[f"emb{i}"]
+        keep = co.nonoutlying([len(x) for x in c["chunklets"]])
+        head = np.array([co.is_heading(x) for x in c["chunklets"]])
+        got, status, proj = co.chunk_costs_device(X, X.shape[1], [0, len(X)], keep, head)
+        _, info = co.chunk_costs_f64(X, keep, head)
+        assert status[0] == 0 and proj[0] == info["proj"], c["name"]
+        if keep.any() and float(info["pn_all"].min()) < 1e-9:
+            continue                                                      # the reference's test follows rounding
+        err = np.abs(got[:-1].astype(np.float64) - z[f"cost{i}"])
+        assert (err <= co.chunk_cost_bound(X.shape[1], int(keep.sum()), info)).all(), c["name"]
+        checked += 1
+    assert checked >= 40
+
+
+
+@pytest.mark.parametrize("dtype", [np.float16, np.float32])
+def test_projection_edge_rows_decide_alike(dtype):
+    """The planted rows of the projection test's edge: the restatement skips the projection at |y| = eps and keeps it
+    one step above, and the reference's float32 NumPy (run on the same mask) takes the same decisions and costs."""
+    for delta, kept in co.EPS_EDGE[np.dtype(dtype)]:
+        X = co.eps_edge_rows(delta, 40, dtype)
+        head = np.zeros(4, bool)
+        got, status, proj = co.chunk_costs_device(X, 40, [0, 4], co.EPS_EDGE_KEEP, head)
+        assert status[0] == 0 and proj[0] == kept, delta
+        want = co.chunk_costs_f32_flags(X, co.EPS_EDGE_KEEP, head)
+        np.testing.assert_array_equal(got[:-1], want)
+        assert (want[:2] == co.SQRT_EPS32).all() == kept       # kept: rows 0 and 1 project onto -e1 and e1
