@@ -512,6 +512,44 @@ int rl_chunk_partition(const float* costs, const int32_t* lens, const int64_t* d
                        int n_docs, int64_t n_chunklets, int32_t* cuts, int32_t* counts, int32_t* status,
                        void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- text analysis of the BM25 index: DuckDB fts's tokenizer, english stop list and Snowball porter stemmer ----------
+ * The host analyzer (raglite_b200/_fts.py, Analyzer.analyze) bit for bit, in four steps around two host round trips:
+ * rl_fts_mark finds the words, rl_fts_stem stems them, rl_fts_verify and rl_fts_stem_bytes settle the distinct stems
+ * exactly, rl_fts_term_keys turns the term id of each distinct stem into postings keys.  No global atomics: every
+ * output is the same run to run.
+ *
+ * rl_fts_mark: text = n_bytes of UTF-8 (bodies joined by a separator byte, so that no word spans two bodies).
+ * class_table uint8 [0x110000] (device) classifies each code point as lower(strip_accents(chr(cp))) does: 1..26 the
+ * letter a..z, 0xFF dropped (it vanishes: combining marks and what decomposes into marks only), anything else a
+ * separator.  '\' is a separator that, with the dropped code points removed, swallows the letter right after a run of
+ * backslashes of odd length (the `\\.` of the tokenizer's regular expression).  Writes mark uint8 [n_bytes]: at the
+ * lead byte of each kept letter the letter, upper case when it starts a word, lower case otherwise; 0 at every other
+ * byte.  A parallel scan of the tokenizer's three-state automaton, exact for runs of any length.  workspace >=
+ * rl_fts_workspace_bytes(n_bytes); n_bytes == 0 is valid and launches nothing. */
+size_t rl_fts_workspace_bytes(int64_t n_bytes);
+int rl_fts_mark(const uint8_t* text, int64_t n_bytes, const uint8_t* class_table, uint8_t* mark, void* workspace,
+                size_t workspace_bytes, void* stream);
+/* rl_fts_stem: word w = letters[word_off[w] .. word_off[w + 1]) (letters uint8 'a'..'z', word_off int64 [n_words + 1],
+ * both device).  stop (device uint64 [n_stop][2]): the stop list, each entry zero-padded to 16 bytes and read as two
+ * big-endian uint64 (hi, lo), sorted ascending.  A word equal to an entry gets keep[w] = -1.  Any other word is stemmed
+ * by Snowball's porter: its stem is letters word_off[w] .. word_off[w] + keep[w] followed by the nonzero bytes of
+ * tail[w], low byte first (at most 8), and hash[w] is a 64-bit hash of the stem cut to its low hash_bits bits
+ * (1 <= hash_bits <= 64; fewer bits only make collisions, which rl_fts_verify detects). */
+int rl_fts_stem(const uint8_t* letters, const int64_t* word_off, int64_t n_words, const uint64_t* stop, int n_stop,
+                int hash_bits, int32_t* keep, uint64_t* tail, int64_t* hash, void* stream);
+/* rl_fts_verify: differ[t] = 1 when the stems of the words word_a[t] and word_b[t] differ byte for byte, else 0
+ * (word_a, word_b int64 [n]; stems as rl_fts_stem left them, of words with keep >= 0). */
+int rl_fts_verify(const uint8_t* letters, const int64_t* word_off, const int32_t* keep, const uint64_t* tail,
+                  const int64_t* word_a, const int64_t* word_b, int64_t n, uint8_t* differ, void* stream);
+/* rl_fts_stem_bytes: the stems of words[0 .. n) as a bytes CSR: stem u at out[out_off[u] .. out_off[u + 1]) (out_off
+ * int64 [n + 1], each length keep + the number of tail letters). */
+int rl_fts_stem_bytes(const uint8_t* letters, const int64_t* word_off, const int32_t* keep, const uint64_t* tail,
+                      const int64_t* words, int64_t n, const int64_t* out_off, uint8_t* out, void* stream);
+/* rl_fts_term_keys: the postings keys of n tokens, key[t] = stem_term[tok_stem[t]] << 32 | (chunk_base + owner[t])
+ * (tok_stem, owner int64 [n]; stem_term int32, the term id of each distinct stem; chunk_base >= 0). */
+int rl_fts_term_keys(const int64_t* tok_stem, const int64_t* owner, int64_t n, const int32_t* stem_term,
+                     int64_t chunk_base, int64_t* key, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -10,8 +10,10 @@ Layout on the device (``rl_bm25_stats`` / ``rl_bm25_topk_global``, include/ragli
     df        int32   [V]       live chunks holding each term       (rl_bm25_stats, recomputed after every change)
     corpus    float64 [3]       N, sum of doc_len, avgdl over the live chunks
 
-The host keeps the ``stem -> term id`` dictionary (``_fts.Analyzer``) and, from each refresh, ``df``, ``N`` and the sum
-of ``doc_len`` as integers: a search looks up the statistics of its query terms there and uploads them with its plan.
+The bodies are analysed on the device (``_fts.analyze_on_device``); the host keeps the ``stem -> term id`` dictionary
+(``_fts.Analyzer``, which the device analysis grows exactly as the host analysis would) and, from each refresh, ``df``,
+``N`` and the sum of ``doc_len`` as integers: a search looks up the statistics of its query terms there and uploads them
+with its plan.
 A ``CorpusIndex`` owns one of these and builds it on its first keyword search; appended chunks are analysed on the next
 search, deletes only make the statistics stale (tombstoned chunks keep their postings and are masked), ``compact``
 remaps the postings.
@@ -31,7 +33,7 @@ import numpy as np
 import torch
 
 from . import _lib, _pgfts
-from ._fts import Analyzer
+from ._fts import Analyzer, analyze_on_device
 
 K1, B_PARAM = 1.2, 0.75          # match_bm25 defaults
 MAX_RESULTS = 4096               # RL_MAX_SURVIVORS, the num_hits cap of the vector path
@@ -146,21 +148,20 @@ class KeywordIndex(_Postings):
         self.alive: torch.Tensor | None = None   # uint8 [C] of the last refresh; None = no tombstones
         self.stale = True
         self.build_seconds = {"analysis": 0.0, "postings": 0.0}
+        self.analysis_seconds = {"encode": 0.0, "device": 0.0, "dictionary": 0.0}   # the split of build_seconds["analysis"]
 
     def extend(self, bodies: Sequence[str]) -> None:
-        """Index the bodies of the chunks ``n_chunks, n_chunks + 1, ...`` (new terms get new ids).  The new (term, chunk)
-        pairs are counted and merged into the postings on the device: one sort of the packed ``term << 32 | chunk``
-        keys."""
+        """Index the bodies of the chunks ``n_chunks, n_chunks + 1, ...`` (new terms get new ids).  The bodies are
+        analysed on the device (``_fts.analyze_on_device``: the packed ``term << 32 | chunk`` key of every kept token),
+        and the new (term, chunk) pairs are counted and merged into the postings there: one sort of the keys."""
         t0 = time.perf_counter()
-        terms, owners, lens = self.analyzer.analyze(bodies)
-        t1 = time.perf_counter()
         dev = self.device
+        key, lens = analyze_on_device(self.analyzer, bodies, dev, chunk_base=self.n_chunks, seconds=self.analysis_seconds)
+        t1 = time.perf_counter()
         with torch.cuda.device(dev):
-            owners = torch.from_numpy(owners).to(dev, dtype=torch.int64) + self.n_chunks
-            key = (torch.from_numpy(terms).to(dev, dtype=torch.int64) << 32) | owners
             key, tf = torch.unique(key, sorted=True, return_counts=True)
             self.tf = self._merge_postings(key, tf, self.tf, len(self.analyzer.term_ids))
-            self.doc_len = torch.cat([self.doc_len, torch.from_numpy(lens).to(dev)])
+            self.doc_len = torch.cat([self.doc_len, lens])
             torch.cuda.current_stream().synchronize()
         self.n_chunks += len(bodies)
         self.stale = True

@@ -32,7 +32,8 @@ EXPORTS = [
     "rl_sat_token_logits", "rl_sat_workspace_bytes", "rl_sat_char_probas", "rl_sentence_partition_workspace_bytes",
     "rl_sentence_partition", "rl_chunklet_partition_workspace_bytes", "rl_chunklet_partition",
     "rl_chunk_similarities_workspace_bytes", "rl_chunk_similarities", "rl_chunk_partition_workspace_bytes",
-    "rl_chunk_partition",
+    "rl_chunk_partition", "rl_fts_workspace_bytes", "rl_fts_mark", "rl_fts_stem", "rl_fts_verify", "rl_fts_stem_bytes",
+    "rl_fts_term_keys",
 ]
 
 
@@ -142,15 +143,21 @@ def _declare(lib: C.CDLL) -> None:
     lib.rl_chunk_similarities.argtypes = [vp, i32, i64, i32, vp, i32, i64, vp, vp, vp, vp, vp, C.c_size_t, vp]
     lib.rl_chunk_partition_workspace_bytes.argtypes = [i64, i32]
     lib.rl_chunk_partition.argtypes = [vp, vp, vp, vp, i32, i64, vp, vp, vp, vp, C.c_size_t, vp]
+    lib.rl_fts_workspace_bytes.argtypes = [i64]
+    lib.rl_fts_mark.argtypes = [vp, i64, vp, vp, vp, C.c_size_t, vp]
+    lib.rl_fts_stem.argtypes = [vp, vp, i64, vp, i32, i32, vp, vp, vp, vp]
+    lib.rl_fts_verify.argtypes = [vp, vp, vp, vp, vp, vp, i64, vp, vp]
+    lib.rl_fts_stem_bytes.argtypes = [vp, vp, vp, vp, vp, i64, vp, vp, vp]
+    lib.rl_fts_term_keys.argtypes = [vp, vp, i64, vp, i64, vp, vp]
     for name in ("rl_chunklet_partition_workspace_bytes", "rl_chunk_similarities_workspace_bytes",
-                 "rl_chunk_partition_workspace_bytes"):
+                 "rl_chunk_partition_workspace_bytes", "rl_fts_workspace_bytes"):
         getattr(lib, name).restype = C.c_size_t
     for name in EXPORTS:
         if name not in ("rl_last_error", "rl_maxsim_workspace_bytes", "rl_xenc_linear_image_bytes", "rl_xenc_workspace_bytes",
                         "rl_hits_packed_bytes", "rl_bm25_workspace_bytes", "rl_bm25_packed_bytes",
                         "rl_sat_workspace_bytes", "rl_sentence_partition_workspace_bytes",
                         "rl_chunklet_partition_workspace_bytes", "rl_chunk_similarities_workspace_bytes",
-                        "rl_chunk_partition_workspace_bytes"):
+                        "rl_chunk_partition_workspace_bytes", "rl_fts_workspace_bytes"):
             getattr(lib, name).restype = C.c_int
 
 

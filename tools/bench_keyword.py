@@ -4,7 +4,9 @@ next to the NumPy port of DuckDB's FTS tables and ``match_bm25`` (tests/keyword_
 Corpus: seeded, ``--chunks`` bodies (default 1.25 M, the chunk count of the headline shard) of 0-600 words drawn from a
 Zipf distribution over a generated vocabulary.  Queries: ``--batch`` queries of 3-12 words from the same distribution,
 top ``--k`` (256 x top-64: what ``hybrid_search`` asks for under ``search_and_rerank_chunks``' defaults, 2 x 4 x 8).
-Prints one JSON line: index build time (host analysis / device postings / statistics), queries/s end to end, CUDA-event
+Prints one JSON line: index build time (device analysis and its split into host encoding, device work and the dictionary
+round trip / device postings / statistics), the host analyzer (``Analyzer.analyze``) timed on the same bodies and
+``analysis_match`` (the device-built dictionary and postings identical to the host analysis), queries/s end to end, CUDA-event
 time of the top-k launch, per-kernel device times (torch.profiler), algorithmic bytes over kernel time against the
 H100's 3.35 TB/s, the port's queries/s for ``--oracle-queries`` queries, and how many of those the device matched.
 At the default size the host stages dominate the run (generating 375 M words, analysing them for the index and again for
@@ -37,6 +39,9 @@ ap.add_argument("--seed", type=int, default=0)
 ap.add_argument("--shards", type=int, default=0,
                 help="1: also time the sharded path (ShardedIndex(group=None)) against the bare index, alternating, "
                      "and the merge alone at R = 2, 8 and k = 64, 4096")
+ap.add_argument("--accents", type=float, default=0.0,
+                help="a seeded fraction of the vocabulary words get one accented vowel and capitals, so that the "
+                     "analyzers' non-ASCII paths are measured too")
 ap.add_argument("--dialect", choices=["duckdb", "postgresql"], default="duckdb",
                 help="postgresql: ts_rank over synthesised tsvectors instead of BM25")
 args = ap.parse_args()
@@ -55,6 +60,16 @@ from synth import make_corpus
 
 rng = np.random.default_rng(args.seed)
 vocab = ko.make_vocab(args.vocab, args.seed + 1)
+if args.accents > 0:   # one vowel accented, the word capitalised or upper-cased
+    acc_rng = np.random.default_rng(args.seed + 2)
+    accented = dict(zip("aeiou", "áéíóú"))
+    for i in np.flatnonzero(acc_rng.random(len(vocab)) < args.accents):
+        w = vocab[i]
+        at = [j for j, ch in enumerate(w) if ch in accented]
+        if at:
+            j = at[int(acc_rng.integers(0, len(at)))]
+            w = w[:j] + accented[w[j]] + w[j + 1:]
+        vocab[i] = w.upper() if acc_rng.random() < 0.5 else w.capitalize()
 p = 1.0 / np.arange(1, len(vocab) + 1) ** 1.07
 p /= p.sum()
 words_sp = [w + " " for w in vocab]
@@ -246,10 +261,17 @@ alg_bytes = postings * 12 + B * C * 8 * 2 + B * C   # postings (doc, tf, doc_len
 t0 = time.perf_counter()
 an = Analyzer()
 terms, owners, dlen = an.analyze(bodies)
-pairs = np.unique((terms.astype(np.int64) << 32) | owners)
+host_analysis_s = time.perf_counter() - t0
+pairs, pair_tf = np.unique((terms.astype(np.int64) << 32) | owners, return_counts=True)
 ix = ko.FTSIndex(an.term_ids, dlen.astype(np.int64), np.ones(C, bool), owners.astype(np.int64), terms.astype(np.int64),
                  float(C), float(dlen.sum()) / C, np.bincount(pairs >> 32, minlength=len(an.term_ids)).astype(np.int64))
 oracle_build_s = time.perf_counter() - t0
+# the device analysis against the host's: the dictionary, ids included, and the postings it produced
+analysis_match = bool(
+    list(kw.analyzer.term_ids.items()) == list(an.term_ids.items())
+    and np.array_equal(kw.term_off.cpu().numpy(), np.searchsorted(pairs >> 32, np.arange(len(an.term_ids) + 1)))
+    and np.array_equal(kw.doc.cpu().numpy(), (pairs & 0xFFFFFFFF).astype(np.int32))
+    and np.array_equal(kw.tf.cpu().numpy(), pair_tf) and np.array_equal(kw.doc_len.cpu().numpy(), dlen))
 stage("port tables built")
 nq = min(args.oracle_queries, B)
 t0 = time.perf_counter()
@@ -320,7 +342,10 @@ except Exception:  # noqa: BLE001
 print(json.dumps({
     "metric": f"BM25 keyword_search queries/sec ({B} queries x top-{k}, {C} chunks)", "card": card,
     "chunks": C, "tokens": int(lens.sum()), "terms": kw.n_terms, "postings": int(kw.doc.numel()), "corpus_gen_s": gen_s,
-    "build_s": build_s, "build_host_analysis_s": kw.build_seconds["analysis"], "build_device_postings_s": kw.build_seconds["postings"],
+    "build_s": build_s, "build_device_analysis_s": kw.build_seconds["analysis"],
+    "build_device_analysis_split_s": kw.analysis_seconds, "host_analysis_s": host_analysis_s,
+    "analysis_speedup": host_analysis_s / kw.build_seconds["analysis"], "analysis_match": analysis_match,
+    "build_device_postings_s": kw.build_seconds["postings"], "accents": args.accents,
     "stats_s": stats_s, "queries_per_s": B / float(np.median(wall)), "batch_wall_ms_median": 1e3 * float(np.median(wall)),
     "topk_kernel_ms": kernel_ms, "kernel_ms": per_kernel, "query_groups": -(-B // group),
     "algorithmic_gb": alg_bytes / 1e9, "algorithmic_tb_per_s": alg_bytes / (kernel_ms * 1e-3) / 1e12,
