@@ -11,6 +11,7 @@ import numpy as np
 import pytest
 import torch
 
+import fts_oracle as fo
 import keyword_oracle as ko
 from raglite_b200 import _fts
 
@@ -34,18 +35,7 @@ def _check(bodies, **kw):
     return dev
 
 
-HAZARDS = [
-    "", " ", " \t\n.,;!?-", "123 456", "\\\\\\", "\n\n",
-    "Café résumé naïve façade Ærøskøbing Straße İstanbul ﬁne K ÉTÉ",           # accented Latin, ligature, Kelvin sign
-    "Ελληνικά κείμενα με τόνους", "漢字かな交じり文 한국어", "emoji 😀🎉 mixed😀in words",  # Greek, CJK, emoji
-    "ét́e combining̈marks à́̂b ́start end́",         # marks inside words
-    "THE The thé Thé AND aNd alls ALL c'mon don't it's",                          # stop words, any case, accented
-    "lone \ud800 surrogate \udfff here x\ud800y", "nul\x00byte\x00 and \x00",
-    "Kelvin İi ẞ",
-]
-for n in range(1, 6):   # backslash runs before letters, newlines, marks and the end of a body
-    HAZARDS += ["a" + "\\" * n + "bc d", "x" + "\\" * n + "\nyz", "p" + "\\" * n + "́q r", "\\" * n,
-                "k" + "\\" * n + "́\\́m n", "\\" * n + "word"]
+HAZARDS = fo.HAZARDS
 
 
 def test_generated_corpora_and_hazards():
