@@ -305,7 +305,13 @@ typedef struct rl_xenc_layer {
   const float* down_bias;
   const float* ln2_g;
   const float* ln2_b;
+  /* Image type of each linear (appended: every earlier field keeps its offset; a zero-initialised tail is the fp16
+   * images of rl_xenc_pack_linear): RL_XENC_IMAGE_F16 or RL_XENC_IMAGE_QUANT (rl_xenc_pack_qlinear /
+   * rl_xenc_concat_qlinear, K % 128 == 0). */
+  int32_t qkv_type, o_type, up_type, down_type;
 } rl_xenc_layer;
+#define RL_XENC_IMAGE_F16 0
+#define RL_XENC_IMAGE_QUANT 1
 
 typedef struct rl_xenc_weights {
   int32_t n_layers, hidden, n_heads, ffn, vocab, max_pos, type_vocab;
@@ -330,6 +336,25 @@ int rl_xenc_pack_linear(const float* W, int N, int K, void* image, void* stream)
  * K % 8 == 0, bias 16-byte aligned. */
 int rl_xenc_linear(const void* X, const void* image, const float* bias, void* Y, int T, int N, int K, int act,
                    void* stream);
+/* GGUF-quantized weights, by GGML type id: Q8_0 = 8, Q4_K = 12, Q6_K = 14.  `blocks` (device) holds W[N, K] as GGUF
+ * stores it: row n's K / block_elems blocks at n * (K / block_elems) * block_bytes (Q8_0 32 elements in 34 bytes, Q4_K
+ * and Q6_K 256 in 144 and 210).  Values are ggml's formulas in float32 without contraction -- Q8_0 d q, Q4_K
+ * (d sc) q - (dmin m), Q6_K (d sc) (q - 32) -- rounded once to fp16 to nearest even. */
+/* rows x K elements to fp16 out[rows, K]. */
+int rl_dequant_rows_f16(int type, const void* blocks, int64_t rows, int K, void* out, void* stream);
+/* Quantized linear image: the blocks reordered per 128-row pass and 128-element K slice, at most 1.06x the GGUF bytes
+ * plus a 2 KB header holding each pass's type.  N % 32 == 0, N <= 8192, K % 128 == 0 and whole blocks per row; 0 bytes
+ * for any other shape. */
+size_t rl_xenc_qlinear_image_bytes(int type, int N, int K);
+int rl_xenc_pack_qlinear(int type, const void* blocks, int N, int K, void* image, void* stream);
+/* The image of the row-wise concatenation of n_parts images (one K; every part but the last N % 128 == 0), for parts of
+ * different types, e.g. Q | K | V.  image holds at least the sum of the parts' sizes.  Reads the parts' headers with a
+ * synchronous copy on `stream`. */
+int rl_xenc_concat_qlinear(const void* const* parts, int n_parts, void* image, void* stream);
+/* Debug/test hook: rl_xenc_linear on a quantized image (the launch rl_xenc_encode makes for RL_XENC_IMAGE_QUANT); equal
+ * bit for bit to rl_xenc_linear on rl_xenc_pack_linear of the dequantized weights.  N and K must be the image's. */
+int rl_xenc_linear_q(const void* X, const void* image, const float* bias, void* Y, int T, int N, int K, int act,
+                     void* stream);
 size_t rl_xenc_workspace_bytes(const rl_xenc_weights* w, int T);
 /* Packed variable-length batch: input_ids/type_ids/pos_ids [T], cu_seqlens [P+1]; max_len = longest
  * sequence.  out_logit [P, n_labels] row-major ([P] at one label); out_score [P] is FlashRank's score:

@@ -4,7 +4,8 @@ Drop-in surface (reference ``raglite/__init__.py`` names for this path): ``RAGLi
 ``vector_search``, ``keyword_search``, ``hybrid_search``, ``rerank_chunks``, ``embed_strings``; plus the device-resident ``CorpusIndex`` /
 ``ShardedIndex`` that replace the database for this path and the batched ``vector_search_batch`` /
 ``keyword_search_batch``; and
-``TokenEmbedderEngine``, the embedding model's encoder on the GPU behind ``embed_strings`` / ``embed_queries``; and
+``TokenEmbedderEngine``, the embedding model's encoder on the GPU behind ``embed_strings`` / ``embed_queries`` (from a
+Hugging Face directory or the config's GGUF file, ``register_gguf_embedder``); and
 ``split_sentences`` with ``SaTEngine``, the sentence splitter's SaT model and partition on the GPU; and
 ``split_chunklets`` / ``split_chunks`` / ``split_documents``, the chunklet and chunk partitions on the GPU.
 """
@@ -19,7 +20,7 @@ from ._chunks import (
     split_documents,
 )
 from ._config import RAGLiteConfig
-from ._embed import embed_queries, embed_strings, register_token_embedder
+from ._embed import embed_queries, embed_strings, register_gguf_embedder, register_token_embedder
 from ._index import Chunk, CorpusIndex, get_index, merge_hits, register_index, unregister_index
 from ._query_adapter import update_query_adapter
 from ._search import (
@@ -78,6 +79,7 @@ __all__ = [
     "merge_hits",
     "register_index",
     "reciprocal_rank_fusion",
+    "register_gguf_embedder",
     "register_token_embedder",
     "rerank_chunks",
     "retrieve_chunk_spans",

@@ -34,6 +34,16 @@ def register_token_embedder(embedder: str, model: Any) -> None:
     _TOKEN_EMBEDDERS[embedder] = model
 
 
+def register_gguf_embedder(config: RAGLiteConfig, hub_cache: Any | None = None, **kw: Any) -> Any:
+    """Load the GGUF file ``config.embedder`` names from the Hugging Face hub cache onto the GPU
+    (``TokenEmbedderEngine.from_embedder_string``) and register it for that string; returns the engine."""
+    from ._xenc import TokenEmbedderEngine
+
+    engine = TokenEmbedderEngine.from_embedder_string(config.embedder, hub_cache=hub_cache, **kw)
+    register_token_embedder(config.embedder, engine)
+    return engine
+
+
 def _token_embedder(config: RAGLiteConfig) -> Any:
     if config.embedder in _TOKEN_EMBEDDERS:
         return _TOKEN_EMBEDDERS[config.embedder]

@@ -33,8 +33,11 @@ EXPORTS = [
     "rl_sentence_partition", "rl_chunklet_partition_workspace_bytes", "rl_chunklet_partition",
     "rl_chunk_similarities_workspace_bytes", "rl_chunk_similarities", "rl_chunk_partition_workspace_bytes",
     "rl_chunk_partition", "rl_fts_workspace_bytes", "rl_fts_mark", "rl_fts_stem", "rl_fts_verify", "rl_fts_stem_bytes",
-    "rl_fts_term_keys",
+    "rl_fts_term_keys", "rl_dequant_rows_f16", "rl_xenc_qlinear_image_bytes", "rl_xenc_pack_qlinear",
+    "rl_xenc_concat_qlinear", "rl_xenc_linear_q",
 ]
+RL_XENC_IMAGE_F16 = 0
+RL_XENC_IMAGE_QUANT = 1
 
 
 class ScanParams(C.Structure):
@@ -60,7 +63,8 @@ class ScanStats(C.Structure):
 
 class XencLayer(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in ("qkv_img", "qkv_bias", "o_img", "o_bias", "ln1_g", "ln1_b", "up_img", "up_bias",
-                                           "down_img", "down_bias", "ln2_g", "ln2_b")]
+                                           "down_img", "down_bias", "ln2_g", "ln2_b")] + [
+        (n, C.c_int32) for n in ("qkv_type", "o_type", "up_type", "down_type")]
 
 
 class XencWeights(C.Structure):
@@ -149,15 +153,20 @@ def _declare(lib: C.CDLL) -> None:
     lib.rl_fts_verify.argtypes = [vp, vp, vp, vp, vp, vp, i64, vp, vp]
     lib.rl_fts_stem_bytes.argtypes = [vp, vp, vp, vp, vp, i64, vp, vp, vp]
     lib.rl_fts_term_keys.argtypes = [vp, vp, i64, vp, i64, vp, vp]
+    lib.rl_dequant_rows_f16.argtypes = [i32, vp, i64, i32, vp, vp]
+    lib.rl_xenc_qlinear_image_bytes.argtypes = [i32, i32, i32]
+    lib.rl_xenc_pack_qlinear.argtypes = [i32, vp, i32, i32, vp, vp]
+    lib.rl_xenc_concat_qlinear.argtypes = [C.POINTER(C.c_void_p), i32, vp, vp]
+    lib.rl_xenc_linear_q.argtypes = [vp, vp, vp, vp, i32, i32, i32, i32, vp]
     for name in ("rl_chunklet_partition_workspace_bytes", "rl_chunk_similarities_workspace_bytes",
-                 "rl_chunk_partition_workspace_bytes", "rl_fts_workspace_bytes"):
+                 "rl_chunk_partition_workspace_bytes", "rl_fts_workspace_bytes", "rl_xenc_qlinear_image_bytes"):
         getattr(lib, name).restype = C.c_size_t
     for name in EXPORTS:
         if name not in ("rl_last_error", "rl_maxsim_workspace_bytes", "rl_xenc_linear_image_bytes", "rl_xenc_workspace_bytes",
                         "rl_hits_packed_bytes", "rl_bm25_workspace_bytes", "rl_bm25_packed_bytes",
                         "rl_sat_workspace_bytes", "rl_sentence_partition_workspace_bytes",
                         "rl_chunklet_partition_workspace_bytes", "rl_chunk_similarities_workspace_bytes",
-                        "rl_chunk_partition_workspace_bytes", "rl_fts_workspace_bytes"):
+                        "rl_chunk_partition_workspace_bytes", "rl_fts_workspace_bytes", "rl_xenc_qlinear_image_bytes"):
             getattr(lib, name).restype = C.c_int
 
 

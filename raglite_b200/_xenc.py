@@ -25,6 +25,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from ._gguf import QUANT_TYPES, GGUFTensor, tensor_to_f32
 from ._lib import XencLayer, XencWeights, check
 
 
@@ -100,16 +101,19 @@ class _EncoderEngine:
         self._layers = (XencLayer * n_layers)()
         for l in range(n_layers):
             pre = f"encoder.layer.{l}."
-            qkv_w = torch.cat([sd[pre + f"attention.self.{n}.weight"] for n in ("query", "key", "value")], dim=0)
             qkv_b = torch.cat([sd[pre + f"attention.self.{n}.bias"] for n in ("query", "key", "value")], dim=0)
             qkv_b = qkv_b.detach().to(device=self.device, dtype=torch.float32).contiguous()
             self._keep.append(qkv_b)
             L = self._layers[l]
-            L.qkv_img, L.qkv_bias = self._packed(qkv_w).data_ptr(), qkv_b.data_ptr()
-            L.o_img, L.o_bias = self._packed(sd[pre + "attention.output.dense.weight"]).data_ptr(), self._f32(pre + "attention.output.dense.bias").data_ptr()
+            L.qkv_img, L.qkv_type = self._image([sd[pre + f"attention.self.{n}.weight"] for n in ("query", "key", "value")])
+            L.qkv_bias = qkv_b.data_ptr()
+            L.o_img, L.o_type = self._image([sd[pre + "attention.output.dense.weight"]])
+            L.o_bias = self._f32(pre + "attention.output.dense.bias").data_ptr()
             L.ln1_g, L.ln1_b = self._f32(pre + "attention.output.LayerNorm.weight").data_ptr(), self._f32(pre + "attention.output.LayerNorm.bias").data_ptr()
-            L.up_img, L.up_bias = self._packed(sd[pre + "intermediate.dense.weight"]).data_ptr(), self._f32(pre + "intermediate.dense.bias").data_ptr()
-            L.down_img, L.down_bias = self._packed(sd[pre + "output.dense.weight"]).data_ptr(), self._f32(pre + "output.dense.bias").data_ptr()
+            L.up_img, L.up_type = self._image([sd[pre + "intermediate.dense.weight"]])
+            L.up_bias = self._f32(pre + "intermediate.dense.bias").data_ptr()
+            L.down_img, L.down_type = self._image([sd[pre + "output.dense.weight"]])
+            L.down_bias = self._f32(pre + "output.dense.bias").data_ptr()
             L.ln2_g, L.ln2_b = self._f32(pre + "output.LayerNorm.weight").data_ptr(), self._f32(pre + "output.LayerNorm.bias").data_ptr()
         w = XencWeights()
         w.n_layers, w.hidden, w.n_heads, w.ffn = n_layers, hidden, n_heads, ffn
@@ -132,9 +136,58 @@ class _EncoderEngine:
         return t
 
     def _f16(self, name: str) -> torch.Tensor:
-        t = self._sd[name].detach().to(device=self.device, dtype=torch.float16).contiguous()
+        w = self._sd[name]
+        if isinstance(w, GGUFTensor):   # an embedding table of a GGUF file: quantized ones are dequantized on the device
+            if w.ggml_type not in QUANT_TYPES:
+                w = torch.from_numpy(tensor_to_f32(w))
+            else:
+                blocks = torch.from_numpy(w.data.copy()).to(self.device)
+                t = torch.empty(w.shape, dtype=torch.float16, device=self.device)
+                with torch.cuda.device(self.device):
+                    check(self.lib.rl_dequant_rows_f16(w.ggml_type, blocks.data_ptr(), w.shape[0], w.shape[1], t.data_ptr(),
+                                                       _stream()), "rl_dequant_rows_f16")
+                    torch.cuda.current_stream().synchronize()
+                self._keep.append(t)
+                return t
+        t = w.detach().to(device=self.device, dtype=torch.float16).contiguous()
         self._keep.append(t)
         return t
+
+    def _image(self, parts: list[Any]) -> tuple[int, int]:
+        """The packed image of the row-wise concatenation of ``parts`` (torch float weights, or tensors of a GGUF file)
+        and its ``RL_XENC_IMAGE_*`` type.  Quantized parts stay quantized: one image when they share a type, else one
+        image per part concatenated pass by pass.  Quantized parts were checked by ``_gguf.bert_plan`` before any device
+        work."""
+        quant = [isinstance(p, GGUFTensor) and p.ggml_type in QUANT_TYPES for p in parts]
+        if not any(quant):
+            ws = [torch.from_numpy(tensor_to_f32(p)) if isinstance(p, GGUFTensor) else p for p in parts]
+            return self._packed(torch.cat(ws, dim=0) if len(ws) > 1 else ws[0]).data_ptr(), _lib.RL_XENC_IMAGE_F16
+        K = parts[0].shape[1]   # (bert_plan has checked the parts: all quantized, K % 128 == 0)
+        groups = [list(parts)] if len({p.ggml_type for p in parts}) == 1 else [[p] for p in parts]
+        imgs = []
+        for g in groups:
+            blocks = torch.from_numpy(np.concatenate([p.data for p in g])).to(self.device)
+            N = sum(p.shape[0] for p in g)
+            img = torch.empty(int(self.lib.rl_xenc_qlinear_image_bytes(g[0].ggml_type, N, K)), dtype=torch.uint8,
+                              device=self.device)
+            with torch.cuda.device(self.device):
+                check(self.lib.rl_xenc_pack_qlinear(g[0].ggml_type, blocks.data_ptr(), N, K, img.data_ptr(), _stream()),
+                      "rl_xenc_pack_qlinear")
+                torch.cuda.current_stream().synchronize()
+            imgs.append(img)
+        if len(imgs) > 1:
+            out = torch.empty(sum(i.numel() for i in imgs), dtype=torch.uint8, device=self.device)
+            ptrs = (C.c_void_p * len(imgs))(*[i.data_ptr() for i in imgs])
+            with torch.cuda.device(self.device):
+                check(self.lib.rl_xenc_concat_qlinear(ptrs, len(imgs), out.data_ptr(), _stream()), "rl_xenc_concat_qlinear")
+                torch.cuda.current_stream().synchronize()
+            imgs = [out]
+        self._keep.append(imgs[0])
+        return imgs[0].data_ptr(), _lib.RL_XENC_IMAGE_QUANT
+
+    def weight_bytes(self) -> int:
+        """Device bytes this engine holds for its weights: images, embedding tables, biases and LayerNorms."""
+        return sum(int(t.numel() * t.element_size()) for t in self._keep)
 
     def _packed(self, weight: torch.Tensor) -> torch.Tensor:
         W = weight.detach().to(device=self.device, dtype=torch.float32).contiguous()
@@ -469,6 +522,42 @@ class TokenEmbedderEngine(_EncoderEngine):
         if not (path / "tokenizer.json").exists():
             raise FileNotFoundError(f"No tokenizer.json in {path}")
         return cls.from_hf(model, Tokenizer.from_file(str(path / "tokenizer.json")), n_ctx=n_ctx, **kw)
+
+    @classmethod
+    def from_gguf(cls, path: Path | str, n_ctx: int = 512, tokenizer: Any | None = None, **kw: Any) -> "TokenEmbedderEngine":
+        """Load a llama.cpp GGUF file of a BERT / XLM-RoBERTa embedder (``general.architecture == "bert"``, e.g.
+        lm-kit/bge-m3-gguf) with F32 / F16 / Q8_0 / Q4_K / Q6_K weights.  Quantized linears stay quantized on the device
+        and are expanded inside the linear kernel; embedding tables are dequantized to fp16 once.  The tokenizer is rebuilt
+        from the file's SentencePiece Unigram metadata unless ``tokenizer`` (a ``tokenizers.Tokenizer``, or the path of a
+        ``tokenizer.json``) is given.  ``n_ctx`` 0 means the file's context length; it is capped at 512.  Every check
+        that can fail raises ``ValueError`` before any device work."""
+        from ._gguf import GGUFFile, bert_plan, gguf_tokenizer
+
+        f = GGUFFile(path)
+        plan = bert_plan(f)
+        if tokenizer is None:
+            tokenizer = gguf_tokenizer(f)
+        elif isinstance(tokenizer, (str, Path)):
+            from tokenizers import Tokenizer
+
+            tokenizer = Tokenizer.from_file(str(tokenizer))
+        # 1-D tensors (biases, norms) as float32; 2-D weights stay GGUF tensors for _image / _f16.
+        sd = {k: (torch.from_numpy(tensor_to_f32(t)) if len(t.shape) == 1 else t) for k, t in plan.state_dict.items()}
+        max_pos = sd["embeddings.position_embeddings.weight"].shape[0]
+        # the converter drops XLM-RoBERTa's first pad_token_id + 1 position rows: positions count from 0 here
+        return cls(sd, n_layers=plan.n_layers, hidden=plan.hidden, n_heads=plan.n_heads, ffn=plan.ffn, max_pos=max_pos,
+                   ln_eps=plan.ln_eps, pos_offset=0, tokenizer=tokenizer,
+                   n_ctx=int(n_ctx) if n_ctx else plan.context_length, **kw)
+
+    @classmethod
+    def from_embedder_string(cls, embedder: str, hub_cache: Path | str | None = None, **kw: Any) -> "TokenEmbedderEngine":
+        """The engine behind a RAGLite ``config.embedder`` such as ``llama-cpp-python/lm-kit/bge-m3-gguf/*F16.gguf@512``:
+        the one GGUF file in the Hugging Face hub cache that matches it (``HF_HUB_CACHE``, else ``HF_HOME/hub``, else
+        ``~/.cache/huggingface/hub``).  Nothing is downloaded."""
+        from ._gguf import find_cached_gguf, parse_embedder
+
+        repo_id, filename, n_ctx = parse_embedder(embedder)
+        return cls.from_gguf(find_cached_gguf(repo_id, filename, hub_cache), n_ctx=n_ctx, **kw)
 
     # ---- llama-like protocol -----------------------------------------------------------------------
     def _tokenizer(self) -> EmbedderTokenizer:

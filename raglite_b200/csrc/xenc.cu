@@ -106,6 +106,40 @@ __global__ void pack_linear_kernel(const float* __restrict__ W, int N, int K, __
 // columns past K arrive as zeros) and one bulk copy of the pre-swizzled weight slice into a stage; two consumer
 // warpgroups (64 tokens each) run wgmma.m64n128k16 on it and, after the last slice, add the bias, apply the
 // activation, round to fp16 and stage the tile in shared memory so that it leaves as 16-byte row-contiguous stores.
+// Epilogue of one work item, run by each consumer warpgroup on its 64 tokens: + bias -> activation -> fp16 -> shared
+// staging (columns >= nb belong to no output: skipped) -> 16-byte row-contiguous stores.
+__device__ __forceinline__ void linear_epilogue(const float (&acc)[64], const float* __restrict__ bias, __half* __restrict__ Y,
+                                                int T, int N, int act, int m_tile, int pass, int wg, unsigned char* stg) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, wt = threadIdx.x & 127;
+  const int r_lo = (warp & 3) * 16 + (lane >> 2);   // rows r_lo and r_lo + 8 of this warpgroup's 64
+  const int c_lane = 2 * (lane & 3);
+  const int nb = pass_rows(N, pass);
+  const int n0 = pass * kPassN;
+#pragma unroll
+  for (int c8 = 0; c8 < kPassN / 8; ++c8) {
+    if (8 * c8 >= nb) break;
+    const int c = 8 * c8 + c_lane;
+    const float2 bb = __ldg(reinterpret_cast<const float2*>(bias + n0 + c));
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float x0 = acc[4 * c8 + 2 * h] + bb.x, x1 = acc[4 * c8 + 2 * h + 1] + bb.y;
+      if (act == 1) { x0 = gelu_erf(x0); x1 = gelu_erf(x1); }
+      *reinterpret_cast<uint32_t*>(stg + (uint32_t)(r_lo + 8 * h) * kEpiPitch + (uint32_t)c * 2u) = pack_half2(x0, x1);
+    }
+  }
+  named_bar_sync(2 + wg, 128);
+  const int row_chunks = nb / 8;   // 16-byte chunks per row (nb is a multiple of 32)
+  const int row_base = m_tile * kTileM + wg * 64;
+  for (int idx = wt; idx < 64 * row_chunks; idx += 128) {
+    const int rr = idx / row_chunks, ch = idx - rr * row_chunks;
+    const int grow = row_base + rr;
+    if (grow < T)
+      *reinterpret_cast<uint4*>(Y + (size_t)grow * N + n0 + ch * 8) =
+          *reinterpret_cast<const uint4*>(stg + (uint32_t)rr * kEpiPitch + (uint32_t)ch * 16u);
+  }
+  named_bar_sync(2 + wg, 128);   // the staging buffer is free for the next item
+}
+
 struct LinArgs {
   const __half* img;   // packed weights
   const float* bias;   // [N]
@@ -158,9 +192,7 @@ __global__ void __launch_bounds__(kLinThreads, 1) linear_wgmma_kernel(const __gr
       }
     }
   } else if (warp < kLinConsumerWarps) {
-    const int wg = warp >> 2, wt = threadIdx.x & 127;
-    const int r_lo = (warp & 3) * 16 + (lane >> 2);   // rows r_lo and r_lo + 8 of this warpgroup's 64
-    const int c_lane = 2 * (lane & 3);
+    const int wg = warp >> 2;
     unsigned char* stg = epi + (size_t)wg * 64 * kEpiPitch;
     int stage = 0;
     uint32_t phase = 0;
@@ -168,8 +200,6 @@ __global__ void __launch_bounds__(kLinThreads, 1) linear_wgmma_kernel(const __gr
     for (int64_t it = 0; it < my_items; ++it) {
       const int64_t item = first + it * stride;
       const int m_tile = (int)(item / t.n_pass), pass = (int)(item % t.n_pass);
-      const int nb = pass_rows(t.N, pass);
-      const int n0 = pass * kPassN;
       int prev = -1;
       for (int ks = 0; ks < t.n_ks; ++ks) {
         mbar_wait(&full[stage], phase);
@@ -189,33 +219,344 @@ __global__ void __launch_bounds__(kLinThreads, 1) linear_wgmma_kernel(const __gr
       wgmma_wait<0>();
       __syncwarp();
       if (lane == 0) mbar_arrive(&empty[prev]);
-      // epilogue: + bias -> activation -> fp16 -> shared staging (columns >= nb belong to no output: skipped)
-#pragma unroll
-      for (int c8 = 0; c8 < kPassN / 8; ++c8) {
-        if (8 * c8 >= nb) break;
-        const int c = 8 * c8 + c_lane;
-        const float2 bb = __ldg(reinterpret_cast<const float2*>(t.bias + n0 + c));
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          float x0 = acc[4 * c8 + 2 * h] + bb.x, x1 = acc[4 * c8 + 2 * h + 1] + bb.y;
-          if (t.act == 1) { x0 = gelu_erf(x0); x1 = gelu_erf(x1); }
-          *reinterpret_cast<uint32_t*>(stg + (uint32_t)(r_lo + 8 * h) * kEpiPitch + (uint32_t)c * 2u) = pack_half2(x0, x1);
-        }
-      }
-      named_bar_sync(2 + wg, 128);
-      const int row_chunks = nb / 8;   // 16-byte chunks per row (nb is a multiple of 32)
-      const int row_base = m_tile * kTileM + wg * 64;
-      for (int idx = wt; idx < 64 * row_chunks; idx += 128) {
-        const int rr = idx / row_chunks, ch = idx - rr * row_chunks;
-        const int grow = row_base + rr;
-        if (grow < t.T)
-          *reinterpret_cast<uint4*>(t.Y + (size_t)grow * t.N + n0 + ch * 8) =
-              *reinterpret_cast<const uint4*>(stg + (uint32_t)rr * kEpiPitch + (uint32_t)ch * 16u);
-      }
-      named_bar_sync(2 + wg, 128);   // the staging buffer is free for the next item
+      linear_epilogue(acc, t.bias, t.Y, t.T, t.N, t.act, m_tile, pass, wg, stg);
     }
   }
 }
+// ---- GGUF-quantized weights ------------------------------------------------------------------------------
+// Types by their GGML ids.  A block of K elements of one row: Q8_0 32 elements (fp16 d, 32 int8), Q4_K 256 (fp16 d,
+// fp16 dmin, 12 bytes of 6-bit scales and mins, 128 bytes of nibbles), Q6_K 256 (128 bytes of low nibbles, 64 of high
+// bit pairs, 16 int8 scales, fp16 d).  Every value is ggml's formula in float32, each product and difference rounded on
+// its own (no contraction), then rounded once to fp16 to nearest even:
+//   Q8_0 d q      Q4_K (d sc) q - (dmin m)      Q6_K (d sc) (q - 32)
+constexpr int kGgmlQ8_0 = 8, kGgmlQ4_K = 12, kGgmlQ6_K = 14;
+
+__host__ __device__ inline int q_block_elems(int type) { return type == kGgmlQ8_0 ? 32 : 256; }
+__host__ __device__ inline int q_block_bytes(int type) { return type == kGgmlQ8_0 ? 34 : type == kGgmlQ4_K ? 144 : 210; }
+inline bool q_type_ok(int type) { return type == kGgmlQ8_0 || type == kGgmlQ4_K || type == kGgmlQ6_K; }
+
+// The small integer u (< 2^23) as float without a conversion instruction: its bits under 2^23's exponent, minus 2^23 +
+// `bias`.  Exact, so (float)(u - bias) either way.
+__device__ __forceinline__ float small_int_f(uint32_t u, float bias) {
+  return __fsub_rn(__uint_as_float(0x4B000000u | u), 8388608.f + bias);
+}
+__device__ __forceinline__ float ld_half(const unsigned char* p) {
+  return __half2float(__ushort_as_half(*reinterpret_cast<const unsigned short*>(p)));
+}
+// Q4_K's 6-bit scale and min of sub-block j (ggml's get_scale_min_k4).
+__host__ __device__ inline void q4k_scale_min(int j, const unsigned char* s, int& sc, int& m) {
+  if (j < 4) {
+    sc = s[j] & 63;
+    m = s[j + 4] & 63;
+  } else {
+    sc = (s[j + 4] & 0xF) | ((s[j - 4] >> 6) << 4);
+    m = (s[j + 4] >> 4) | ((s[j] >> 6) << 4);
+  }
+}
+
+// rows x K elements from GGUF blocks (row r's blocks at r * K / block_elems) to fp16: one thread per element.
+__global__ void dequant_rows_kernel(int type, const unsigned char* __restrict__ blocks, int64_t rows, int K,
+                                    __half* __restrict__ out) {
+  const int be = q_block_elems(type), bb = q_block_bytes(type);
+  const int64_t total = rows * K;
+  for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t r = idx / K;
+    const int k = (int)(idx - r * K);
+    const unsigned char* b = blocks + (r * (K / be) + k / be) * bb;
+    const int e = k % be;
+    float y;
+    if (type == kGgmlQ8_0) {
+      y = __fmul_rn(ld_half(b), (float)(int8_t)b[2 + e]);
+    } else if (type == kGgmlQ4_K) {
+      // ggml walks 64 elements at a time: 32 low nibbles (sub-block 2 j64), then the same 32 bytes' high nibbles
+      const int j64 = e / 64, hi = (e % 64) / 32, l = e % 32;
+      int sc, m;
+      q4k_scale_min(2 * j64 + hi, b + 4, sc, m);
+      const int q = (b[16 + 32 * j64 + l] >> (4 * hi)) & 0xF;
+      y = __fsub_rn(__fmul_rn(__fmul_rn(ld_half(b), (float)sc), (float)q), __fmul_rn(ld_half(b + 2), (float)m));
+    } else {
+      // 128 elements at a time (n): four groups g of 32 from ql[64 n ..], qh[32 n ..], scales[8 n ..]
+      const int n = e / 128, g = (e % 128) / 32, l = e % 32;
+      const unsigned char* ql = b + 64 * n;
+      const unsigned char* qh = b + 128 + 32 * n;
+      const int8_t* sc = reinterpret_cast<const int8_t*>(b + 192 + 8 * n);
+      const int q = ((ql[l + 32 * (g & 1)] >> (4 * (g >> 1))) & 0xF) | (((qh[l] >> (2 * g)) & 3) << 4);
+      y = __fmul_rn(__fmul_rn(ld_half(b + 208), (float)sc[l / 16 + 2 * g]), (float)(q - 32));
+    }
+    out[idx] = __float2half_rn(y);
+  }
+}
+
+// ---- quantized weight image ---------------------------------------------------------------------------------
+// Header (QImgHead, then n_pass QImgPass) and, from kQImgData on, per pass and 128-element K slice one run of nb16
+// (the pass's rows rounded up to 16) rows of row_bytes each: one bulk copy per stage.  A row's slice (zero bytes for the
+// padding rows, which decode to +0):
+//   Q8_0  136 B: four fp16 d, then 128 int8
+//   Q4_K   76 B: fp16 d, fp16 dmin, the four 6-bit scales and four mins unpacked to bytes, the 64 nibble bytes of the
+//                half super-block (low nibbles: elements 0-31 and 64-95, high nibbles: 32-63 and 96-127)
+//   Q6_K  108 B: the half super-block's 64 ql bytes, 32 qh bytes, 8 int8 scales, fp16 d, 2 zero bytes
+// That is 1.0, 1.056 and 1.029 times the GGUF bytes.  Each pass carries its own type, so images of tensors of different
+// types concatenate pass by pass (rl_xenc_concat_qlinear).
+constexpr int kQSliceK = 128;                  // K elements per stage: two wgmma slices
+constexpr uint32_t kQMaxRowBytes = 136;
+struct QImgHead { int32_t n_pass, N, K, magic; };
+struct QImgPass { int32_t type, row_bytes; int64_t offset; };   // offset from the image's start
+constexpr int32_t kQImgMagic = 0x51494d47;     // "QIMG"
+constexpr size_t kQImgMaxPasses = 64;          // N <= 8192
+constexpr size_t kQImgData = 2048;             // where the passes' rows start (1024-aligned room for the header)
+static_assert(sizeof(QImgHead) + kQImgMaxPasses * sizeof(QImgPass) <= kQImgData, "the header must fit before the data");
+
+__host__ __device__ inline uint32_t q_row_bytes(int type) { return type == kGgmlQ8_0 ? 136u : type == kGgmlQ4_K ? 76u : 108u; }
+inline size_t q_pass_bytes(int type, int N, int K, int pass) {
+  const int nb16 = (pass_rows(N, pass) + 15) / 16 * 16;
+  return (size_t)(K / kQSliceK) * nb16 * q_row_bytes(type);
+}
+
+// One thread per (pass, K slice, row): reorders the row's GGUF bytes of that slice into the image.
+__global__ void pack_qlinear_kernel(int type, const unsigned char* __restrict__ blocks, int N, int K, unsigned char* __restrict__ img) {
+  const int n_qs = K / kQSliceK, n_pass = (N + kPassN - 1) / kPassN;
+  const uint32_t rb = q_row_bytes(type);
+  const int be = q_block_elems(type), bb = q_block_bytes(type);
+  const int64_t total = (int64_t)n_pass * n_qs * kPassN;
+  for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
+    const int r = (int)(idx % kPassN);
+    const int s = (int)((idx / kPassN) % n_qs);
+    const int pass = (int)(idx / ((int64_t)kPassN * n_qs));
+    const int nb16 = (pass_rows(N, pass) + 15) / 16 * 16;
+    if (r >= nb16) continue;
+    const int n = pass * kPassN + r;
+    unsigned char* o = img + kQImgData + (size_t)pass * kPassN * n_qs * rb + ((size_t)s * nb16 + r) * rb;
+    if (n >= N) {
+      for (uint32_t i = 0; i < rb; ++i) o[i] = 0;
+      continue;
+    }
+    const unsigned char* row = blocks + (size_t)n * (K / be) * bb;
+    const int k0 = s * kQSliceK;
+    if (type == kGgmlQ8_0) {
+      for (int i = 0; i < 4; ++i) {
+        const unsigned char* b = row + (size_t)(k0 / 32 + i) * bb;
+        o[2 * i] = b[0];
+        o[2 * i + 1] = b[1];
+        for (int l = 0; l < 32; ++l) o[8 + 32 * i + l] = b[2 + l];
+      }
+    } else if (type == kGgmlQ4_K) {
+      const unsigned char* b = row + (size_t)(k0 / 256) * bb;
+      const int h = (k0 / 128) & 1;
+      for (int i = 0; i < 4; ++i) o[i] = b[i];
+      for (int i = 0; i < 4; ++i) {
+        int sc, m;
+        q4k_scale_min(4 * h + i, b + 4, sc, m);
+        o[4 + i] = (unsigned char)sc;
+        o[8 + i] = (unsigned char)m;
+      }
+      for (int i = 0; i < 64; ++i) o[12 + i] = b[16 + 64 * h + i];
+    } else {
+      const unsigned char* b = row + (size_t)(k0 / 256) * bb;
+      const int h = (k0 / 128) & 1;
+      for (int i = 0; i < 64; ++i) o[i] = b[64 * h + i];
+      for (int i = 0; i < 32; ++i) o[64 + i] = b[128 + 32 * h + i];
+      for (int i = 0; i < 8; ++i) o[96 + i] = b[192 + 8 * h + i];
+      o[104] = b[208];
+      o[105] = b[209];
+      o[106] = o[107] = 0;
+    }
+  }
+}
+
+// Four fp16 values from the four bytes of w (each < 2^23 after `bias` is added back), as two half2 words:
+// y_i = mul(scale, byte_i - bias) - sub.
+template <bool SUB>
+__device__ __forceinline__ uint2 dq4(uint32_t w, float bias, float scale, float sub) {
+  float y[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const float q = small_int_f(__byte_perm(w, 0u, 0x4440u + i), bias);
+    y[i] = SUB ? __fsub_rn(__fmul_rn(scale, q), sub) : __fmul_rn(scale, q);
+  }
+  return make_uint2(pack_half2(y[0], y[1]), pack_half2(y[2], y[3]));
+}
+
+// Dequantize one image row's half slice (64 elements: B slice `half` of the stage) into the 128B-swizzled fp16 rows the
+// wgmma reads: chunk c (elements 8c .. 8c + 7) of row r lands at r * 128 + ((c ^ (r & 7)) * 16).
+__device__ __forceinline__ void dequant_row_half(int type, const unsigned char* __restrict__ src, int half, int r,
+                                                 unsigned char* __restrict__ dst) {
+  unsigned char* drow = dst + (uint32_t)r * 128u;
+  auto put = [&](int c, uint2 lo, uint2 hi) {
+    *reinterpret_cast<uint4*>(drow + ((c ^ (r & 7)) << 4)) = make_uint4(lo.x, lo.y, hi.x, hi.y);
+  };
+  if (type == kGgmlQ8_0) {
+    const uint32_t* q = reinterpret_cast<const uint32_t*>(src + 8 + 64 * half);
+#pragma unroll
+    for (int b = 0; b < 2; ++b) {
+      const float d = ld_half(src + 2 * (2 * half + b));
+#pragma unroll
+      for (int c = 0; c < 4; ++c)   // int8 q + 128 = the byte with its top bit flipped
+        put(4 * b + c, dq4<false>(q[8 * b + 2 * c] ^ 0x80808080u, 128.f, d, 0.f),
+            dq4<false>(q[8 * b + 2 * c + 1] ^ 0x80808080u, 128.f, d, 0.f));
+    }
+  } else if (type == kGgmlQ4_K) {
+    const float d = ld_half(src), dmin = ld_half(src + 2);
+    const uint32_t* q = reinterpret_cast<const uint32_t*>(src + 12 + 32 * half);
+#pragma unroll
+    for (int sub = 0; sub < 2; ++sub) {   // low nibbles: sub-block 2 half, high nibbles: 2 half + 1
+      const float d1 = __fmul_rn(d, (float)src[4 + 2 * half + sub]);
+      const float m1 = __fmul_rn(dmin, (float)src[8 + 2 * half + sub]);
+#pragma unroll
+      for (int c = 0; c < 4; ++c)
+        put(4 * sub + c, dq4<true>((q[2 * c] >> (4 * sub)) & 0x0F0F0F0Fu, 0.f, d1, m1),
+            dq4<true>((q[2 * c + 1] >> (4 * sub)) & 0x0F0F0F0Fu, 0.f, d1, m1));
+    }
+  } else {
+    const float d = ld_half(src + 104);
+    const int8_t* sc = reinterpret_cast<const int8_t*>(src + 96);
+    const uint32_t* qh = reinterpret_cast<const uint32_t*>(src + 64);
+#pragma unroll
+    for (int gg = 0; gg < 2; ++gg) {   // group g = 2 half + gg: ql bytes 32 (g & 1) on, nibble g >> 1, qh bits 2 g
+      const int g = 2 * half + gg;
+      const uint32_t* ql = reinterpret_cast<const uint32_t*>(src + 32 * (g & 1));
+#pragma unroll
+      for (int c = 0; c < 4; ++c) {
+        const float ds = __fmul_rn(d, (float)sc[c / 2 + 2 * g]);
+        uint2 v[2];
+#pragma unroll
+        for (int w = 0; w < 2; ++w) {
+          const int i = 2 * c + w;
+          const uint32_t q = ((ql[i] >> (4 * half)) & 0x0F0F0F0Fu) | (((qh[i] >> (2 * g)) & 0x03030303u) << 4);
+          v[w] = dq4<false>(q, 32.f, ds, 0.f);
+        }
+        put(4 * gg + c, v[0], v[1]);
+      }
+    }
+  }
+}
+
+// ---- wgmma linear layer on a quantized image ----------------------------------------------------------------
+// linear_wgmma_kernel's work items, wgmma sequence (slices of 64 in ascending K) and epilogue.  A stage spans 128 K: the
+// producer issues two TMA copies of the activations and one bulk copy of the slice's quantized rows; eight dequantizer
+// warps (a thread per row and 64-element half) expand them into the stage's two swizzled fp16 B tiles, fence them for
+// the async proxy and arrive on the stage's full barrier beside the activations' transaction count.
+constexpr int kDqWarps = 8;
+constexpr int kQLinDqWarp0 = kLinProdWarp + 1;
+constexpr int kQLinThreads = (kLinConsumerWarps + 1 + kDqWarps) * 32;
+constexpr uint32_t kQABytes = 2 * kABytes;                     // two 64-wide activation slices
+constexpr uint32_t kQBBytes = 2 * kPassN * 128u;               // two swizzled fp16 weight slices
+constexpr uint32_t kQRawBytes = kPassN * kQMaxRowBytes;        // quantized rows as they arrive
+constexpr uint32_t kQStageBytes = kQABytes + kQBBytes + kQRawBytes;   // 81 KB, a multiple of 1024
+constexpr int kQMaxStages = 4;
+
+struct QLinArgs {
+  const unsigned char* img;   // quantized image
+  const float* bias;          // [N]
+  __half* Y;                  // [T, N]
+  int T, N, K, act;
+  int n_pass, n_qs, stages;
+};
+
+__global__ void __launch_bounds__(kQLinThreads, 1) linear_q_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const QLinArgs t) {
+  extern __shared__ unsigned char smem_dyn[];
+  unsigned char* base = smem_dyn + ((1024u - (smem_u32(smem_dyn) & 1023u)) & 1023u);
+  uint64_t* full = reinterpret_cast<uint64_t*>(base + (size_t)t.stages * kQStageBytes);
+  uint64_t* raw = full + kQMaxStages;
+  uint64_t* empty = raw + kQMaxStages;
+  unsigned char* epi = reinterpret_cast<unsigned char*>(empty + kQMaxStages);
+  const QImgPass* passes = reinterpret_cast<const QImgPass*>(t.img + sizeof(QImgHead));
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int m_tiles = (t.T + kTileM - 1) / kTileM;
+  const int64_t n_items = (int64_t)m_tiles * t.n_pass;
+  const int64_t first = blockIdx.x, stride = gridDim.x;
+  const int64_t my_items = first < n_items ? (n_items - first + stride - 1) / stride : 0;
+
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < t.stages; ++i) {
+      mbar_init(&full[i], 1 + kDqWarps);         // the producer's expect_tx + one arrival per dequantizer warp
+      mbar_init(&raw[i], 1);
+      mbar_init(&empty[i], kLinConsumerWarps);
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (warp == kLinProdWarp) {
+    if (lane == 0 && my_items > 0) {
+      asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int64_t it = 0; it < my_items; ++it) {
+        const int64_t item = first + it * stride;
+        const int m_tile = (int)(item / t.n_pass), pass = (int)(item % t.n_pass);
+        const QImgPass pp = passes[pass];
+        const uint32_t qbytes = (uint32_t)((pass_rows(t.N, pass) + 15) / 16 * 16) * (uint32_t)pp.row_bytes;
+        const unsigned char* src = t.img + pp.offset;
+        for (int qs = 0; qs < t.n_qs; ++qs) {
+          mbar_wait(&empty[stage], phase ^ 1u);
+          unsigned char* st = base + (size_t)stage * kQStageBytes;
+          mbar_arrive_expect_tx(&full[stage], kQABytes);
+          tma_load_2d(st, &tmA, 2 * qs * kSliceK, m_tile * kTileM, &full[stage]);
+          tma_load_2d(st + kABytes, &tmA, (2 * qs + 1) * kSliceK, m_tile * kTileM, &full[stage]);
+          mbar_arrive_expect_tx(&raw[stage], qbytes);
+          bulk_g2s(st + kQABytes + kQBBytes, src + (size_t)qs * qbytes, qbytes, &raw[stage]);
+          if (++stage == t.stages) { stage = 0; phase ^= 1u; }
+        }
+      }
+    }
+  } else if (warp >= kQLinDqWarp0) {
+    const int dt = threadIdx.x - kQLinDqWarp0 * 32;
+    const int r = dt & (kPassN - 1), half = dt / kPassN;
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int64_t it = 0; it < my_items; ++it) {
+      const int64_t item = first + it * stride;
+      const int pass = (int)(item % t.n_pass);
+      const QImgPass pp = passes[pass];
+      const bool live = r < pass_rows(t.N, pass);   // the rest of the B rows feed no stored column: left stale
+      for (int qs = 0; qs < t.n_qs; ++qs) {
+        mbar_wait(&raw[stage], phase);
+        unsigned char* st = base + (size_t)stage * kQStageBytes;
+        if (live)
+          dequant_row_half(pp.type, st + kQABytes + kQBBytes + (uint32_t)r * (uint32_t)pp.row_bytes, half, r,
+                           st + kQABytes + (uint32_t)half * (kPassN * 128u));
+        fence_proxy_async();   // the generic-proxy stores become visible to the consumers' wgmma
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&full[stage]);
+        if (++stage == t.stages) { stage = 0; phase ^= 1u; }
+      }
+    }
+  } else {
+    const int wg = warp >> 2;
+    unsigned char* stg = epi + (size_t)wg * 64 * kEpiPitch;
+    int stage = 0;
+    uint32_t phase = 0;
+    float acc[64];
+    for (int64_t it = 0; it < my_items; ++it) {
+      const int64_t item = first + it * stride;
+      const int m_tile = (int)(item / t.n_pass), pass = (int)(item % t.n_pass);
+      int prev = -1;
+      for (int qs = 0; qs < t.n_qs; ++qs) {
+        mbar_wait(&full[stage], phase);
+        const uint32_t st_addr = smem_u32(base + (size_t)stage * kQStageBytes);
+        wgmma_fence();
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          wgmma_slice(acc, make_kmajor_sw128_desc(st_addr + (uint32_t)h * kABytes + (uint32_t)wg * (64u * 128u)),
+                      make_kmajor_sw128_desc(st_addr + kQABytes + (uint32_t)h * (kPassN * 128u)), qs > 0 || h > 0);
+        wgmma_commit();
+        if (prev >= 0) {
+          wgmma_wait<1>();
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&empty[prev]);
+        }
+        prev = stage;
+        if (++stage == t.stages) { stage = 0; phase ^= 1u; }
+      }
+      wgmma_wait<0>();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty[prev]);
+      linear_epilogue(acc, t.bias, t.Y, t.T, t.N, t.act, m_tile, pass, wg, stg);
+    }
+  }
+}
+
 // 16-byte asynchronous global -> shared copy (zero-fills when src_bytes == 0).
 __device__ __forceinline__ void cp_async_16(uint32_t dst_smem, const void* src, uint32_t src_bytes) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst_smem), "l"(src), "r"(src_bytes) : "memory");
@@ -851,6 +1192,160 @@ static int launch_linear(const __half* X, const void* img, const float* bias, __
   return RL_OK;
 }
 
+// ---- quantized images: sizes, packing, concatenation, launch ------------------------------------------------------
+static bool qlinear_shape_ok(int type, int N, int K) {
+  return q_type_ok(type) && N > 0 && N % 32 == 0 && (size_t)(N + kPassN - 1) / kPassN <= kQImgMaxPasses && K > 0 &&
+         K % kQSliceK == 0 && K % q_block_elems(type) == 0;
+}
+
+extern "C" size_t rl_xenc_qlinear_image_bytes(int type, int N, int K) {
+  if (!qlinear_shape_ok(type, N, K)) return 0;
+  size_t bytes = kQImgData;
+  for (int p = 0; p < (N + kPassN - 1) / kPassN; ++p) bytes += q_pass_bytes(type, N, K, p);
+  return bytes;
+}
+
+// The header of an image: written from the host (a pageable copy: the stream is synchronised before it starts).
+static int write_qimg_head(void* image, int N, int K, const int* types, cudaStream_t stream) {
+  unsigned char head[kQImgData];
+  memset(head, 0, sizeof(head));
+  const int n_pass = (N + kPassN - 1) / kPassN;
+  QImgHead h{n_pass, N, K, kQImgMagic};
+  memcpy(head, &h, sizeof(h));
+  int64_t off = (int64_t)kQImgData;
+  for (int p = 0; p < n_pass; ++p) {
+    QImgPass pp{types[p], (int32_t)q_row_bytes(types[p]), off};
+    memcpy(head + sizeof(QImgHead) + p * sizeof(QImgPass), &pp, sizeof(pp));
+    off += (int64_t)q_pass_bytes(types[p], N, K, p);
+  }
+  RL_CUDA_CHECK(cudaMemcpyAsync(image, head, kQImgData, cudaMemcpyHostToDevice, stream));
+  return RL_OK;
+}
+
+extern "C" int rl_xenc_pack_qlinear(int type, const void* blocks, int N, int K, void* image, void* stream_) {
+  RL_REQUIRE(blocks && image, RL_EINVAL, "rl_xenc_pack_qlinear: null pointer");
+  RL_REQUIRE(qlinear_shape_ok(type, N, K), RL_EUNSUPPORTED,
+             "rl_xenc_pack_qlinear: type=%d N=%d K=%d unsupported (GGML Q8_0 = 8, Q4_K = 12 or Q6_K = 14; N %% 32 == 0, "
+             "N <= %d, K %% 128 == 0 and a whole number of blocks)", type, N, K, (int)(kQImgMaxPasses * kPassN));
+  cudaStream_t stream = (cudaStream_t)stream_;
+  int types[kQImgMaxPasses];
+  for (auto& ty : types) ty = type;
+  const int rc = write_qimg_head(image, N, K, types, stream);
+  if (rc != RL_OK) return rc;
+  pack_qlinear_kernel<<<1024, 128, 0, stream>>>(type, reinterpret_cast<const unsigned char*>(blocks), N, K,
+                                                reinterpret_cast<unsigned char*>(image));
+  RL_CUDA_CHECK(cudaGetLastError());
+  return RL_OK;
+}
+
+extern "C" int rl_xenc_concat_qlinear(const void* const* parts, int n_parts, void* image, void* stream_) {
+  RL_REQUIRE(parts && image && n_parts > 0, RL_EINVAL, "rl_xenc_concat_qlinear: bad arguments");
+  cudaStream_t stream = (cudaStream_t)stream_;
+  RL_REQUIRE((size_t)n_parts <= kQImgMaxPasses, RL_EUNSUPPORTED, "rl_xenc_concat_qlinear: too many parts");
+  unsigned char head[kQImgData];
+  int types[kQImgMaxPasses];
+  size_t payload[kQImgMaxPasses];
+  int N = 0, K = 0, n_pass = 0;
+  for (int i = 0; i < n_parts; ++i) {
+    RL_REQUIRE(parts[i], RL_EINVAL, "rl_xenc_concat_qlinear: null part");
+    RL_CUDA_CHECK(cudaMemcpyAsync(head, parts[i], kQImgData, cudaMemcpyDeviceToHost, stream));
+    RL_CUDA_CHECK(cudaStreamSynchronize(stream));
+    QImgHead h;
+    memcpy(&h, head, sizeof(h));
+    RL_REQUIRE(h.magic == kQImgMagic && h.n_pass > 0 && (size_t)h.n_pass <= kQImgMaxPasses, RL_EINVAL,
+               "rl_xenc_concat_qlinear: part %d is not a quantized image", i);
+    RL_REQUIRE(i == 0 || h.K == K, RL_EINVAL, "rl_xenc_concat_qlinear: parts differ in K");
+    RL_REQUIRE(i == n_parts - 1 || h.N % kPassN == 0, RL_EUNSUPPORTED,
+               "rl_xenc_concat_qlinear: every part but the last needs N %% %d == 0", kPassN);
+    RL_REQUIRE((size_t)(n_pass + h.n_pass) <= kQImgMaxPasses, RL_EUNSUPPORTED, "rl_xenc_concat_qlinear: N too large");
+    K = h.K;
+    payload[i] = 0;
+    for (int p = 0; p < h.n_pass; ++p) {
+      QImgPass pp;
+      memcpy(&pp, head + sizeof(QImgHead) + p * sizeof(QImgPass), sizeof(pp));
+      types[n_pass + p] = pp.type;
+      payload[i] += q_pass_bytes(pp.type, h.N, K, p);
+    }
+    n_pass += h.n_pass;
+    N += h.N;
+  }
+  const int rc = write_qimg_head(image, N, K, types, stream);
+  if (rc != RL_OK) return rc;
+  size_t off = kQImgData;
+  for (int i = 0; i < n_parts; ++i) {   // each part's passes, header excluded, one after the other
+    RL_CUDA_CHECK(cudaMemcpyAsync(reinterpret_cast<unsigned char*>(image) + off,
+                                  reinterpret_cast<const unsigned char*>(parts[i]) + kQImgData, payload[i],
+                                  cudaMemcpyDeviceToDevice, stream));
+    off += payload[i];
+  }
+  return RL_OK;
+}
+
+static int launch_qlinear(const __half* X, const void* img, const float* bias, __half* Y, int T, int N, int K, int act,
+                          int sm_count, cudaStream_t stream) {
+  EncodeTiledFn enc = encode_tiled_fn();
+  RL_REQUIRE(enc != nullptr, RL_ECUDA, "cuTensorMapEncodeTiled is not available from this driver");
+  RL_REQUIRE((reinterpret_cast<uintptr_t>(X) & 15) == 0 && (reinterpret_cast<uintptr_t>(img) & 15) == 0, RL_EINVAL,
+             "linear: X and the image must be 16-byte aligned");
+  RL_REQUIRE(K % kQSliceK == 0 && (N + kPassN - 1) / kPassN <= (int)kQImgMaxPasses, RL_EUNSUPPORTED,
+             "quantized linear: K %% %d == 0 and N <= %d required", kQSliceK, (int)(kQImgMaxPasses * kPassN));
+  CUtensorMap tm;
+  const cuuint64_t gdim[2] = {(cuuint64_t)K, (cuuint64_t)T};
+  const cuuint64_t gstr[1] = {(cuuint64_t)K * sizeof(__half)};
+  const cuuint32_t box[2] = {(cuuint32_t)kSliceK, (cuuint32_t)kTileM};
+  const cuuint32_t estr[2] = {1, 1};
+  const CUresult r = enc(&tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<__half*>(X), gdim, gstr, box, estr,
+                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  RL_REQUIRE(r == CUDA_SUCCESS, RL_ECUDA, "cuTensorMapEncodeTiled failed (%d) for X[%d, %d]", (int)r, T, K);
+  QLinArgs t;
+  t.img = reinterpret_cast<const unsigned char*>(img); t.bias = bias; t.Y = Y; t.T = T; t.N = N; t.K = K; t.act = act;
+  t.n_pass = (N + kPassN - 1) / kPassN;
+  t.n_qs = K / kQSliceK;
+  const uint32_t tail = 3 * kQMaxStages * 8 + kEpiBytes;   // barriers + epilogue staging
+  int stages = (int)((kSmemBudget - 1024 - tail) / kQStageBytes);
+  if (stages > kQMaxStages) stages = kQMaxStages;
+  t.stages = stages;
+  const size_t smem = (size_t)stages * kQStageBytes + tail + 1024;
+  RL_CUDA_CHECK(cudaFuncSetAttribute(linear_q_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  const int64_t items = (int64_t)((T + kTileM - 1) / kTileM) * t.n_pass;
+  const int grid = (int)(items < sm_count ? items : sm_count);
+  linear_q_wgmma_kernel<<<grid, kQLinThreads, smem, stream>>>(tm, t);
+  RL_CUDA_CHECK(cudaGetLastError());
+  return RL_OK;
+}
+
+// The linear of an encoder layer by its image type: RL_XENC_IMAGE_F16 (rl_xenc_pack_linear) or RL_XENC_IMAGE_QUANT.
+static int launch_linear_typed(int image_type, const __half* X, const void* img, const float* bias, __half* Y, int T, int N,
+                               int K, int act, int sm_count, cudaStream_t stream) {
+  if (image_type == RL_XENC_IMAGE_QUANT) return launch_qlinear(X, img, bias, Y, T, N, K, act, sm_count, stream);
+  return launch_linear(X, img, bias, Y, T, N, K, act, sm_count, stream);
+}
+
+extern "C" int rl_xenc_linear_q(const void* X, const void* image, const float* bias, void* Y, int T, int N, int K, int act,
+                                void* stream) {
+  RL_REQUIRE(X && image && bias && Y && T >= 0, RL_EINVAL, "rl_xenc_linear_q: bad arguments");
+  RL_REQUIRE(N % 32 == 0 && K % kQSliceK == 0, RL_EUNSUPPORTED, "rl_xenc_linear_q: N %% 32 and K %% 128 must be 0");
+  RL_REQUIRE((reinterpret_cast<uintptr_t>(bias) & 15) == 0, RL_EINVAL, "rl_xenc_linear_q: bias must be 16-byte aligned");
+  if (T == 0) return RL_OK;
+  int dev = 0, sms = 132;
+  RL_CUDA_CHECK(cudaGetDevice(&dev));
+  RL_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  return launch_qlinear(reinterpret_cast<const __half*>(X), image, bias, reinterpret_cast<__half*>(Y), T, N, K, act, sms,
+                        (cudaStream_t)stream);
+}
+
+extern "C" int rl_dequant_rows_f16(int type, const void* blocks, int64_t rows, int K, void* out, void* stream) {
+  RL_REQUIRE(blocks && out && rows >= 0, RL_EINVAL, "rl_dequant_rows_f16: bad arguments");
+  RL_REQUIRE(q_type_ok(type) && K > 0 && K % q_block_elems(type) == 0, RL_EUNSUPPORTED,
+             "rl_dequant_rows_f16: type=%d K=%d unsupported (Q8_0 = 8, Q4_K = 12 or Q6_K = 14, whole blocks per row)", type, K);
+  if (rows == 0) return RL_OK;
+  dequant_rows_kernel<<<2048, 256, 0, (cudaStream_t)stream>>>(type, reinterpret_cast<const unsigned char*>(blocks), rows, K,
+                                                              reinterpret_cast<__half*>(out));
+  RL_CUDA_CHECK(cudaGetLastError());
+  return RL_OK;
+}
+
 extern "C" int rl_xenc_linear(const void* X, const void* image, const float* bias, void* Y, int T, int N, int K, int act,
                               void* stream) {
   RL_REQUIRE(X && image && bias && Y && T >= 0, RL_EINVAL, "rl_xenc_linear: bad arguments");
@@ -1000,17 +1495,17 @@ static int encoder_forward(const rl_xenc_weights* w, const int32_t* input_ids, c
   RL_CUDA_CHECK(cudaGetLastError());
   for (int l = 0; l < w->n_layers; ++l) {
     const rl_xenc_layer& L = w->layers[l];
-    rc = launch_linear(hidden, L.qkv_img, L.qkv_bias, qkv, T, 3 * H, H, 0, sms, stream);
+    rc = launch_linear_typed(L.qkv_type, hidden, L.qkv_img, L.qkv_bias, qkv, T, 3 * H, H, 0, sms, stream);
     if (rc != RL_OK) return rc;
     rc = encoder_attention_launch(head_dim, qkv, cu_seqlens, seq_order, P, max_len, H, nh, ctx, stream);
     if (rc != RL_OK) return rc;
-    rc = launch_linear(ctx, L.o_img, L.o_bias, tmp, T, H, H, 0, sms, stream);
+    rc = launch_linear_typed(L.o_type, ctx, L.o_img, L.o_bias, tmp, T, H, H, 0, sms, stream);
     if (rc != RL_OK) return rc;
     launch_add_ln(tmp, hidden, L.ln1_g, L.ln1_b, w->ln_eps, T, H, hidden, stream);
     RL_CUDA_CHECK(cudaGetLastError());
-    rc = launch_linear(hidden, L.up_img, L.up_bias, ffn, T, F, H, 1, sms, stream);
+    rc = launch_linear_typed(L.up_type, hidden, L.up_img, L.up_bias, ffn, T, F, H, 1, sms, stream);
     if (rc != RL_OK) return rc;
-    rc = launch_linear(ffn, L.down_img, L.down_bias, tmp, T, H, F, 0, sms, stream);
+    rc = launch_linear_typed(L.down_type, ffn, L.down_img, L.down_bias, tmp, T, H, F, 0, sms, stream);
     if (rc != RL_OK) return rc;
     if (out_f32 != nullptr && l == w->n_layers - 1) launch_add_ln(tmp, hidden, L.ln2_g, L.ln2_b, w->ln_eps, T, H, out_f32, stream);
     else launch_add_ln(tmp, hidden, L.ln2_g, L.ln2_b, w->ln_eps, T, H, hidden, stream);
