@@ -307,7 +307,8 @@ typedef struct rl_xenc_layer {
   const float* ln2_b;
   /* Image type of each linear (appended: every earlier field keeps its offset; a zero-initialised tail is the fp16
    * images of rl_xenc_pack_linear): RL_XENC_IMAGE_F16 or RL_XENC_IMAGE_QUANT (rl_xenc_pack_qlinear /
-   * rl_xenc_concat_qlinear, K % 128 == 0). */
+   * rl_xenc_concat_qlinear, K % 128 == 0, N <= 8192).  rl_xenc_encode and rl_xenc_score refuse any other type
+   * (RL_EINVAL) and a quantized linear of another shape (RL_EUNSUPPORTED) before any CUDA call. */
   int32_t qkv_type, o_type, up_type, down_type;
 } rl_xenc_layer;
 #define RL_XENC_IMAGE_F16 0

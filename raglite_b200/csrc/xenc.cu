@@ -1325,7 +1325,9 @@ static int launch_linear_typed(int image_type, const __half* X, const void* img,
 extern "C" int rl_xenc_linear_q(const void* X, const void* image, const float* bias, void* Y, int T, int N, int K, int act,
                                 void* stream) {
   RL_REQUIRE(X && image && bias && Y && T >= 0, RL_EINVAL, "rl_xenc_linear_q: bad arguments");
-  RL_REQUIRE(N % 32 == 0 && K % kQSliceK == 0, RL_EUNSUPPORTED, "rl_xenc_linear_q: N %% 32 and K %% 128 must be 0");
+  RL_REQUIRE(N > 0 && N % 32 == 0 && (size_t)(N + kPassN - 1) / kPassN <= kQImgMaxPasses && K > 0 && K % kQSliceK == 0,
+             RL_EUNSUPPORTED, "rl_xenc_linear_q: N=%d K=%d unsupported (N %% 32 == 0, 0 < N <= %d, K %% 128 == 0, K > 0)", N, K,
+             (int)(kQImgMaxPasses * kPassN));
   RL_REQUIRE((reinterpret_cast<uintptr_t>(bias) & 15) == 0, RL_EINVAL, "rl_xenc_linear_q: bias must be 16-byte aligned");
   if (T == 0) return RL_OK;
   int dev = 0, sms = 132;
@@ -1518,6 +1520,28 @@ static int encoder_forward(const rl_xenc_weights* w, const int32_t* input_ids, c
 constexpr int kEncodeMaxHidden = 1024;
 constexpr int kEncodeMaxLen = 512;
 
+// Every layer's image types, checked before the forward's first launch: RL_XENC_IMAGE_F16 or RL_XENC_IMAGE_QUANT, and a
+// quantized linear's shape within launch_qlinear's (K % 128 == 0, N <= 8192).  qkv [3H, H], o [H, H], up [F, H], down [H, F].
+static int check_layer_images(const rl_xenc_weights* w, const char* fn) {
+  const int H = w->hidden, F = w->ffn;
+  for (int l = 0; l < w->n_layers; ++l) {
+    const rl_xenc_layer& L = w->layers[l];
+    const int types[4] = {L.qkv_type, L.o_type, L.up_type, L.down_type};
+    const int Ns[4] = {3 * H, H, F, H}, Ks[4] = {H, H, H, F};
+    static const char* names[4] = {"qkv", "o", "up", "down"};
+    for (int i = 0; i < 4; ++i) {
+      RL_REQUIRE(types[i] == RL_XENC_IMAGE_F16 || types[i] == RL_XENC_IMAGE_QUANT, RL_EINVAL,
+                 "%s: layer %d %s image type %d unsupported (RL_XENC_IMAGE_F16 = 0 or RL_XENC_IMAGE_QUANT = 1)", fn, l,
+                 names[i], types[i]);
+      RL_REQUIRE(types[i] != RL_XENC_IMAGE_QUANT ||
+                     (Ks[i] % kQSliceK == 0 && (size_t)(Ns[i] + kPassN - 1) / kPassN <= kQImgMaxPasses),
+                 RL_EUNSUPPORTED, "%s: layer %d quantized %s linear [%d, %d] unsupported (K %% %d == 0 and N <= %d required)",
+                 fn, l, names[i], Ns[i], Ks[i], kQSliceK, (int)(kQImgMaxPasses * kPassN));
+    }
+  }
+  return RL_OK;
+}
+
 // rl_xenc_score takes the union of two envelopes.  The cross-encoder's own (head_dim 32, H <= 512, max_len up to the
 // position table, bounded by attention2_kernel's shared memory) and the token encoder's (head_dim 32 or 64, H <= 1024,
 // max_len <= 512, at least one layer, as rl_xenc_encode).  Both run encoder_forward; the envelopes differ in checks only.
@@ -1547,6 +1571,8 @@ extern "C" int rl_xenc_score(const rl_xenc_weights* w, const int32_t* input_ids,
   }
   RL_REQUIRE(workspace && workspace_bytes >= rl_xenc_workspace_bytes(w, T), RL_ENOSPACE, "rl_xenc_score: workspace too small");
   RL_REQUIRE(P <= T, RL_EINVAL, "rl_xenc_score: more sequences than tokens");
+  const int lc = check_layer_images(w, "rl_xenc_score");
+  if (lc != RL_OK) return lc;
   int dev = 0, sms = 132;
   RL_CUDA_CHECK(cudaGetDevice(&dev));
   RL_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
@@ -1573,6 +1599,8 @@ extern "C" int rl_xenc_encode(const rl_xenc_weights* w, const int32_t* input_ids
   RL_REQUIRE(P <= T, RL_EINVAL, "rl_xenc_encode: more sequences (%d) than tokens (%d)", P, T);
   RL_REQUIRE(workspace && (reinterpret_cast<uintptr_t>(workspace) & 15) == 0 && workspace_bytes >= rl_xenc_workspace_bytes(w, T),
              RL_ENOSPACE, "rl_xenc_encode: workspace must be 16-byte aligned and hold rl_xenc_workspace_bytes(w, T) bytes");
+  const int lc = check_layer_images(w, "rl_xenc_encode");
+  if (lc != RL_OK) return lc;
   int dev = 0, sms = 132;
   RL_CUDA_CHECK(cudaGetDevice(&dev));
   RL_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));

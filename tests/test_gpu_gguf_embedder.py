@@ -59,7 +59,7 @@ def _run(lib, fn, X, img, bias, N, K, act):  # noqa: ANN001, ANN202
 
 
 SHAPES = [(1, 32, 256), (127, 96, 1024), (128, 1024, 1024), (129, 3072, 1024), (4097, 4096, 1024), (129, 1024, 4096),
-          (4097, 1024, 4096), (1, 4096, 256), (128, 32, 4096), (127, 3072, 256)]
+          (4097, 1024, 4096), (1, 4096, 256), (128, 32, 4096), (127, 3072, 256), (65536, 4096, 1024), (65536, 1024, 4096)]
 
 
 @pytest.mark.parametrize("ty", [Q8_0, Q4_K, Q6_K, "qkv"])
