@@ -284,6 +284,16 @@ int rl_span_collate(const int64_t* ranked, int B, int M, const int32_t* chunk_do
 int rl_segment_mean_pool(const float* X, int64_t ld, int d, const int32_t* row_begin,
                          const int32_t* row_end, int S, int normalize, uint16_t* out, void* stream);
 
+/* ---- Standard embedding type's chunk rows: _insert.py:132-145 -------------------------------------
+ * out[r] = alpha * X[r] + one_minus_alpha * F[chunk(r)] with NumPy's float16 arithmetic: each product and the
+ * sum computed in float32 and rounded to float16 (round to nearest even).  X[n_rows, d] chunklet rows (fp16, row
+ * stride ldx), F[n_chunks, d] full-chunk rows (fp16, dense), chunk_off[n_chunks + 1] the CSR of chunk rows over
+ * [0, n_rows] (chunk(r) = the c with chunk_off[c] <= r < chunk_off[c + 1]), alpha / one_minus_alpha fp16 bit
+ * patterns, out[n_rows, d] fp16 (dense).  d and ldx multiples of 8, X / F / out 16-byte aligned. */
+int rl_chunk_embedding_blend(const uint16_t* X, int64_t ldx, const uint16_t* F, const int64_t* chunk_off,
+                             int64_t n_chunks, int64_t n_rows, int d, uint16_t alpha, uint16_t one_minus_alpha,
+                             uint16_t* out, void* stream);
+
 /* ---- Cross-encoder scoring: _search.py:364-397 (reranker.rank -> FlashRank -> onnxruntime) --------
  * BERT / XLM-RoBERTa cross-encoder forward (ms-marco-MiniLM-L-12-v2 architecture and wider:
  * LayerNorm(word+pos+type) -> n_layers x [self-attention, dense+residual+LN, dense+GELU(erf),

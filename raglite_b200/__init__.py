@@ -7,7 +7,9 @@ Drop-in surface (reference ``raglite/__init__.py`` names for this path): ``RAGLi
 ``TokenEmbedderEngine``, the embedding model's encoder on the GPU behind ``embed_strings`` / ``embed_queries`` (from a
 Hugging Face directory or the config's GGUF file, ``register_gguf_embedder``); and
 ``split_sentences`` with ``SaTEngine``, the sentence splitter's SaT model and partition on the GPU; and
-``split_chunklets`` / ``split_chunks`` / ``split_documents``, the chunklet and chunk partitions on the GPU.
+``split_chunklets`` / ``split_chunks`` / ``split_documents``, the chunklet and chunk partitions on the GPU; and
+``Document`` with ``insert_documents`` / ``delete_documents`` / ``delete_documents_by_metadata``, ingest into the
+registered index on the GPU.
 """
 
 from ._chunks import (
@@ -22,6 +24,7 @@ from ._chunks import (
 from ._config import RAGLiteConfig
 from ._embed import embed_queries, embed_strings, register_gguf_embedder, register_token_embedder
 from ._index import Chunk, CorpusIndex, get_index, merge_hits, register_index, unregister_index
+from ._insert import Document, delete_documents, delete_documents_by_metadata, insert_documents
 from ._query_adapter import update_query_adapter
 from ._search import (
     ChunkSpan,
@@ -55,10 +58,13 @@ __all__ = [
     "Chunk",
     "ChunkSpan",
     "CorpusIndex",
+    "Document",
     "RAGLiteConfig",
     "SaTEngine",
     "TokenEmbedderEngine",
     "collate_spans_device",
+    "delete_documents",
+    "delete_documents_by_metadata",
     "hybrid_search",
     "keyword_search",
     "keyword_search_batch",
@@ -76,6 +82,7 @@ __all__ = [
     "split_chunks_batch",
     "split_documents",
     "get_index",
+    "insert_documents",
     "merge_hits",
     "register_index",
     "reciprocal_rank_fusion",

@@ -23,6 +23,7 @@ from . import _lib
 from ._config import RAGLiteConfig
 from ._embed import (
     _device_path,
+    _mean_pool_device,
     _pool_planned,
     _token_embedder,
     count_tokens,
@@ -220,11 +221,10 @@ def chunk_partition(costs: torch.Tensor, row_off: np.ndarray, sizes: Sequence[np
     return [h_cuts[row_off[i]:row_off[i] + h_cs[i]].tolist() for i in range(D)]
 
 
-def _split_chunks_all(docs_chunklets: Sequence[Sequence[str]], docs_embeddings: Sequence[np.ndarray], max_size: int,
-                      device_rows: tuple[torch.Tensor, np.ndarray] | None = None
+def _split_chunks_all(docs_chunklets: Sequence[Sequence[str]], docs_embeddings: Sequence[np.ndarray], max_size: int
                       ) -> list[tuple[list[str], list[np.ndarray]]]:
     """``split_chunks`` of every document: checks and early exits on the host, one similarity and one partition launch
-    per embedding width for the rest.  ``device_rows`` = (X, row offsets) when the rows already lie on the device."""
+    per embedding width for the rest."""
     _check_max_size(max_size)
     out: list[Any] = []
     todo: list[int] = []
@@ -237,13 +237,10 @@ def _split_chunks_all(docs_chunklets: Sequence[Sequence[str]], docs_embeddings: 
             todo.append(i)
     if not todo:
         return out
-    if device_rows is not None:
-        groups = [todo]
-    else:                                  # one launch per embedding width: each document is its own problem
-        widths = sorted({int(docs_embeddings[i].shape[1]) for i in todo})
-        groups = [[i for i in todo if docs_embeddings[i].shape[1] == w] for w in widths]
-    for group in groups:
-        for i, c in zip(group, _chunk_cuts(docs_chunklets, docs_embeddings, group, max_size, device_rows), strict=True):
+    # one launch per embedding width: each document is its own problem
+    widths = sorted({int(docs_embeddings[i].shape[1]) for i in todo})
+    for group in ([i for i in todo if docs_embeddings[i].shape[1] == w] for w in widths):
+        for i, c in zip(group, _chunk_cuts(docs_chunklets, docs_embeddings, group, max_size, None), strict=True):
             out[i] = (_join_pieces(docs_chunklets[i], c), np.split(docs_embeddings[i], c))
     return out
 
@@ -287,11 +284,16 @@ def _embed_batch_device(docs_strings: Sequence[Sequence[str]], config: RAGLiteCo
                         ) -> tuple[torch.Tensor, np.ndarray]:
     """fp16 ``[sum n_b, d]`` device rows of every document's ``embed_strings`` and the row offsets.  With a
     late-chunking embedder on the device path, every document is planned as ``embed_strings`` plans it and all of their
-    segments run in packed forwards and one pool launch (as ``embed_queries`` does); otherwise document by document."""
+    segments run in packed forwards and one pool launch (as ``embed_queries`` does); the standard embedding type pools
+    every string of every document in one call; a late-chunking embedder off the device path goes document by
+    document."""
     model = _token_embedder(config)
     off = _offsets([len(s) for s in docs_strings])
     dev = torch.device("cuda", torch.cuda.current_device())
-    if not _device_path(model) or embedding_type(config=config) != "late_chunking":
+    if embedding_type(config=config) != "late_chunking":
+        flat = [s for strings in docs_strings for s in strings]
+        return (_mean_pool_device(flat, config) if flat else torch.zeros((0, 1), dtype=torch.float16, device=dev)), off
+    if not _device_path(model):
         mats = [torch.from_numpy(np.asarray(embed_strings(list(s), config=config))).to(dev) for s in docs_strings if s]
         return (torch.cat(mats) if mats else torch.zeros((0, 1), dtype=torch.float16, device=dev)), off
     texts, all_tokens, all_segments = [], [], []
@@ -320,13 +322,19 @@ def embed_strings_batch(docs_strings: Sequence[Sequence[str]], *, config: RAGLit
     return [host[off[b]:off[b + 1]] for b in range(len(docs_strings))]
 
 
-def split_documents(docs: Sequence[str], *, config: RAGLiteConfig | None = None
-                    ) -> list[tuple[list[str], list[np.ndarray]]]:
-    """Steps 1-4 of the reference's ``_create_chunk_records`` for every document: ``split_sentences`` (``max_len`` =
-    ``config.chunk_max_size``), ``split_chunklets``, ``embed_strings`` and ``split_chunks`` (``max_size`` the same).
-    Returns what ``split_chunks`` returns, per document.  Each document is parsed by markdown-it once; the chunklet
-    embeddings stay on the device from the pool to the similarity kernel."""
-    config = config or RAGLiteConfig()
+def _nonzero_norm_rows(X: torch.Tensor) -> np.ndarray:
+    """Per fp16 device row, whether ``np.linalg.norm(row) > 0.0`` as NumPy computes it in float16: a square that rounds
+    to a positive half makes the sum positive, and a NaN anywhere makes it NaN."""
+    sq = X * X
+    return ((sq > 0).any(dim=1) & ~sq.isnan().any(dim=1)).cpu().numpy()
+
+
+def _split_documents_device(docs: Sequence[str], config: RAGLiteConfig
+                            ) -> tuple[list[list[str]], torch.Tensor, np.ndarray, list[list[int]]]:
+    """Steps 1-4 of the reference's ``_create_chunk_records`` for every document, the rows left on the device:
+    ``(chunklets per document, fp16 chunklet rows X [sum n_b, d], per-document row offsets [D + 1], per-document chunk
+    cuts)``, a document's cuts being the chunklet indices that start a chunk, but the first.  Each document is parsed by
+    markdown-it once; ``split_chunks``' checks run in its order, per document."""
     docs = list(docs)
     _token_embedder(config)                       # the embedder's error before any device work
     max_size = int(config.chunk_max_size)
@@ -336,6 +344,31 @@ def split_documents(docs: Sequence[str], *, config: RAGLiteConfig | None = None
     cuts = _chunklet_cuts(sentences, max_size, [parsed[d] for d in docs])
     chunklets = [_join_pieces(s, c) for s, c in zip(sentences, cuts, strict=True)]
     X, off = _embed_batch_device(chunklets, config)
+    nonzero = _nonzero_norm_rows(X)
+    chunk_cuts: list[list[int]] = []
+    todo: list[int] = []
+    for b, c in enumerate(chunklets):
+        size = np.asarray([len(x) for x in c])
+        if not np.all(size <= max_size):
+            raise ValueError(CHUNKLET_TOO_LARGE)
+        if not nonzero[off[b]:off[b + 1]].all():
+            raise ValueError(ZERO_NORM)
+        chunk_cuts.append([])
+        if len(c) > 1 and sum(size) > max_size:
+            todo.append(b)
+    if todo:
+        for b, cut in zip(todo, _chunk_cuts(chunklets, [], todo, max_size, (X, off)), strict=True):
+            chunk_cuts[b] = cut
+    return chunklets, X, off, chunk_cuts
+
+
+def split_documents(docs: Sequence[str], *, config: RAGLiteConfig | None = None
+                    ) -> list[tuple[list[str], list[np.ndarray]]]:
+    """Steps 1-4 of the reference's ``_create_chunk_records`` for every document: ``split_sentences`` (``max_len`` =
+    ``config.chunk_max_size``), ``split_chunklets``, ``embed_strings`` and ``split_chunks`` (``max_size`` the same).
+    Returns what ``split_chunks`` returns, per document.  Each document is parsed by markdown-it once; the chunklet
+    embeddings stay on the device from the pool to the similarity kernel."""
+    chunklets, X, off, cuts = _split_documents_device(docs, config or RAGLiteConfig())
     host = X.cpu().numpy()
-    return _split_chunks_all(chunklets, [host[off[b]:off[b + 1]] for b in range(len(docs))], max_size,
-                             device_rows=(X, off))
+    return [(_join_pieces(c, cut), np.split(host[off[b]:off[b + 1]], cut))
+            for b, (c, cut) in enumerate(zip(chunklets, cuts, strict=True))]

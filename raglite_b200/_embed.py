@@ -186,21 +186,26 @@ def embed_strings_with_late_chunking(sentences: list[str], *, config: RAGLiteCon
     return _pool_planned(model, texts, num_tokens, segments, normalize=config.embedder_normalize).cpu().numpy()
 
 
-def embed_strings_without_late_chunking(strings: list[str], *, config: RAGLiteConfig | None = None) -> FloatMatrix:
-    """Plain per-string mean pool (``_embed.py:144-184``) for llama-like embedders; API embedders
-    (LiteLLM) are outside the accelerated path."""
-    config = config or RAGLiteConfig()
+def _mean_pool_device(strings: Sequence[str], config: RAGLiteConfig) -> torch.Tensor:
+    """fp16 ``[n, d]`` device rows of ``embed_strings_without_late_chunking``: on the device path every string runs in
+    one packed forward and one pool launch (a string's row does not depend on the others in the call)."""
     model = _token_embedder(config)
     if _device_path(model):
         X, offs = model.embed_token_ids(model.token_ids_for_embedding(list(strings)))
-        return segment_mean_pool(X, offs[:-1], offs[1:], normalize=2 if config.embedder_normalize else 0).cpu().numpy()
+        return segment_mean_pool(X, offs[:-1], offs[1:], normalize=2 if config.embedder_normalize else 0)
     outs = []
     for i in range(0, len(strings), 96):  # batch size 96 (_embed.py:173)
         mats = [np.asarray(m, dtype=np.float32) for m in model.embed(list(strings[i : i + 96]))]
         X = torch.from_numpy(np.concatenate(mats, axis=0)).cuda()
         cuts = np.concatenate([[0], np.cumsum([len(m) for m in mats])])
         outs.append(segment_mean_pool(X, cuts[:-1], cuts[1:], normalize=2 if config.embedder_normalize else 0))
-    return torch.cat(outs, dim=0).cpu().numpy()
+    return torch.cat(outs, dim=0)
+
+
+def embed_strings_without_late_chunking(strings: list[str], *, config: RAGLiteConfig | None = None) -> FloatMatrix:
+    """Plain per-string mean pool (``_embed.py:144-184``) for llama-like embedders; API embedders
+    (LiteLLM) are outside the accelerated path."""
+    return _mean_pool_device(strings, config or RAGLiteConfig()).cpu().numpy()
 
 
 def embed_queries(queries: Sequence[str], *, config: RAGLiteConfig | None = None) -> FloatMatrix:

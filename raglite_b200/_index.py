@@ -174,6 +174,7 @@ class CorpusIndex:
             raise ValueError("chunk_ids must have one entry per chunk")
         self.chunks = list(chunks) if chunks is not None else None
         self.chunk_metadata = list(chunk_metadata) if chunk_metadata is not None else None
+        self.documents: dict[str, Any] = {}   # Document records of insert_documents, by id (delete_documents_by_metadata)
         self._alive: torch.Tensor | None = None        # uint8 [n_rows]; None = no tombstones
         self._alive_buf: torch.Tensor | None = None    # capacity buffer behind _alive
         self._bufs: dict[str, torch.Tensor] | None = None  # owned capacity buffers once the index has grown

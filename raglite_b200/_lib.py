@@ -34,7 +34,7 @@ EXPORTS = [
     "rl_chunk_similarities_workspace_bytes", "rl_chunk_similarities", "rl_chunk_partition_workspace_bytes",
     "rl_chunk_partition", "rl_fts_workspace_bytes", "rl_fts_mark", "rl_fts_stem", "rl_fts_verify", "rl_fts_stem_bytes",
     "rl_fts_term_keys", "rl_dequant_rows_f16", "rl_xenc_qlinear_image_bytes", "rl_xenc_pack_qlinear",
-    "rl_xenc_concat_qlinear", "rl_xenc_linear_q",
+    "rl_xenc_concat_qlinear", "rl_xenc_linear_q", "rl_chunk_embedding_blend",
 ]
 RL_XENC_IMAGE_F16 = 0
 RL_XENC_IMAGE_QUANT = 1
@@ -111,6 +111,7 @@ def _declare(lib: C.CDLL) -> None:
     lib.rl_rrf_fuse.argtypes = [vp, vp, i32, i32, i32, C.c_double, i32, vp, vp, vp, vp]
     lib.rl_span_collate.argtypes = [vp, i32, i32, vp, vp, vp, vp, vp, i64, vp, i32, vp, vp, vp, vp, vp, vp, vp]
     lib.rl_segment_mean_pool.argtypes = [vp, i64, i32, vp, vp, i32, i32, vp, vp]
+    lib.rl_chunk_embedding_blend.argtypes = [vp, i64, vp, vp, i64, i64, i32, C.c_uint16, C.c_uint16, vp, vp]
     lib.rl_xenc_linear_image_bytes.argtypes = [i32, i32]
     lib.rl_xenc_linear_image_bytes.restype = C.c_size_t
     lib.rl_xenc_pack_linear.argtypes = [vp, i32, i32, vp, vp]

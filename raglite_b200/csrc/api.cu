@@ -165,7 +165,7 @@ static int device_sm_count(int* out) {
 
 using namespace rl;
 
-extern "C" int rl_version(void) { return 109; }
+extern "C" int rl_version(void) { return 110; }
 extern "C" const char* rl_last_error(void) { return g_err; }
 
 extern "C" int rl_device_info(int* sm_count, int* cc_major, int* cc_minor, size_t* l2_bytes) {

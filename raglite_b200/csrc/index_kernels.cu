@@ -4,6 +4,7 @@
 //   rl_chunk_row_map     -- CSR chunk offsets -> per-row owner
 //   rl_adapter_apply     -- reference _search.py:58-62  (float64 matvec, cast to query dtype)
 //   rl_segment_mean_pool -- reference _embed.py:129-140 / :154-164 (mean pool, L2, fp16)
+//   rl_chunk_embedding_blend -- reference _insert.py:132-145 (α-blend of chunklet and full-chunk rows, fp16)
 #include <cuda_fp16.h>
 
 #include "common.cuh"
@@ -222,6 +223,47 @@ __global__ void __launch_bounds__(256) segment_mean_pool_kernel(const float* __r
   }
 }
 
+// NumPy's float16 a * x (one rounding: the product of two halves is exact in float32).
+__device__ __forceinline__ float blend_term(float a, float x) { return __half2float(__float2half_rn(__fmul_rn(a, x))); }
+
+// One warp per row, grid-stride: the row's chunk by binary search over the CSR, then 8 halves per lane and
+// 16-byte load.  out = fp16(fp16(a x) + fp16(b f)), as NumPy evaluates α * e + (1 - α) * f on float16 rows with
+// weak Python scalars; __fmul_rn / __fadd_rn keep the compiler from contracting the float32 steps into an FMA.
+__global__ void __launch_bounds__(256) chunk_embedding_blend_kernel(const __half* __restrict__ X, int64_t ldx,
+                                                                    const __half* __restrict__ F,
+                                                                    const int64_t* __restrict__ chunk_off,
+                                                                    int64_t n_chunks, int64_t n_rows, int d,
+                                                                    float a, float b, __half* __restrict__ out) {
+  const int lane = threadIdx.x & 31;
+  const int64_t warp = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int64_t n_warps = (int64_t)gridDim.x * (blockDim.x >> 5);
+  for (int64_t r = warp; r < n_rows; r += n_warps) {
+    int64_t lo = 0, hi = n_chunks;  // chunk_off[lo] <= r < chunk_off[hi]
+    while (hi - lo > 1) {
+      const int64_t mid = (lo + hi) >> 1;
+      if (__ldg(chunk_off + mid) <= r) lo = mid;
+      else hi = mid;
+    }
+    const __half* x = X + r * ldx;
+    const __half* f = F + lo * d;
+    __half* o = out + r * d;
+    for (int c = lane * 8; c < d; c += 256) {
+      const uint4 xv = __ldg(reinterpret_cast<const uint4*>(x + c));
+      const uint4 fv = __ldg(reinterpret_cast<const uint4*>(f + c));
+      const __half2* xh = reinterpret_cast<const __half2*>(&xv);
+      const __half2* fh = reinterpret_cast<const __half2*>(&fv);
+      uint4 ov;
+      __half2* oh = reinterpret_cast<__half2*>(&ov);
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const float2 xf = __half22float2(xh[e]), ff = __half22float2(fh[e]);
+        oh[e] = __halves2half2(__float2half_rn(__fadd_rn(blend_term(a, xf.x), blend_term(b, ff.x))),
+                               __float2half_rn(__fadd_rn(blend_term(a, xf.y), blend_term(b, ff.y))));
+      }
+      *reinterpret_cast<uint4*>(o + c) = ov;
+    }
+  }
+}
 
 // out[row] = chunk_ok[row_chunk[row]] (all-ones when chunk_ok is null) AND alive[row] (when given): the
 // per-row byte mask the scan epilogue reads.  chunk_ok is the metadata filter resolved per chunk
@@ -327,6 +369,26 @@ extern "C" int rl_segment_mean_pool(const float* X, int64_t ld, int d, const int
   RL_CUDA_CHECK(cudaFuncSetAttribute(segment_mean_pool_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   segment_mean_pool_kernel<<<S, 256, smem, (cudaStream_t)stream>>>(X, ld, d, row_begin, row_end, normalize,
                                                                      reinterpret_cast<__half*>(out));
+  RL_CUDA_CHECK(cudaGetLastError());
+  return RL_OK;
+}
+
+extern "C" int rl_chunk_embedding_blend(const uint16_t* X, int64_t ldx, const uint16_t* F, const int64_t* chunk_off,
+                                        int64_t n_chunks, int64_t n_rows, int d, uint16_t alpha,
+                                        uint16_t one_minus_alpha, uint16_t* out, void* stream) {
+  RL_REQUIRE(n_rows >= 0 && n_chunks >= 0 && d > 0 && ldx >= d && (n_rows == 0 || n_chunks > 0), RL_EINVAL,
+             "rl_chunk_embedding_blend: bad shape");
+  RL_REQUIRE(d % 8 == 0 && ldx % 8 == 0 && ((reinterpret_cast<uintptr_t>(X) | reinterpret_cast<uintptr_t>(F) |
+                                             reinterpret_cast<uintptr_t>(out)) & 15) == 0,
+             RL_EUNSUPPORTED, "rl_chunk_embedding_blend: d and ldx must be multiples of 8 and X, F, out 16-byte aligned");
+  if (n_rows == 0) return RL_OK;
+  RL_REQUIRE(X && F && chunk_off && out, RL_EINVAL, "rl_chunk_embedding_blend: null pointer");
+  const __half_raw ra{alpha}, rb{one_minus_alpha};
+  const int64_t blocks = (n_rows + 7) / 8;
+  const int grid = (int)(blocks < 132 * 16 ? blocks : 132 * 16);
+  chunk_embedding_blend_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(
+      reinterpret_cast<const __half*>(X), ldx, reinterpret_cast<const __half*>(F), chunk_off, n_chunks, n_rows, d,
+      __half2float(__half(ra)), __half2float(__half(rb)), reinterpret_cast<__half*>(out));
   RL_CUDA_CHECK(cudaGetLastError());
   return RL_OK;
 }
