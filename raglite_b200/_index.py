@@ -65,6 +65,40 @@ def csr_from_row_chunk_ids(ids: Sequence[ChunkId], known: set[ChunkId] | None = 
     return np.asarray(offsets, dtype=np.int64), chunk_ids
 
 
+def stats_unit_scale(stats: np.ndarray) -> bool:
+    """The gate of the fp16 scan's unscaled fast path on ``rl_row_stats`` statistics ``{max |e|, max |x|, max 1/|e|,
+    zero row}``: every row has 1/|e| <= 2 (norm >= 0.5), no value exceeds 1024 and no row is zero."""
+    return bool(0.0 < stats[2] <= 2.0 and stats[1] <= 1024.0 and stats[3] == 0.0)
+
+
+def fp16_rows_unit_scale(h: np.ndarray) -> bool:
+    """``stats_unit_scale`` of float16 rows ``h [n, d]`` as ``rl_row_stats_f16`` computes the statistics: per row the
+    float64 sum of squares s, then float32(1 / sqrt(s)).  The float64 sum is the kernel's in any order wherever the gate
+    can go either way: float16 squares are multiples of 2^-48, so a sum below 16 holds every partial sum exactly, and
+    a larger one gives 1/sqrt(s) < 0.25."""
+    if h.size == 0:
+        return False
+    h64 = h.astype(np.float64)
+    s = np.einsum("ij,ij->i", h64, h64)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        inv = (1.0 / np.sqrt(s)).astype(np.float32)
+    return bool((s > 0).all() and (inv <= 2.0).all() and np.abs(h).max() <= 1024)
+
+
+def fp16_rows_unit_scale_device(X: torch.Tensor) -> bool:
+    """``stats_unit_scale`` of contiguous float16 device rows ``X [n, d]`` (d % 8 == 0), from ``rl_row_stats_f16``
+    itself.  Synchronises."""
+    n, d = int(X.shape[0]), int(X.shape[1])
+    if n == 0:
+        return False
+    dev = X.device
+    inv, sq = torch.empty(n, dtype=torch.float32, device=dev), torch.empty(n, dtype=torch.float32, device=dev)
+    st = torch.zeros(4, dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        check(_lib.load().rl_row_stats_f16(_ptr(X), n, d, d, _ptr(inv), _ptr(sq), _ptr(st), _stream()), "rl_row_stats_f16")
+    return stats_unit_scale(st.cpu().numpy())
+
+
 @dataclass
 class Chunk:
     """Minimal stand-in for ``raglite._database.Chunk`` (``_database.py:196-324``): what
@@ -254,11 +288,7 @@ class CorpusIndex:
             return E, storage
         d = int(E.shape[1]) if E.ndim == 2 else 0
         h = _rows.lossless_float16(E) if d % 8 == 0 and E.size else None
-        if h is None:
-            return E.astype(np.float32, copy=False), "fp32"
-        # the cosine fast path of the float16 layout needs rows that are not tiny (norm >= 0.5)
-        nrm = np.linalg.norm(h.astype(np.float32), axis=1)
-        if nrm.size and (nrm.min() < 0.5 or np.abs(h).max() > 1024):
+        if h is None or not fp16_rows_unit_scale(h):   # the cosine fast path of the float16 layout needs unit-scale rows
             return E.astype(np.float32, copy=False), "fp32"
         return h, "fp16"
 
@@ -268,13 +298,20 @@ class CorpusIndex:
         anything else must stay float32."""
         if self.storage == "fp32":
             return E.to(device=self.device, dtype=torch.float32).contiguous()
+        Eh = self._lossless_fp16(E)
+        if Eh is None:
+            raise ValueError("storage='fp16' needs embeddings that are exactly representable in float16")
+        return Eh
+
+    def _lossless_fp16(self, E: torch.Tensor) -> torch.Tensor | None:
+        """``E`` as float16 rows on the device, or None when a value is not exactly representable in float16."""
         Eh = E.to(device=self.device, dtype=torch.float16).contiguous()
         if E.dtype != torch.float16:
             step = 1 << 20
             for r0 in range(0, int(E.shape[0]), step):
                 blk = E[r0:r0 + step].to(self.device, dtype=torch.float32)
                 if not torch.equal(Eh[r0:r0 + step].float(), blk):
-                    raise ValueError("storage='fp16' needs embeddings that are exactly representable in float16")
+                    return None
         return Eh
 
     # ---- mutation: the index follows the chunk_embedding table --------------------------------------
@@ -298,12 +335,20 @@ class CorpusIndex:
         """Host copy of the decision the scan otherwise takes on the device: can rows enter the fp16 tensor-core
         scan unscaled (norms >= 0.5, |x| <= 1024, no zero row -- normalised embeddings)?  Read once per index
         change (build / append / compact synchronise anyway), passed as ``rl_scan_params.rows_unit_scale``."""
-        self._rows_unit_scale = False
-        if self.n_rows:
-            st = self.stats.cpu().numpy()
-            self._rows_unit_scale = bool(0.0 < st[2] <= 2.0 and st[1] <= 1024.0 and st[3] == 0.0)
+        self._rows_unit_scale = bool(self.n_rows) and stats_unit_scale(self.stats.cpu().numpy())
         if self.storage == "fp16":   # an empty shard holds no row too small for the cosine fast path
             self._fp16_cosine_ok = self._rows_unit_scale or self.n_rows == 0
+
+    def _widen_to_fp32(self) -> None:
+        """Move the rows to float32 storage (same values; the capacity buffer keeps its size).  ``append`` does this
+        before it adds rows that the float16 layout cannot hold losslessly, or that would take its cosine fast path
+        away: a search never starts failing because of an earlier append.  The row statistics stay valid."""
+        cap = int(self._bufs["E"].shape[0]) if self._bufs is not None else self.n_rows
+        E32 = torch.empty((cap, self.d), dtype=torch.float32, device=self.device)
+        E32[: self.n_rows] = self.E
+        if self._bufs is not None:
+            self._bufs["E"] = E32
+        self.E, self.storage = E32[: self.n_rows], "fp32"
 
     @property
     def rows_unit_scale(self) -> bool:
@@ -340,7 +385,9 @@ class CorpusIndex:
     ) -> None:
         """Append whole chunks (rows of a chunk contiguous) behind the resident rows: one flush of
         ``insert_documents`` (``_insert.py:247-255``).  Only the new rows are read: their norms are
-        computed by ``rl_row_stats``, which folds their maxima into the shard statistics."""
+        computed by ``rl_row_stats``, which folds their maxima into the shard statistics.  A float16 index moves to
+        float32 storage first when a new row is not exactly representable in float16, or when the index passes the
+        cosine fast path's gate (``fp16_rows_unit_scale``) and a new row does not."""
         E = torch.as_tensor(embeddings)
         if E.ndim != 2 or int(E.shape[1]) != self.d:
             raise ValueError(f"embeddings must be [n_rows, {self.d}]")
@@ -373,7 +420,12 @@ class CorpusIndex:
             self._shard_guard.check_local_growth(self.n_chunks + c_new)
         with self._lock, torch.cuda.device(self.device):
             self._invalidate_filters()
-            rows = self._to_storage(E)
+            rows = self._lossless_fp16(E) if self.storage == "fp16" else None
+            if self.storage == "fp16" and (rows is None or (self._fp16_cosine_ok and not fp16_rows_unit_scale_device(rows))):
+                self._widen_to_fp32()
+                rows = None
+            if rows is None:
+                rows = self._to_storage(E)
             n0 = self.n_rows
             self._reserve(n0 + m)
             for name in self._ROW_ARRAYS:

@@ -30,7 +30,7 @@ from . import _lib
 from ._chunks import _join_pieces, _offsets, _parse, _split_documents_device
 from ._config import RAGLiteConfig
 from ._embed import _mean_pool_device, _token_embedder, embedding_type
-from ._index import Chunk, CorpusIndex, get_index, register_index
+from ._index import Chunk, CorpusIndex, fp16_rows_unit_scale_device, get_index, register_index
 from ._lib import check
 from ._typing import DocumentId
 
@@ -269,12 +269,12 @@ def insert_documents(documents: list[Document], *, max_workers: int | None = Non
 
 
 def _auto_storage(X: torch.Tensor) -> str:
-    """``CorpusIndex._pick_storage(rows, "auto")`` for fp16 device rows: float16 unless d % 8 != 0, a row's norm is
-    below 0.5 or a value's magnitude above 1024."""
+    """``CorpusIndex._pick_storage(rows, "auto")`` for fp16 device rows: float16 unless d % 8 != 0 or the rows fail
+    the fp16 cosine fast path's gate as ``rl_row_stats_f16`` decides it (a zero row, a norm below 0.5, a value's
+    magnitude above 1024)."""
     if X.shape[1] % 8 or X.numel() == 0:
         return "fp32"
-    small = torch.linalg.vector_norm(X.float(), dim=1).min() < 0.5
-    return "fp32" if bool(small | (X.abs().max() > 1024)) else "fp16"
+    return "fp16" if fp16_rows_unit_scale_device(X.contiguous()) else "fp32"
 
 
 def delete_documents(document_ids: list[DocumentId], *, config: RAGLiteConfig | None = None,
