@@ -586,6 +586,66 @@ int rl_fts_stem_bytes(const uint8_t* letters, const int64_t* word_off, const int
 int rl_fts_term_keys(const int64_t* tok_stem, const int64_t* owner, int64_t n, const int32_t* stem_term,
                      int64_t chunk_base, int64_t* key, void* stream);
 
+/* ---- decoder-only LLM (llama.cpp's "qwen3" architecture): prefill, KV-cached decode and sampling -------------------
+ * Weights are quantized images (rl_xenc_pack_qlinear).  A linear of N > RL_LLM_PART_ROWS rows is held as parts of
+ * RL_LLM_PART_ROWS rows (the last one shorter): part i holds rows [RL_LLM_PART_ROWS i, ...).  head_dim is 128; the
+ * query heads n_head are a multiple of the KV heads n_kv with a group n_head / n_kv <= RL_LLM_MAX_GROUP; query head h
+ * reads KV head h / group.  The KV cache is one fp16 array per K and V, [n_layers][n_ctx][n_kv][128].
+ * Numerics: residual stream fp32; every linear's input and output fp16 (fp32 accumulation); RMSNorm, QK-norm, RoPE,
+ * softmax and SwiGLU in fp32.  Nothing reduces through atomics: every output is the same run to run. */
+#define RL_LLM_HEAD_DIM 128
+#define RL_LLM_MAX_GROUP 8
+#define RL_LLM_PART_ROWS 8192
+#define RL_LLM_MAX_PARTS 32
+#define RL_LLM_MAX_TOP_K 256
+typedef struct rl_llm_linear {
+  const void* parts[RL_LLM_MAX_PARTS]; /* device images; part i has min(RL_LLM_PART_ROWS, N - RL_LLM_PART_ROWS i) rows */
+  int32_t n_parts, N, K;
+} rl_llm_linear;
+typedef struct rl_llm_layer {
+  rl_llm_linear q, k, v, o, gate, up, down;
+  const float *attn_norm, *q_norm, *k_norm, *ffn_norm; /* device fp32 [hidden], [128], [128], [hidden] */
+} rl_llm_layer;
+typedef struct rl_llm_weights {
+  int32_t n_layers, hidden, n_head, n_kv, ffn, vocab, n_ctx;
+  float eps, rope_base;
+  rl_llm_linear token_embd; /* [vocab, hidden] */
+  rl_llm_linear output;     /* [vocab, hidden]; a copy of token_embd when the file ties them */
+  const float* output_norm;
+  const rl_llm_layer* layers; /* HOST array of n_layers entries */
+} rl_llm_weights;
+size_t rl_llm_workspace_bytes(const rl_llm_weights* w, int T_max);
+/* One forward step of T tokens (ids: device int32 [T]) at positions p0 .. p0 + T - 1: their K / V enter the cache
+ * and logits (device fp32 [vocab]) get the last row's.  T == 1 runs every linear as a GEMV; T > 1 runs the wgmma
+ * linear.  Needs 1 <= T <= T_max of the workspace and p0 + T <= n_ctx. */
+int rl_llm_forward(const rl_llm_weights* w, const int32_t* ids, int T, int p0, void* k_cache, void* v_cache,
+                   float* logits, void* workspace, size_t workspace_bytes, void* stream);
+/* Test and measurement hooks of the forward's steps. */
+size_t rl_llm_qgemv_workspace_bytes(int N, int K);
+/* y[n] = sum_k W[n, k] x[k] over the image values of W (x fp16 [K]; y fp32 when y_f32, else fp16), fp32 partial sums
+ * over K slices reduced in a fixed order. */
+int rl_llm_qgemv(const rl_llm_linear* w, const void* x, void* y, int y_f32, void* workspace, size_t workspace_bytes,
+                 void* stream);
+/* out[t] (fp32 [T, K]) = the element values of rows ids[t] of the image linear (ggml's formulas, not rounded). */
+int rl_llm_embed(const rl_llm_linear* table, const int32_t* ids, int T, float* out, void* stream);
+/* qkv fp16 [T, (n_head + 2 n_kv) 128] -> q_out fp16 [T, n_head, 128] (RMSNorm per head with q_norm, then NEOX RoPE at
+ * position p0 + t), k_cache[p0 + t] (the same with k_norm) and v_cache[p0 + t] (copied); caches [n_ctx][n_kv][128]. */
+int rl_llm_qk_norm_rope(const void* qkv, int T, int p0, int n_head, int n_kv, const float* q_norm, const float* k_norm,
+                        float eps, float rope_base, int n_ctx, void* q_out, void* k_cache, void* v_cache, void* stream);
+/* Causal attention of q fp16 [T, n_head, 128] (positions p0 + t) over cache rows 0 .. p0 + t -> out fp16
+ * [T, n_head 128].  splits: 0 chooses; s > 0 cuts the keys into s ranges combined in order. */
+size_t rl_llm_attention_workspace_bytes(int T, int n_head, int n_kv, int n_keys, int splits);
+int rl_llm_attention(const void* q, const void* k_cache, const void* v_cache, int T, int p0, int n_head, int n_kv,
+                     int splits, void* out, void* workspace, size_t workspace_bytes, void* stream);
+/* One token from fp32 logits [V] (device): repeat penalty over hist (device int32 [n_hist], the distinct ids only),
+ * then temperature == 0: argmax (lowest id on ties); else top-k (1 <= top_k <= RL_LLM_MAX_TOP_K), top-p (min_keep 1),
+ * min-p, temperature, and the inverse CDF at u in [0, 1) over the candidates by descending logit, ties by ascending
+ * id.  out_id: device int32 [1]. */
+size_t rl_llm_sample_workspace_bytes(int V);
+int rl_llm_sample(const float* logits, int V, const int32_t* hist, int n_hist, float temperature, int top_k, float top_p,
+                  float min_p, float repeat_penalty, float u, int32_t* out_id, void* workspace, size_t workspace_bytes,
+                  void* stream);
+
 #ifdef __cplusplus
 }
 #endif

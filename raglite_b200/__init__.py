@@ -9,7 +9,8 @@ Hugging Face directory or the config's GGUF file, ``register_gguf_embedder``); a
 ``split_sentences`` with ``SaTEngine``, the sentence splitter's SaT model and partition on the GPU; and
 ``split_chunklets`` / ``split_chunks`` / ``split_documents``, the chunklet and chunk partitions on the GPU; and
 ``Document`` with ``insert_documents`` / ``delete_documents`` / ``delete_documents_by_metadata``, ingest into the
-registered index on the GPU.
+registered index on the GPU; and
+``LlmEngine`` with ``rag`` / ``add_context`` / ``retrieve_context``, generation with the config's Qwen3 GGUF on the GPU.
 """
 
 from ._chunks import (
@@ -25,7 +26,9 @@ from ._config import RAGLiteConfig
 from ._embed import embed_queries, embed_strings, register_gguf_embedder, register_token_embedder
 from ._index import Chunk, CorpusIndex, get_index, merge_hits, register_index, unregister_index
 from ._insert import Document, delete_documents, delete_documents_by_metadata, insert_documents
+from ._llm import LlmEngine, register_gguf_llm, register_llm
 from ._query_adapter import update_query_adapter
+from ._rag import RAG_INSTRUCTION_TEMPLATE, add_context, get_context_size, rag, retrieve_context
 from ._search import (
     ChunkSpan,
     collate_spans_device,
@@ -55,7 +58,15 @@ from ._sentences import (
 from ._xenc import TokenEmbedderEngine
 
 __all__ = [
+    "RAG_INSTRUCTION_TEMPLATE",
     "Chunk",
+    "LlmEngine",
+    "add_context",
+    "get_context_size",
+    "rag",
+    "register_gguf_llm",
+    "register_llm",
+    "retrieve_context",
     "ChunkSpan",
     "CorpusIndex",
     "Document",

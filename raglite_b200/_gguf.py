@@ -333,3 +333,89 @@ def find_cached_gguf(repo_id: str, filename: str, hub_cache: Path | str | None =
         raise FileNotFoundError(f"{what} matching {filename!r} in {snaps}/*/ (candidates: {cands}); download the GGUF "
                                 "file with llama-cpp-python or huggingface_hub first")
     return next(iter(distinct.values()))
+
+
+# ---- Qwen3 decoders (llama.cpp's "qwen3" architecture) ------------------------------------------------------------------
+# Tensor names as llama.cpp's converter writes them for Qwen3 (recalled, not checked against a downloaded file): Q and K
+# unpermuted (the NEOX rotation over pairs (i, i + 64) applies), QK-norm an RMSNorm over each head's 128 values.
+_QWEN3_BLOCK = ("attn_norm", "attn_q", "attn_k", "attn_v", "attn_q_norm", "attn_k_norm", "attn_output", "ffn_norm",
+                "ffn_gate", "ffn_up", "ffn_down")
+QWEN3_HEAD_DIM = 128
+QWEN3_MAX_GROUP = 8
+
+
+@dataclass(frozen=True)
+class Qwen3Plan:
+    n_layers: int
+    hidden: int
+    n_head: int
+    n_kv: int
+    ffn: int
+    vocab: int
+    context_length: int
+    rope_base: float
+    eps: float
+    tensors: dict[str, GGUFTensor]   # GGUF name -> tensor; "output.weight" is token_embd's when the file ties them
+    tied: bool
+
+
+def qwen3_plan(f: GGUFFile) -> Qwen3Plan:
+    """Check a GGUF file against what the decoder runs (head_dim 128, GQA group <= 8, hidden and ffn multiples of 256,
+    2-D weights Q8_0 / Q4_K / Q6_K, norms F32) and collect its tensors.  Raises ``ValueError`` (nothing touches a
+    device)."""
+    arch = f.get("general.architecture")
+    if arch != "qwen3":
+        raise ValueError(f"{f.path}: general.architecture={arch!r} unsupported: the decoder loads 'qwen3'")
+
+    def key(k: str) -> Any:
+        v = f.get(f"qwen3.{k}")
+        if v is None:
+            raise ValueError(f"{f.path}: metadata key qwen3.{k} is missing")
+        return v
+
+    n_layers, ctx, hidden = int(key("block_count")), int(key("context_length")), int(key("embedding_length"))
+    ffn, n_head, n_kv = int(key("feed_forward_length")), int(key("attention.head_count")), int(key("attention.head_count_kv"))
+    k_len, v_len = int(key("attention.key_length")), int(key("attention.value_length"))
+    rope_base, eps = float(key("rope.freq_base")), float(key("attention.layer_norm_rms_epsilon"))
+    if k_len != QWEN3_HEAD_DIM or v_len != QWEN3_HEAD_DIM:
+        raise ValueError(f"{f.path}: head_dim {k_len} / {v_len} unsupported (key_length = value_length = 128)")
+    if n_head <= 0 or n_kv <= 0 or n_head % n_kv or n_head // n_kv > QWEN3_MAX_GROUP:
+        raise ValueError(f"{f.path}: head_count={n_head} head_count_kv={n_kv} unsupported (head_count a multiple of "
+                         f"head_count_kv, group <= {QWEN3_MAX_GROUP})")
+    if hidden <= 0 or hidden % 256 or ffn <= 0 or ffn % 256 or n_layers < 1:
+        raise ValueError(f"{f.path}: hidden={hidden} ffn={ffn} layers={n_layers} unsupported (hidden and ffn multiples "
+                         "of 256, at least one layer)")
+
+    def tensor(name: str, shape: tuple[int, ...]) -> GGUFTensor:
+        t = f.tensors.get(name)
+        if t is None:
+            raise ValueError(f"{f.path}: tensor {name!r} is missing")
+        if t.shape != shape:
+            raise ValueError(f"{f.path}: tensor {name!r} has shape {list(t.shape)}, expected {list(shape)}")
+        if len(shape) == 1 and t.ggml_type != F32:
+            raise ValueError(f"{f.path}: norm {name!r} is {t.type_name}; norms must be F32")
+        if len(shape) == 2 and t.ggml_type not in QUANT_TYPES:
+            raise ValueError(f"{f.path}: tensor {name!r} is {t.type_name}; 2-D weights must be Q8_0, Q4_K or Q6_K")
+        return t
+
+    emb = f.tensors.get("token_embd.weight")
+    if emb is None:
+        raise ValueError(f"{f.path}: tensor 'token_embd.weight' is missing")
+    vocab = emb.shape[0]
+    if vocab % 32:
+        raise ValueError(f"{f.path}: token_embd has {vocab} rows; the quantized image needs a multiple of 32")
+    nq, nkv = n_head * QWEN3_HEAD_DIM, n_kv * QWEN3_HEAD_DIM
+    ts = {"token_embd.weight": tensor("token_embd.weight", (vocab, hidden)),
+          "output_norm.weight": tensor("output_norm.weight", (hidden,))}
+    tied = "output.weight" not in f.tensors
+    ts["output.weight"] = ts["token_embd.weight"] if tied else tensor("output.weight", (vocab, hidden))
+    shapes = {"attn_norm": (hidden,), "attn_q": (nq, hidden), "attn_k": (nkv, hidden), "attn_v": (nkv, hidden),
+              "attn_q_norm": (QWEN3_HEAD_DIM,), "attn_k_norm": (QWEN3_HEAD_DIM,), "attn_output": (hidden, nq),
+              "ffn_norm": (hidden,), "ffn_gate": (ffn, hidden), "ffn_up": (ffn, hidden), "ffn_down": (hidden, ffn)}
+    for i in range(n_layers):
+        for n in _QWEN3_BLOCK:
+            ts[f"blk.{i}.{n}.weight"] = tensor(f"blk.{i}.{n}.weight", shapes[n])
+    tokens = f.get("tokenizer.ggml.tokens")
+    if tokens is not None and len(tokens) > vocab:
+        raise ValueError(f"{f.path}: the vocabulary has {len(tokens)} tokens but token_embd has {vocab} rows")
+    return Qwen3Plan(n_layers, hidden, n_head, n_kv, ffn, vocab, ctx, rope_base, eps, ts, tied)

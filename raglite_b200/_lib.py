@@ -34,8 +34,16 @@ EXPORTS = [
     "rl_chunk_similarities_workspace_bytes", "rl_chunk_similarities", "rl_chunk_partition_workspace_bytes",
     "rl_chunk_partition", "rl_fts_workspace_bytes", "rl_fts_mark", "rl_fts_stem", "rl_fts_verify", "rl_fts_stem_bytes",
     "rl_fts_term_keys", "rl_dequant_rows_f16", "rl_xenc_qlinear_image_bytes", "rl_xenc_pack_qlinear",
-    "rl_xenc_concat_qlinear", "rl_xenc_linear_q", "rl_chunk_embedding_blend",
+    "rl_xenc_concat_qlinear", "rl_xenc_linear_q", "rl_chunk_embedding_blend", "rl_llm_workspace_bytes", "rl_llm_forward",
+    "rl_llm_qgemv_workspace_bytes", "rl_llm_qgemv", "rl_llm_embed", "rl_llm_qk_norm_rope", "rl_llm_attention_workspace_bytes",
+    "rl_llm_attention", "rl_llm_sample_workspace_bytes", "rl_llm_sample",
 ]
+_SIZE_T_RESULTS = ("rl_maxsim_workspace_bytes", "rl_xenc_linear_image_bytes", "rl_xenc_workspace_bytes",
+                   "rl_hits_packed_bytes", "rl_bm25_workspace_bytes", "rl_bm25_packed_bytes", "rl_sat_workspace_bytes",
+                   "rl_sentence_partition_workspace_bytes", "rl_chunklet_partition_workspace_bytes",
+                   "rl_chunk_similarities_workspace_bytes", "rl_chunk_partition_workspace_bytes", "rl_fts_workspace_bytes",
+                   "rl_xenc_qlinear_image_bytes", "rl_llm_workspace_bytes", "rl_llm_qgemv_workspace_bytes",
+                   "rl_llm_attention_workspace_bytes", "rl_llm_sample_workspace_bytes")
 RL_XENC_IMAGE_F16 = 0
 RL_XENC_IMAGE_QUANT = 1
 
@@ -75,6 +83,24 @@ class XencWeights(C.Structure):
         ("emb_ln_b", C.c_void_p), ("layers", C.POINTER(XencLayer)), ("pooler_w", C.c_void_p), ("pooler_b", C.c_void_p),
         ("cls_w", C.c_void_p), ("cls_b", C.c_void_p), ("n_labels", C.c_int32),
     ]
+
+
+RL_LLM_MAX_PARTS = 32
+
+
+class LlmLinear(C.Structure):   # rl_llm_linear
+    _fields_ = [("parts", C.c_void_p * RL_LLM_MAX_PARTS), ("n_parts", C.c_int32), ("N", C.c_int32), ("K", C.c_int32)]
+
+
+class LlmLayer(C.Structure):   # rl_llm_layer
+    _fields_ = [(n, LlmLinear) for n in ("q", "k", "v", "o", "gate", "up", "down")] + [
+        (n, C.c_void_p) for n in ("attn_norm", "q_norm", "k_norm", "ffn_norm")]
+
+
+class LlmWeights(C.Structure):   # rl_llm_weights
+    _fields_ = [(n, C.c_int32) for n in ("n_layers", "hidden", "n_head", "n_kv", "ffn", "vocab", "n_ctx")] + [
+        ("eps", C.c_float), ("rope_base", C.c_float), ("token_embd", LlmLinear), ("output", LlmLinear),
+        ("output_norm", C.c_void_p), ("layers", C.POINTER(LlmLayer))]
 
 
 _lock = threading.Lock()
@@ -159,16 +185,20 @@ def _declare(lib: C.CDLL) -> None:
     lib.rl_xenc_pack_qlinear.argtypes = [i32, vp, i32, i32, vp, vp]
     lib.rl_xenc_concat_qlinear.argtypes = [C.POINTER(C.c_void_p), i32, vp, vp]
     lib.rl_xenc_linear_q.argtypes = [vp, vp, vp, vp, i32, i32, i32, i32, vp]
-    for name in ("rl_chunklet_partition_workspace_bytes", "rl_chunk_similarities_workspace_bytes",
-                 "rl_chunk_partition_workspace_bytes", "rl_fts_workspace_bytes", "rl_xenc_qlinear_image_bytes"):
-        getattr(lib, name).restype = C.c_size_t
+    vp, i32, f32 = C.c_void_p, C.c_int32, C.c_float
+    lib.rl_llm_workspace_bytes.argtypes = [C.POINTER(LlmWeights), i32]
+    lib.rl_llm_forward.argtypes = [C.POINTER(LlmWeights), vp, i32, i32, vp, vp, vp, vp, C.c_size_t, vp]
+    lib.rl_llm_qgemv_workspace_bytes.argtypes = [i32, i32]
+    lib.rl_llm_qgemv.argtypes = [C.POINTER(LlmLinear), vp, vp, i32, vp, C.c_size_t, vp]
+    lib.rl_llm_embed.argtypes = [C.POINTER(LlmLinear), vp, i32, vp, vp]
+    lib.rl_llm_qk_norm_rope.argtypes = [vp, i32, i32, i32, i32, vp, vp, f32, f32, i32, vp, vp, vp, vp]
+    lib.rl_llm_attention_workspace_bytes.argtypes = [i32, i32, i32, i32, i32]
+    lib.rl_llm_attention.argtypes = [vp, vp, vp, i32, i32, i32, i32, i32, vp, vp, C.c_size_t, vp]
+    lib.rl_llm_sample_workspace_bytes.argtypes = [i32]
+    lib.rl_llm_sample.argtypes = [vp, i32, vp, i32, f32, i32, f32, f32, f32, f32, vp, vp, C.c_size_t, vp]
     for name in EXPORTS:
-        if name not in ("rl_last_error", "rl_maxsim_workspace_bytes", "rl_xenc_linear_image_bytes", "rl_xenc_workspace_bytes",
-                        "rl_hits_packed_bytes", "rl_bm25_workspace_bytes", "rl_bm25_packed_bytes",
-                        "rl_sat_workspace_bytes", "rl_sentence_partition_workspace_bytes",
-                        "rl_chunklet_partition_workspace_bytes", "rl_chunk_similarities_workspace_bytes",
-                        "rl_chunk_partition_workspace_bytes", "rl_fts_workspace_bytes", "rl_xenc_qlinear_image_bytes"):
-            getattr(lib, name).restype = C.c_int
+        if name != "rl_last_error":
+            getattr(lib, name).restype = C.c_size_t if name in _SIZE_T_RESULTS else C.c_int
 
 
 def load(*, build_if_missing: bool = True) -> C.CDLL:

@@ -9,7 +9,7 @@ from __future__ import annotations
 
 import contextlib
 from collections.abc import Sequence
-from dataclasses import dataclass
+from dataclasses import dataclass, field, replace
 from typing import Any
 
 import numpy as np
@@ -398,6 +398,7 @@ class ChunkSpan:
     """A run of consecutive chunks of one document (reference ``_database.py:326-398``)."""
 
     chunks: list[Chunk]
+    document: Any = field(default=None, compare=False, repr=False)   # the Document record, when the index holds one
 
     @property
     def document_id(self) -> str:
@@ -413,6 +414,50 @@ class ChunkSpan:
 
     def __str__(self) -> str:
         return self.content
+
+    @property
+    def source(self) -> str:
+        """The document's url, else its filename (``_database.py:350``): from the ``Document`` record when the span
+        has one, else from the first chunk's ``url`` / ``filename`` metadata (lists, as ``insert_documents`` stores
+        every value, give their first value that is not None)."""
+        if self.document is not None:
+            return str(self.document.url or self.document.filename or "")
+        meta = self.chunks[0].metadata_ if self.chunks else {}
+
+        def first(key: str) -> Any:
+            v = meta.get(key)
+            if isinstance(v, (list, tuple)):
+                v = next((x for x in v if x is not None), None)
+            return v
+
+        return str(first("url") or first("filename") or "")
+
+    def to_xml(self, index: int | None = None) -> str:
+        """The span as the ``<document>`` element RAG prompts carry (``_database.py:338-360``)."""
+        if not self.chunks:
+            return ""
+        from xml.sax.saxutils import escape
+
+        attr = f' index="{index}"' if index is not None else ""
+        return "\n".join([
+            f'<document{attr} id="{self.document_id}">',
+            f"<source>{self.source}</source>",
+            f'<span from_chunk_id="{self.chunks[0].id}" to_chunk_id="{self.chunks[-1].id}">',
+            f"<headings>\n{escape(self.chunks[0].headings.strip())}\n</headings>",
+            f"<content>\n{escape(''.join(c.body for c in self.chunks).strip())}\n</content>",
+            "</span>",
+            "</document>"])
+
+    def to_json(self, index: int | None = None) -> str:
+        """The span as a JSON object (``_database.py:362-385``)."""
+        if not self.chunks:
+            return "{}"
+        import json
+
+        return json.dumps({**({"index": index} if index is not None else {}), "id": self.document_id, "source": self.source,
+                           "span": {"from_chunk_id": self.chunks[0].id, "to_chunk_id": self.chunks[-1].id,
+                                    "headings": self.chunks[0].headings.strip(),
+                                    "content": "".join(c.body for c in self.chunks).strip()}})
 
 
 # ---- fusion and span collation batched on device chunk indices -----------------------------------------------
@@ -547,8 +592,17 @@ def retrieve_chunk_spans(
             n_span = int(out["n_span"][0])
             member = out["member"][0].tolist()
             start, length = out["span_start"][0, :n_span].tolist(), out["span_len"][0, :n_span].tolist()
-            return [ChunkSpan([local.chunks[member[s + j]] for j in range(n)]) for s, n in zip(start, length, strict=True)]
-    return _retrieve_chunk_spans_host(chunk_ids, neighbors=neighbors, config=config)
+            return with_documents([ChunkSpan([local.chunks[member[s + j]] for j in range(n)])
+                                   for s, n in zip(start, length, strict=True)], index)
+    return with_documents(_retrieve_chunk_spans_host(chunk_ids, neighbors=neighbors, config=config), index)
+
+
+def with_documents(spans: list[ChunkSpan], index: Any) -> list[ChunkSpan]:
+    """``spans`` with the ``Document`` record of each span's document set from the index's ``documents`` (the records
+    ``insert_documents`` kept), where it holds one and the span has none."""
+    docs = getattr(getattr(index, "local", index), "documents", None) or {}
+    return [replace(s, document=docs[s.document_id]) if s.document is None and s.document_id in docs else s
+            for s in spans]
 
 
 def _retrieve_chunk_spans_host(

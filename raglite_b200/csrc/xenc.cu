@@ -19,6 +19,7 @@
 
 #include "common.cuh"
 #include "hopper_ptx.cuh"
+#include "qimg.cuh"
 
 namespace rl {
 namespace {
@@ -109,7 +110,8 @@ __global__ void pack_linear_kernel(const float* __restrict__ W, int N, int K, __
 // Epilogue of one work item, run by each consumer warpgroup on its 64 tokens: + bias -> activation -> fp16 -> shared
 // staging (columns >= nb belong to no output: skipped) -> 16-byte row-contiguous stores.
 __device__ __forceinline__ void linear_epilogue(const float (&acc)[64], const float* __restrict__ bias, __half* __restrict__ Y,
-                                                int T, int N, int act, int m_tile, int pass, int wg, unsigned char* stg) {
+                                                int ldy, int T, int N, int act, int m_tile, int pass, int wg,
+                                                unsigned char* stg) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, wt = threadIdx.x & 127;
   const int r_lo = (warp & 3) * 16 + (lane >> 2);   // rows r_lo and r_lo + 8 of this warpgroup's 64
   const int c_lane = 2 * (lane & 3);
@@ -134,7 +136,7 @@ __device__ __forceinline__ void linear_epilogue(const float (&acc)[64], const fl
     const int rr = idx / row_chunks, ch = idx - rr * row_chunks;
     const int grow = row_base + rr;
     if (grow < T)
-      *reinterpret_cast<uint4*>(Y + (size_t)grow * N + n0 + ch * 8) =
+      *reinterpret_cast<uint4*>(Y + (size_t)grow * ldy + n0 + ch * 8) =
           *reinterpret_cast<const uint4*>(stg + (uint32_t)rr * kEpiPitch + (uint32_t)ch * 16u);
   }
   named_bar_sync(2 + wg, 128);   // the staging buffer is free for the next item
@@ -143,8 +145,8 @@ __device__ __forceinline__ void linear_epilogue(const float (&acc)[64], const fl
 struct LinArgs {
   const __half* img;   // packed weights
   const float* bias;   // [N]
-  __half* Y;           // [T, N]
-  int T, N, K, act;    // act: 0 none, 1 GELU(erf)
+  __half* Y;           // [T, ldy]
+  int ldy, T, N, K, act;    // act: 0 none, 1 GELU(erf)
   int n_pass, n_ks, stages;
 };
 
@@ -219,22 +221,12 @@ __global__ void __launch_bounds__(kLinThreads, 1) linear_wgmma_kernel(const __gr
       wgmma_wait<0>();
       __syncwarp();
       if (lane == 0) mbar_arrive(&empty[prev]);
-      linear_epilogue(acc, t.bias, t.Y, t.T, t.N, t.act, m_tile, pass, wg, stg);
+      linear_epilogue(acc, t.bias, t.Y, t.ldy, t.T, t.N, t.act, m_tile, pass, wg, stg);
     }
   }
 }
-// ---- GGUF-quantized weights ------------------------------------------------------------------------------
-// Types by their GGML ids.  A block of K elements of one row: Q8_0 32 elements (fp16 d, 32 int8), Q4_K 256 (fp16 d,
-// fp16 dmin, 12 bytes of 6-bit scales and mins, 128 bytes of nibbles), Q6_K 256 (128 bytes of low nibbles, 64 of high
-// bit pairs, 16 int8 scales, fp16 d).  Every value is ggml's formula in float32, each product and difference rounded on
-// its own (no contraction), then rounded once to fp16 to nearest even:
-//   Q8_0 d q      Q4_K (d sc) q - (dmin m)      Q6_K (d sc) (q - 32)
-constexpr int kGgmlQ8_0 = 8, kGgmlQ4_K = 12, kGgmlQ6_K = 14;
 
-__host__ __device__ inline int q_block_elems(int type) { return type == kGgmlQ8_0 ? 32 : 256; }
-__host__ __device__ inline int q_block_bytes(int type) { return type == kGgmlQ8_0 ? 34 : type == kGgmlQ4_K ? 144 : 210; }
-inline bool q_type_ok(int type) { return type == kGgmlQ8_0 || type == kGgmlQ4_K || type == kGgmlQ6_K; }
-
+// ---- GGUF-quantized weights (types and image layout: qimg.cuh) -----------------------------------------
 // The small integer u (< 2^23) as float without a conversion instruction: its bits under 2^23's exponent, minus 2^23 +
 // `bias`.  Exact, so (float)(u - bias) either way.
 __device__ __forceinline__ float small_int_f(uint32_t u, float bias) {
@@ -243,17 +235,6 @@ __device__ __forceinline__ float small_int_f(uint32_t u, float bias) {
 __device__ __forceinline__ float ld_half(const unsigned char* p) {
   return __half2float(__ushort_as_half(*reinterpret_cast<const unsigned short*>(p)));
 }
-// Q4_K's 6-bit scale and min of sub-block j (ggml's get_scale_min_k4).
-__host__ __device__ inline void q4k_scale_min(int j, const unsigned char* s, int& sc, int& m) {
-  if (j < 4) {
-    sc = s[j] & 63;
-    m = s[j + 4] & 63;
-  } else {
-    sc = (s[j + 4] & 0xF) | ((s[j - 4] >> 6) << 4);
-    m = (s[j + 4] >> 4) | ((s[j] >> 6) << 4);
-  }
-}
-
 // rows x K elements from GGUF blocks (row r's blocks at r * K / block_elems) to fp16: one thread per element.
 __global__ void dequant_rows_kernel(int type, const unsigned char* __restrict__ blocks, int64_t rows, int K,
                                     __half* __restrict__ out) {
@@ -287,26 +268,8 @@ __global__ void dequant_rows_kernel(int type, const unsigned char* __restrict__ 
   }
 }
 
-// ---- quantized weight image ---------------------------------------------------------------------------------
-// Header (QImgHead, then n_pass QImgPass) and, from kQImgData on, per pass and 128-element K slice one run of nb16
-// (the pass's rows rounded up to 16) rows of row_bytes each: one bulk copy per stage.  A row's slice (zero bytes for the
-// padding rows, which decode to +0):
-//   Q8_0  136 B: four fp16 d, then 128 int8
-//   Q4_K   76 B: fp16 d, fp16 dmin, the four 6-bit scales and four mins unpacked to bytes, the 64 nibble bytes of the
-//                half super-block (low nibbles: elements 0-31 and 64-95, high nibbles: 32-63 and 96-127)
-//   Q6_K  108 B: the half super-block's 64 ql bytes, 32 qh bytes, 8 int8 scales, fp16 d, 2 zero bytes
-// That is 1.0, 1.056 and 1.029 times the GGUF bytes.  Each pass carries its own type, so images of tensors of different
-// types concatenate pass by pass (rl_xenc_concat_qlinear).
-constexpr int kQSliceK = 128;                  // K elements per stage: two wgmma slices
-constexpr uint32_t kQMaxRowBytes = 136;
-struct QImgHead { int32_t n_pass, N, K, magic; };
-struct QImgPass { int32_t type, row_bytes; int64_t offset; };   // offset from the image's start
-constexpr int32_t kQImgMagic = 0x51494d47;     // "QIMG"
-constexpr size_t kQImgMaxPasses = 64;          // N <= 8192
-constexpr size_t kQImgData = 2048;             // where the passes' rows start (1024-aligned room for the header)
-static_assert(sizeof(QImgHead) + kQImgMaxPasses * sizeof(QImgPass) <= kQImgData, "the header must fit before the data");
-
-__host__ __device__ inline uint32_t q_row_bytes(int type) { return type == kGgmlQ8_0 ? 136u : type == kGgmlQ4_K ? 76u : 108u; }
+// ---- quantized weight image (layout: qimg.cuh) -----------------------------------------------------
+static_assert(kPassN == kQPassRows, "a wgmma pass is one image pass");
 inline size_t q_pass_bytes(int type, int N, int K, int pass) {
   const int nb16 = (pass_rows(N, pass) + 15) / 16 * 16;
   return (size_t)(K / kQSliceK) * nb16 * q_row_bytes(type);
@@ -447,8 +410,8 @@ constexpr int kQMaxStages = 4;
 struct QLinArgs {
   const unsigned char* img;   // quantized image
   const float* bias;          // [N]
-  __half* Y;                  // [T, N]
-  int T, N, K, act;
+  __half* Y;                  // [T, ldy]
+  int ldy, T, N, K, act;
   int n_pass, n_qs, stages;
 };
 
@@ -552,7 +515,7 @@ __global__ void __launch_bounds__(kQLinThreads, 1) linear_q_wgmma_kernel(const _
       wgmma_wait<0>();
       __syncwarp();
       if (lane == 0) mbar_arrive(&empty[prev]);
-      linear_epilogue(acc, t.bias, t.Y, t.T, t.N, t.act, m_tile, pass, wg, stg);
+      linear_epilogue(acc, t.bias, t.Y, t.ldy, t.T, t.N, t.act, m_tile, pass, wg, stg);
     }
   }
 }
@@ -1176,7 +1139,7 @@ static int launch_linear(const __half* X, const void* img, const float* bias, __
                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   RL_REQUIRE(r == CUDA_SUCCESS, RL_ECUDA, "cuTensorMapEncodeTiled failed (%d) for X[%d, %d]", (int)r, T, K);
   LinArgs t;
-  t.img = reinterpret_cast<const __half*>(img); t.bias = bias; t.Y = Y; t.T = T; t.N = N; t.K = K; t.act = act;
+  t.img = reinterpret_cast<const __half*>(img); t.bias = bias; t.Y = Y; t.ldy = N; t.T = T; t.N = N; t.K = K; t.act = act;
   t.n_pass = (N + kPassN - 1) / kPassN;
   t.n_ks = (K + kSliceK - 1) / kSliceK;
   const uint32_t tail = 2 * kMaxStages * 8 + kEpiBytes;   // barriers + epilogue staging
@@ -1281,8 +1244,8 @@ extern "C" int rl_xenc_concat_qlinear(const void* const* parts, int n_parts, voi
   return RL_OK;
 }
 
-static int launch_qlinear(const __half* X, const void* img, const float* bias, __half* Y, int T, int N, int K, int act,
-                          int sm_count, cudaStream_t stream) {
+static int launch_qlinear_act(const __half* X, const void* img, const float* bias, __half* Y, int ldy, int T, int N, int K,
+                              int act, int sm_count, cudaStream_t stream) {
   EncodeTiledFn enc = encode_tiled_fn();
   RL_REQUIRE(enc != nullptr, RL_ECUDA, "cuTensorMapEncodeTiled is not available from this driver");
   RL_REQUIRE((reinterpret_cast<uintptr_t>(X) & 15) == 0 && (reinterpret_cast<uintptr_t>(img) & 15) == 0, RL_EINVAL,
@@ -1299,7 +1262,7 @@ static int launch_qlinear(const __half* X, const void* img, const float* bias, _
                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   RL_REQUIRE(r == CUDA_SUCCESS, RL_ECUDA, "cuTensorMapEncodeTiled failed (%d) for X[%d, %d]", (int)r, T, K);
   QLinArgs t;
-  t.img = reinterpret_cast<const unsigned char*>(img); t.bias = bias; t.Y = Y; t.T = T; t.N = N; t.K = K; t.act = act;
+  t.img = reinterpret_cast<const unsigned char*>(img); t.bias = bias; t.Y = Y; t.ldy = ldy; t.T = T; t.N = N; t.K = K; t.act = act;
   t.n_pass = (N + kPassN - 1) / kPassN;
   t.n_qs = K / kQSliceK;
   const uint32_t tail = 3 * kQMaxStages * 8 + kEpiBytes;   // barriers + epilogue staging
@@ -1313,6 +1276,18 @@ static int launch_qlinear(const __half* X, const void* img, const float* bias, _
   linear_q_wgmma_kernel<<<grid, kQLinThreads, smem, stream>>>(tm, t);
   RL_CUDA_CHECK(cudaGetLastError());
   return RL_OK;
+}
+
+static int launch_qlinear(const __half* X, const void* img, const float* bias, __half* Y, int T, int N, int K, int act,
+                          int sm_count, cudaStream_t stream) {
+  return launch_qlinear_act(X, img, bias, Y, N, T, N, K, act, sm_count, stream);
+}
+
+int rl::launch_qlinear_ld(const __half* X, const void* img, const float* bias, __half* Y, int ldy, int T, int N, int K,
+                          int sm_count, cudaStream_t stream) {
+  RL_REQUIRE(ldy >= N && ldy % 8 == 0 && (reinterpret_cast<uintptr_t>(Y) & 15) == 0, RL_EINVAL,
+             "quantized linear: ldy=%d must be >= N=%d and a multiple of 8, Y 16-byte aligned", ldy, N);
+  return launch_qlinear_act(X, img, bias, Y, ldy, T, N, K, 0, sm_count, stream);
 }
 
 // The linear of an encoder layer by its image type: RL_XENC_IMAGE_F16 (rl_xenc_pack_linear) or RL_XENC_IMAGE_QUANT.
