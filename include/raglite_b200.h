@@ -646,6 +646,27 @@ int rl_llm_sample(const float* logits, int V, const int32_t* hist, int n_hist, f
                   float min_p, float repeat_penalty, float u, int32_t* out_id, void* workspace, size_t workspace_bytes,
                   void* stream);
 
+/* ---- grammar-constrained sampling ----------------------------------------------------------------------------------
+ * A grammar is a byte-level DFA: trans int16 [n_states, 256] (the next state, or -1), state 0 the start.
+ * rl_grammar_token_index walks every token's bytes from every state: index[s, v] (int16 [n_states, V], device) is the
+ * state after token v's bytes token_bytes[offsets[v] .. offsets[v + 1]) (device uint8 / int64 [V + 1]), or -1 when
+ * a byte has no transition or the piece is empty.  A transition outside [0, n_states) counts as none. */
+#define RL_GRAMMAR_MAX_STATES 1024
+int rl_grammar_token_index(const int16_t* trans, int n_states, const uint8_t* token_bytes, const int64_t* offsets, int V,
+                           int16_t* index, void* stream);
+/* rl_llm_sample restricted to the ids grammar state *state (device int32) allows: v with index[*state, v] >= 0, and
+ * each end-of-generation id in eog_ids (host, n_eog <= RL_LLM_MAX_EOG) exactly when accept[*state] (device uint8
+ * [n_states]), and whose logit is neither -inf nor NaN.  Other ids become -inf before the penalty, and top-k keeps at
+ * most the allowed count.  Then *state
+ * becomes index[*state, *out_id], unchanged after an end-of-generation id.  When nothing is allowed *out_id is
+ * RL_LLM_NO_TOKEN and *state is unchanged. */
+#define RL_LLM_MAX_EOG 8
+#define RL_LLM_NO_TOKEN (-1)
+int rl_llm_sample_masked(const float* logits, int V, const int32_t* hist, int n_hist, float temperature, int top_k,
+                         float top_p, float min_p, float repeat_penalty, float u, const int16_t* index, int n_states,
+                         const uint8_t* accept, const int32_t* eog_ids, int n_eog, int32_t* state, int32_t* out_id,
+                         void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -10,7 +10,8 @@ Hugging Face directory or the config's GGUF file, ``register_gguf_embedder``); a
 ``split_chunklets`` / ``split_chunks`` / ``split_documents``, the chunklet and chunk partitions on the GPU; and
 ``Document`` with ``insert_documents`` / ``delete_documents`` / ``delete_documents_by_metadata``, ingest into the
 registered index on the GPU; and
-``LlmEngine`` with ``rag`` / ``add_context`` / ``retrieve_context``, generation with the config's Qwen3 GGUF on the GPU.
+``LlmEngine`` with ``rag`` / ``async_rag`` / ``add_context`` / ``retrieve_context``, generation with the config's Qwen3
+GGUF on the GPU, searching the knowledge base on its own through grammar-constrained function calling.
 """
 
 from ._chunks import (
@@ -28,7 +29,7 @@ from ._index import Chunk, CorpusIndex, get_index, merge_hits, register_index, u
 from ._insert import Document, delete_documents, delete_documents_by_metadata, insert_documents
 from ._llm import LlmEngine, register_gguf_llm, register_llm
 from ._query_adapter import update_query_adapter
-from ._rag import RAG_INSTRUCTION_TEMPLATE, add_context, get_context_size, rag, retrieve_context
+from ._rag import RAG_INSTRUCTION_TEMPLATE, add_context, async_rag, get_context_size, rag, retrieve_context
 from ._search import (
     ChunkSpan,
     collate_spans_device,
@@ -62,6 +63,7 @@ __all__ = [
     "Chunk",
     "LlmEngine",
     "add_context",
+    "async_rag",
     "get_context_size",
     "rag",
     "register_gguf_llm",

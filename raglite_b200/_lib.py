@@ -36,7 +36,8 @@ EXPORTS = [
     "rl_fts_term_keys", "rl_dequant_rows_f16", "rl_xenc_qlinear_image_bytes", "rl_xenc_pack_qlinear",
     "rl_xenc_concat_qlinear", "rl_xenc_linear_q", "rl_chunk_embedding_blend", "rl_llm_workspace_bytes", "rl_llm_forward",
     "rl_llm_qgemv_workspace_bytes", "rl_llm_qgemv", "rl_llm_embed", "rl_llm_qk_norm_rope", "rl_llm_attention_workspace_bytes",
-    "rl_llm_attention", "rl_llm_sample_workspace_bytes", "rl_llm_sample",
+    "rl_llm_attention", "rl_llm_sample_workspace_bytes", "rl_llm_sample", "rl_grammar_token_index",
+    "rl_llm_sample_masked",
 ]
 _SIZE_T_RESULTS = ("rl_maxsim_workspace_bytes", "rl_xenc_linear_image_bytes", "rl_xenc_workspace_bytes",
                    "rl_hits_packed_bytes", "rl_bm25_workspace_bytes", "rl_bm25_packed_bytes", "rl_sat_workspace_bytes",
@@ -44,6 +45,8 @@ _SIZE_T_RESULTS = ("rl_maxsim_workspace_bytes", "rl_xenc_linear_image_bytes", "r
                    "rl_chunk_similarities_workspace_bytes", "rl_chunk_partition_workspace_bytes", "rl_fts_workspace_bytes",
                    "rl_xenc_qlinear_image_bytes", "rl_llm_workspace_bytes", "rl_llm_qgemv_workspace_bytes",
                    "rl_llm_attention_workspace_bytes", "rl_llm_sample_workspace_bytes")
+RL_LLM_MAX_EOG = 8
+RL_LLM_NO_TOKEN = -1
 RL_XENC_IMAGE_F16 = 0
 RL_XENC_IMAGE_QUANT = 1
 
@@ -196,6 +199,9 @@ def _declare(lib: C.CDLL) -> None:
     lib.rl_llm_attention.argtypes = [vp, vp, vp, i32, i32, i32, i32, i32, vp, vp, C.c_size_t, vp]
     lib.rl_llm_sample_workspace_bytes.argtypes = [i32]
     lib.rl_llm_sample.argtypes = [vp, i32, vp, i32, f32, i32, f32, f32, f32, f32, vp, vp, C.c_size_t, vp]
+    lib.rl_grammar_token_index.argtypes = [vp, i32, vp, vp, i32, vp, vp]
+    lib.rl_llm_sample_masked.argtypes = [vp, i32, vp, i32, f32, i32, f32, f32, f32, f32, vp, i32, vp,
+                                         C.POINTER(C.c_int32), i32, vp, vp, vp, C.c_size_t, vp]
     for name in EXPORTS:
         if name != "rl_last_error":
             getattr(lib, name).restype = C.c_size_t if name in _SIZE_T_RESULTS else C.c_int

@@ -5,6 +5,10 @@ as parts of 8192), an fp16 KV cache of ``n_ctx`` positions and one workspace.  A
 the wgmma quantized linear (``rl_llm_forward`` with T > 1), then each token is one decode step (T = 1: every linear a
 GEMV) and one ``rl_llm_sample`` on the device.  The sampled id feeds the next step on the device; one copy per step
 brings it to the host for the text.
+
+Under a grammar (``generate(..., grammar=...)``) the step samples with ``rl_llm_sample_masked`` instead: the engine
+keeps, per grammar text, its DFA and the token index ``rl_grammar_token_index`` built over ``QwenTokenizer.token_bytes``
+(control tokens as their text), and the DFA state stays on the device between steps.
 """
 
 from __future__ import annotations
@@ -12,6 +16,7 @@ from __future__ import annotations
 import codecs
 import ctypes as C
 import secrets
+from collections import OrderedDict
 from collections.abc import Iterator, Sequence
 from pathlib import Path
 from typing import Any
@@ -21,11 +26,15 @@ import torch
 
 from . import _lib
 from ._gguf import GGUFFile, GGUFTensor, Qwen3Plan, find_cached_gguf, parse_embedder, qwen3_plan
+from ._grammar import Grammar, compile_gbnf
 from ._lib import LlmLayer, LlmLinear, LlmWeights, check
 
 PART_ROWS = 8192
 MAX_TOP_K = 256
 PENALTY_LAST_N = 64
+# Token indexes an engine keeps (least recently used dropped first): each is S x vocab int16 of device memory, 40 MB
+# at 130 states and Qwen3's vocabulary, 311 MB at the 1024-state cap.  rag() uses three grammars per tool.
+MAX_GRAMMARS = 8
 # The Qwen2 pre-tokenizer's split (llama.cpp's LLAMA_VOCAB_PRE_TYPE_QWEN2, transformers' Qwen2TokenizerFast)
 QWEN2_SPLIT = (r"(?i:'s|'t|'re|'ve|'m|'ll|'d)|[^\r\n\p{L}\p{N}]?\p{L}+|\p{N}| ?[^\s\p{L}\p{N}]+[\r\n]*|\s*[\r\n]+|"
                r"\s+(?!\S)|\s+")
@@ -146,6 +155,10 @@ class LlmEngine:
         self._ids_copied: torch.cuda.Event | None = None   # the last copy out of _ids_host
         self._hist_host = torch.empty(PENALTY_LAST_N, dtype=torch.int32, pin_memory=True)
         self.n_past = 0
+        self._grammars: OrderedDict[str, GrammarIndex] = OrderedDict()
+        self._vocab_dev: tuple[torch.Tensor, torch.Tensor] | None = None
+        with torch.cuda.device(self.device):
+            self.grammar_state = torch.zeros(1, dtype=torch.int32, device=self.device)
 
     # -- construction --
     @classmethod
@@ -240,17 +253,57 @@ class LlmEngine:
                 self._forward_dev(self._ids[p0 + lo:].data_ptr(), min(step, n - lo))
         return self.logits
 
+    def grammar_index(self, grammar: "str | Grammar") -> "GrammarIndex":
+        """The DFA and device token index of a grammar (GBNF text or compiled), built once per grammar text and kept
+        for the ``MAX_GRAMMARS`` most recently used."""
+        text = grammar if isinstance(grammar, str) else grammar.text
+        if text in self._grammars:
+            self._grammars.move_to_end(text)
+        else:
+            g = grammar if isinstance(grammar, Grammar) else compile_gbnf(grammar)
+            if self.tokenizer is None:
+                raise ValueError("grammar-constrained generation needs the engine's tokenizer")
+            with torch.cuda.device(self.device):
+                if self._vocab_dev is None:
+                    pieces = list(self.tokenizer.token_bytes[:self.plan.vocab])
+                    pieces += [b""] * (self.plan.vocab - len(pieces))   # ids past the vocabulary: empty, never allowed
+                    offs = np.zeros(len(pieces) + 1, dtype=np.int64)
+                    offs[1:] = np.cumsum([len(p) for p in pieces])
+                    flat = np.frombuffer(b"".join(pieces) or b"\0", dtype=np.uint8)
+                    self._vocab_dev = (torch.from_numpy(flat.copy()).to(self.device), torch.from_numpy(offs).to(self.device))
+                trans = torch.from_numpy(np.ascontiguousarray(g.trans, dtype=np.int16)).to(self.device)
+                index = torch.empty((g.n_states, self.plan.vocab), dtype=torch.int16, device=self.device)
+                check(self.lib.rl_grammar_token_index(trans.data_ptr(), g.n_states, self._vocab_dev[0].data_ptr(),
+                                                      self._vocab_dev[1].data_ptr(), self.plan.vocab, index.data_ptr(),
+                                                      _stream()), "rl_grammar_token_index")
+                accept = torch.from_numpy(g.accept.astype(np.uint8)).to(self.device)
+            self._grammars[text] = GrammarIndex(g, index, accept)
+            while len(self._grammars) > MAX_GRAMMARS:
+                self._grammars.popitem(last=False)
+        return self._grammars[text]
+
     def sample(self, history: Sequence[int], *, temperature: float, top_k: int, top_p: float, min_p: float,
-               repeat_penalty: float, u: float) -> torch.Tensor:
-        """Sample from ``self.logits`` into the device id ``self._tok`` (see ``rl_llm_sample``)."""
+               repeat_penalty: float, u: float, grammar: "GrammarIndex | None" = None) -> torch.Tensor:
+        """Sample from ``self.logits`` into the device id ``self._tok`` (see ``rl_llm_sample``); under ``grammar``,
+        among the ids its state ``self.grammar_state`` allows, advancing that state (see ``rl_llm_sample_masked``)."""
         hist = np.asarray(history[-PENALTY_LAST_N:], dtype=np.int32)
         self._hist_host[:len(hist)] = torch.from_numpy(hist)
         with torch.cuda.device(self.device):
             self._hist[:len(hist)].copy_(self._hist_host[:len(hist)], non_blocking=True)
-            check(self.lib.rl_llm_sample(self.logits.data_ptr(), self.plan.vocab, self._hist.data_ptr(), len(hist),
-                                         float(temperature), int(top_k), float(top_p), float(min_p), float(repeat_penalty),
-                                         float(u), self._tok.data_ptr(), self._sample_ws.data_ptr(),
-                                         self._sample_ws.numel(), _stream()), "rl_llm_sample")
+            if grammar is None:
+                check(self.lib.rl_llm_sample(self.logits.data_ptr(), self.plan.vocab, self._hist.data_ptr(), len(hist),
+                                             float(temperature), int(top_k), float(top_p), float(min_p),
+                                             float(repeat_penalty), float(u), self._tok.data_ptr(),
+                                             self._sample_ws.data_ptr(), self._sample_ws.numel(), _stream()),
+                      "rl_llm_sample")
+            else:
+                eog = sorted(self.stop_ids())
+                check(self.lib.rl_llm_sample_masked(
+                    self.logits.data_ptr(), self.plan.vocab, self._hist.data_ptr(), len(hist), float(temperature),
+                    int(top_k), float(top_p), float(min_p), float(repeat_penalty), float(u), grammar.index.data_ptr(),
+                    grammar.dfa.n_states, grammar.accept.data_ptr(), (C.c_int32 * max(1, len(eog)))(*eog), len(eog),
+                    self.grammar_state.data_ptr(), self._tok.data_ptr(), self._sample_ws.data_ptr(),
+                    self._sample_ws.numel(), _stream()), "rl_llm_sample_masked")
         return self._tok
 
     def stop_ids(self) -> set[int]:
@@ -263,9 +316,12 @@ class LlmEngine:
 
     def generate_ids(self, prompt_ids: Sequence[int], *, max_tokens: int | None = None, temperature: float = 0.6,
                      top_k: int = 20, top_p: float = 0.95, min_p: float = 0.0, repeat_penalty: float = 1.1,
-                     seed: int | None = None) -> Iterator[int]:
+                     seed: int | None = None, grammar: "str | Grammar | None" = None) -> Iterator[int]:
         """Token ids after ``prompt_ids`` (a fresh sequence), stop tokens excluded: until a stop token, ``max_tokens``
-        (None: until ``n_ctx``) or the context is full."""
+        (None: until ``n_ctx``) or the context is full.  Under ``grammar`` (GBNF text or compiled) every id keeps the
+        text a prefix of the grammar's language, and a stop token is allowed only where the text is complete; where it
+        is complete and cannot continue, a stop token is the only choice."""
+        gi = None if grammar is None else self.grammar_index(grammar)
         if not (1 <= top_k <= MAX_TOP_K):
             raise ValueError(f"top_k={top_k} unsupported (1 .. {MAX_TOP_K})")
         if temperature < 0:
@@ -277,14 +333,19 @@ class LlmEngine:
         self.reset()
         self.prefill(prompt)
         history, stops = list(prompt), self.stop_ids()
+        if gi is not None:
+            self.grammar_state.zero_()
         n = 0
         while max_tokens is None or n < max_tokens:
             u = min(float(np.float32(rng.random())), float(np.nextafter(np.float32(1), np.float32(0))))
             tok = self.sample(history, temperature=temperature, top_k=top_k, top_p=top_p, min_p=min_p,
-                              repeat_penalty=repeat_penalty, u=u)
+                              repeat_penalty=repeat_penalty, u=u, grammar=gi)
             self._tok_host.copy_(tok, non_blocking=True)
             torch.cuda.current_stream(self.device).synchronize()
             t = int(self._tok_host[0])
+            if t == _lib.RL_LLM_NO_TOKEN:
+                raise RuntimeError("the grammar allows no token of this vocabulary here (and no end-of-generation "
+                                   "token unless the text is complete)")
             if t in stops:
                 return
             yield t
@@ -320,6 +381,13 @@ class LlmEngine:
         pending += dec.decode(b"", final=True)
         if pending:
             yield pending
+
+
+class GrammarIndex:
+    """A grammar on one engine: its DFA, the device token index int16 [S, vocab] and accepting states uint8 [S]."""
+
+    def __init__(self, dfa: Grammar, index: torch.Tensor, accept: torch.Tensor) -> None:
+        self.dfa, self.index, self.accept = dfa, index, accept
 
 
 # ---- registry ----------------------------------------------------------------------------------------------------

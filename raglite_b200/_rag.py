@@ -4,17 +4,18 @@
 Restated in behaviour from the reference (``_rag.py``): the token estimate ``len // 3``, the left clip of the
 messages and the proportional trim of the context to the context window, and the RAG instruction template.  ``rag``
 renders ChatML as llama-cpp-python's chat handler does without tools and samples with the settings RAGLite ends up with
-for a ``qwen3`` model.  Tool calling (the model searching on its own) is not supported: the last message must carry its
-context.
+for a ``qwen3`` model.  When the last message carries no context, the model may search the knowledge base on its own:
+RAGLite's ``search_knowledge_base`` tool through the function-calling protocol of ``_tools.chat_completion``.
 """
 
 from __future__ import annotations
 
+import asyncio
 import contextlib
 import json
 import logging
 import warnings
-from collections.abc import Callable, Iterator, Mapping, Sequence
+from collections.abc import AsyncIterator, Callable, Iterator, Mapping, Sequence
 from typing import Any
 
 import numpy as np
@@ -24,6 +25,7 @@ from ._gguf import parse_embedder
 from ._index import Chunk, get_index
 from ._llm import find_llm, get_llm
 from ._search import ChunkSpan, retrieve_chunk_spans, with_documents
+from ._tools import chat_completion, render_chatml_tools
 
 logger = logging.getLogger(__name__)
 
@@ -152,8 +154,9 @@ def _clip(messages: list[dict[str, str]], max_tokens: int) -> list[dict[str, str
 
 
 def render_chatml(messages: Sequence[Mapping[str, Any]]) -> str:
-    """ChatML as the chat handler renders messages without tools: system, user and assistant messages with content,
-    then the assistant's turn."""
+    """ChatML of the system, user and assistant messages with content, then the assistant's turn.  This equals the
+    chat handler's rendering (``render_chatml_tools``, which ``rag()`` uses) for messages of those roles only; the
+    handler also renders every message's header, an assistant's tool calls and a ``tool`` message's header."""
     parts = [f"<|im_start|>{m['role']}\n{m['content']}<|im_end|>\n" for m in messages
              if m.get("role") in ("system", "user") or (m.get("role") == "assistant" and m.get("content"))]
     return "".join(parts) + "<|im_start|>assistant\n"
@@ -164,18 +167,112 @@ def _has_context(message: Mapping[str, Any]) -> bool:
     return any(tag in content for tag in ("<context>", "<document", "from_chunk_id"))
 
 
-def rag(messages: list[dict[str, str]], *, on_retrieval: Callable[[list[ChunkSpan]], None] | None = None,
-        config: RAGLiteConfig, max_tokens: int | None = None, seed: int | None = None) -> Iterator[str]:
-    """Stream the registered LLM's answer to ``messages`` (whose last message carries its context, from
-    ``retrieve_context`` + ``add_context``), then append it to ``messages`` as the assistant's message."""
-    engine = get_llm(config)
-    clipped = _clip(messages, engine.n_ctx)
-    if not clipped or not _has_context(clipped[-1]):
-        raise NotImplementedError("rag() without context in the last message needs tool calling, which is not supported "
-                                  "here: retrieve it with retrieve_context and add it with add_context first")
-    prompt = engine.tokenizer.encode(render_chatml(clipped))
+# RAGLite's tool for searching the knowledge base (``_rag.py``'s ``_get_tools``).
+SEARCH_KNOWLEDGE_BASE_TOOL = {
+    "type": "function",
+    "function": {
+        "name": "search_knowledge_base",
+        "description": (
+            "Search the knowledge base.\n"
+            "IMPORTANT: You MAY NOT use this function if the question can be answered with common knowledge or "
+            "straightforward reasoning.\n"
+            "For multi-faceted questions, call this function once for each facet."),
+        "parameters": {
+            "type": "object",
+            "properties": {
+                "query": {
+                    "type": "string",
+                    "description": (
+                        "The `query` string MUST be a precise single-faceted question in the user's language.\n"
+                        "The `query` string MUST resolve all pronouns to explicit nouns."),
+                },
+            },
+            "required": ["query"],
+            "additionalProperties": False,
+        },
+    },
+}
+
+
+def _run_tools(tool_calls: list[dict[str, Any]], on_retrieval: Callable[[list[ChunkSpan]], None] | None,
+               config: RAGLiteConfig, *, messages: list[dict[str, Any]]) -> list[dict[str, Any]]:
+    """Run each ``search_knowledge_base`` call in order, limit all their spans together to the context window, and
+    return one ``tool`` message per call (``on_retrieval`` gets each non-empty list)."""
+    spans: dict[str, list[ChunkSpan]] = {}
+    for call in tool_calls:
+        try:
+            if call["function"]["name"] != "search_knowledge_base":
+                raise ValueError(f"Unknown function {call['function']['name']}.")
+            kwargs = json.loads(call["function"]["arguments"])
+            spans[call["id"]] = retrieve_context(**kwargs, config=config)
+        except Exception as e:
+            raise ValueError(f"Error executing tool: {e}") from e
+    spans = _limit_chunkspans(spans, config, messages=messages)
+    out = []
+    for call in tool_calls:
+        found = spans.get(call["id"], [])
+        out.append({"role": "tool", "content": '{"documents": [' + ", ".join(s.to_json(index=i + 1) for i, s in
+                                                                            enumerate(found)) + "]}",
+                    "tool_call_id": call["id"]})
+        if found and callable(on_retrieval):
+            on_retrieval(found)
+    return out
+
+
+def _stream_answer(stream: Iterator[str], messages: list[dict[str, Any]]) -> Iterator[str]:
     pieces = []
-    for piece in engine.generate(prompt, max_tokens=max_tokens, seed=seed, **QWEN3_SAMPLING):
+    for piece in stream:
         pieces.append(piece)
         yield piece
     messages.append({"role": "assistant", "content": "".join(pieces)})
+
+
+def _rag_with_tools(messages: list[dict[str, Any]], *, tools: list[dict[str, Any]], tool_choice: Any,
+                    on_retrieval: Callable[[list[ChunkSpan]], None] | None, config: RAGLiteConfig,
+                    max_tokens: int | None, seed: int | None) -> Iterator[str]:
+    """``rag()``'s function-calling path with the given tools (each one run as ``search_knowledge_base``)."""
+    engine = get_llm(config)
+    calls, stream = chat_completion(engine, _clip(messages, engine.n_ctx), tools=tools, tool_choice=tool_choice,
+                                    max_tokens=max_tokens, seed=seed, sampling=QWEN3_SAMPLING)
+    if calls:
+        messages.append({"role": "assistant", "content": None, "tool_calls": calls})
+        messages.extend(_run_tools(calls, on_retrieval, config, messages=messages))
+        _, stream = chat_completion(engine, _clip(messages, engine.n_ctx), max_tokens=max_tokens, seed=seed,
+                                    sampling=QWEN3_SAMPLING)
+    yield from _stream_answer(stream if stream is not None else iter(()), messages)
+
+
+def rag(messages: list[dict[str, str]], *, on_retrieval: Callable[[list[ChunkSpan]], None] | None = None,
+        config: RAGLiteConfig, max_tokens: int | None = None, seed: int | None = None) -> Iterator[str]:
+    """Stream the registered LLM's answer to ``messages``, then append it to ``messages`` as the assistant's message.
+
+    When the last message carries its context (from ``retrieve_context`` + ``add_context``), the LLM answers it.
+    Otherwise the LLM may first call ``search_knowledge_base`` on the index registered for ``config.db_url``: the
+    tool-call message and one ``tool`` message per call are appended before the answer, and ``on_retrieval`` gets each
+    call's spans.  ``max_tokens`` bounds the answer."""
+    engine = get_llm(config)
+    clipped = _clip(messages, engine.n_ctx)
+    if clipped and _has_context(clipped[-1]):
+        prompt = engine.tokenizer.encode(render_chatml_tools(clipped))   # the handler's text, tool rounds included
+        yield from _stream_answer(engine.generate(prompt, max_tokens=max_tokens, seed=seed, **QWEN3_SAMPLING), messages)
+        return
+    if not clipped or _has_context(messages[-1]) or get_index(config) is None:
+        raise NotImplementedError(
+            "rag() without context in the last message lets the LLM search the knowledge base, which needs an index "
+            f"registered for db_url={config.db_url!r} (register_index, or insert_documents); else retrieve the context "
+            "with retrieve_context and add it with add_context first")
+    yield from _rag_with_tools(messages, tools=[SEARCH_KNOWLEDGE_BASE_TOOL], tool_choice="auto",
+                               on_retrieval=on_retrieval, config=config, max_tokens=max_tokens, seed=seed)
+
+
+async def async_rag(messages: list[dict[str, str]], *, on_retrieval: Callable[[list[ChunkSpan]], None] | None = None,
+                    config: RAGLiteConfig, max_tokens: int | None = None, seed: int | None = None) -> AsyncIterator[str]:
+    """``rag`` as an async generator: each step of the synchronous path runs in a worker thread, off the event loop,
+    and the same messages are appended."""
+    it = rag(messages, on_retrieval=on_retrieval, config=config, max_tokens=max_tokens, seed=seed)
+    done = object()
+    try:
+        while (piece := await asyncio.to_thread(next, it, done)) is not done:
+            yield piece
+    finally:   # a consumer that stops early closes the synchronous path here, not in the garbage collector
+        await asyncio.to_thread(it.close)

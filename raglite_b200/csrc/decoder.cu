@@ -8,7 +8,8 @@
 //   attention_kernel      causal GQA attention over the cache: one CTA per (KV head, 16 query vectors, key range),
 //                         online softmax in fp32; attention_combine_kernel merges key ranges in a fixed order
 //   swiglu_kernel         silu(gate) * up
-//   sample_kernel         repeat penalty, top-k (radix select), top-p, min-p, temperature, inverse-CDF draw
+//   sample_kernel         repeat penalty, top-k (radix select), top-p, min-p, temperature, inverse-CDF draw; its
+//                         masked instance first keeps the ids a grammar state allows (grammar.cu builds the index)
 // Prefill (T > 1) runs the linears on xenc.cu's wgmma quantized linear (launch_qlinear_ld).
 #include <algorithm>
 #include <cub/block/block_scan.cuh>
@@ -404,10 +405,52 @@ __global__ void swiglu_kernel(const __half* __restrict__ gu, int T, int F, __hal
 
 // ---- sampler: one CTA --------------------------------------------------------------------------------------------------
 constexpr int kSampleThreads = 1024;
+// The grammar of a masked draw: the token index (int16 [n_states, V], the state after the token's bytes or -1), the
+// accepting states and the end-of-generation ids, allowed exactly in accepting states whatever their bytes.
+struct SampleMask {
+  const int16_t* index;
+  const uint8_t* accept;
+  int32_t* state;   // device: read, then the state after the drawn token (unchanged after an end-of-generation id)
+  int n_states;
+  int eog[RL_LLM_MAX_EOG];   // -1 past the given ids
+};
+// top-p, min-p, temperature and the inverse CDF at u over the k candidates (descending logit): the slot drawn.
+__device__ int draw(const float* c_logit, int k, float temperature, float top_p, float min_p, float u) {
+  int n = k;
+  if (top_p < 1.f) {   // softmax at temperature 1, smallest prefix whose mass reaches top_p (the crossing one kept)
+    const float mx = c_logit[0];
+    float sum = 0.f;
+    for (int i = 0; i < n; ++i) sum += expf(c_logit[i] - mx);
+    float cum = 0.f;
+    for (int i = 0; i < n; ++i) {
+      cum += expf(c_logit[i] - mx) / sum;
+      if (cum >= top_p) { n = i + 1; break; }
+    }
+  }
+  if (min_p > 0.f) {   // logits >= max + log(min_p), at least one
+    const float cut = c_logit[0] + logf(min_p);
+    int m = 1;
+    while (m < n && c_logit[m] >= cut) ++m;
+    n = m;
+  }
+  const float mx = c_logit[0] / temperature;
+  float sum = 0.f;
+  for (int i = 0; i < n; ++i) sum += expf(c_logit[i] / temperature - mx);
+  const float target = u * sum;
+  float cum = 0.f;
+  int pick = n - 1;
+  for (int i = 0; i < n; ++i) {
+    cum += expf(c_logit[i] / temperature - mx);
+    if (target < cum) { pick = i; break; }
+  }
+  return pick;
+}
+
+template <bool kMasked>
 __global__ void __launch_bounds__(kSampleThreads) sample_kernel(const float* __restrict__ logits, int V, const int32_t* __restrict__ hist,
                                                                int n_hist, float temperature, int top_k, float top_p, float min_p,
                                                                float penalty, float u, float* __restrict__ w,
-                                                               int32_t* __restrict__ out_id) {
+                                                               int32_t* __restrict__ out_id, const SampleMask mask) {
   using Scan = cub::BlockScan<int, kSampleThreads>;
   __shared__ typename Scan::TempStorage scan_tmp;
   __shared__ int hist_bins[256];
@@ -415,9 +458,39 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(const float* __r
   __shared__ int s_need;
   __shared__ float c_logit[RL_LLM_MAX_TOP_K];
   __shared__ int c_id[RL_LLM_MAX_TOP_K];
+  __shared__ int s_allowed;
   const int tid = threadIdx.x;
-  for (int i = tid; i < V; i += kSampleThreads) w[i] = logits[i];
-  __syncthreads();
+  int state = 0;
+  if constexpr (kMasked) {
+    // masked logits are -inf before the penalty (-inf * penalty stays -inf); a state outside the table allows nothing
+    state = *mask.state;
+    const bool valid = state >= 0 && state < mask.n_states;
+    const bool eog_ok = valid && mask.accept[state];
+    const int16_t* row = mask.index + (size_t)(valid ? state : 0) * V;
+    if (tid == 0) s_allowed = 0;
+    __syncthreads();
+    int n_ok = 0;
+    for (int i = tid; i < V; i += kSampleThreads) {
+      bool eog = false;
+#pragma unroll
+      for (int e = 0; e < RL_LLM_MAX_EOG; ++e) eog |= mask.eog[e] == i;   // unused slots hold -1
+      const float x = logits[i];
+      // an id whose own logit is -inf or NaN counts as masked, so every candidate carries mass and the draw's
+      // sums stay finite
+      const bool ok = valid && (eog ? eog_ok : row[i] >= 0) && x > kNegInf;
+      w[i] = ok ? x : kNegInf;
+      n_ok += ok;
+    }
+    atomicAdd(&s_allowed, n_ok);
+    __syncthreads();
+    if (s_allowed == 0) {   // nothing allowed: no token, the state unchanged
+      if (tid == 0) *out_id = RL_LLM_NO_TOKEN;
+      return;
+    }
+  } else {
+    for (int i = tid; i < V; i += kSampleThreads) w[i] = logits[i];
+    __syncthreads();
+  }
   if (tid < n_hist) {   // each distinct id once: its first occurrence applies the penalty
     const int tok = hist[tid];
     bool first = tok >= 0 && tok < V;
@@ -428,7 +501,8 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(const float* __r
     }
   }
   __syncthreads();
-  const int k = temperature == 0.f ? 1 : min(top_k, V);
+  int k = temperature == 0.f ? 1 : min(top_k, V);
+  if constexpr (kMasked) k = min(k, s_allowed);   // the candidates are allowed ids only, so no fallback picks a masked one
   // radix select of the k-th largest order key, 8 bits at a time
   if (tid == 0) { s_prefix = 0; s_mask = 0; s_need = k; }
   for (int shift = 24; shift >= 0; shift -= 8) {
@@ -495,35 +569,16 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(const float* __r
     }
   }
   if (tid != 0) return;
-  if (temperature == 0.f) { *out_id = c_id[0]; return; }
-  int n = k;
-  if (top_p < 1.f) {   // softmax at temperature 1, smallest prefix whose mass reaches top_p (the crossing one kept)
-    const float mx = c_logit[0];
-    float sum = 0.f;
-    for (int i = 0; i < n; ++i) sum += expf(c_logit[i] - mx);
-    float cum = 0.f;
-    for (int i = 0; i < n; ++i) {
-      cum += expf(c_logit[i] - mx) / sum;
-      if (cum >= top_p) { n = i + 1; break; }
-    }
+  int pick = 0;
+  if (temperature != 0.f) pick = draw(c_logit, k, temperature, top_p, min_p, u);
+  const int tok = c_id[pick];
+  *out_id = tok;
+  if constexpr (kMasked) {
+    bool eog = false;
+#pragma unroll
+    for (int e = 0; e < RL_LLM_MAX_EOG; ++e) eog |= mask.eog[e] == tok;
+    if (!eog) *mask.state = mask.index[(size_t)state * V + tok];
   }
-  if (min_p > 0.f) {   // logits >= max + log(min_p), at least one
-    const float cut = c_logit[0] + logf(min_p);
-    int m = 1;
-    while (m < n && c_logit[m] >= cut) ++m;
-    n = m;
-  }
-  const float mx = c_logit[0] / temperature;
-  float sum = 0.f;
-  for (int i = 0; i < n; ++i) sum += expf(c_logit[i] / temperature - mx);
-  const float target = u * sum;
-  float cum = 0.f;
-  int pick = n - 1;
-  for (int i = 0; i < n; ++i) {
-    cum += expf(c_logit[i] / temperature - mx);
-    if (target < cum) { pick = i; break; }
-  }
-  *out_id = c_id[pick];
 }
 
 }  // namespace
@@ -714,8 +769,35 @@ extern "C" int rl_llm_sample(const float* logits, int V, const int32_t* hist, in
              u >= 0.f && u < 1.f, RL_EINVAL, "rl_llm_sample: temperature=%g top_p=%g min_p=%g repeat_penalty=%g u=%g out of "
              "range", temperature, top_p, min_p, repeat_penalty, u);
   RL_REQUIRE(workspace_bytes >= rl_llm_sample_workspace_bytes(V), RL_ENOSPACE, "rl_llm_sample: workspace too small");
-  sample_kernel<<<1, kSampleThreads, 0, (cudaStream_t)stream>>>(logits, V, hist, n_hist, temperature, top_k, top_p, min_p,
-                                                                repeat_penalty, u, reinterpret_cast<float*>(workspace), out_id);
+  sample_kernel<false><<<1, kSampleThreads, 0, (cudaStream_t)stream>>>(logits, V, hist, n_hist, temperature, top_k, top_p,
+                                                                       min_p, repeat_penalty, u,
+                                                                       reinterpret_cast<float*>(workspace), out_id, SampleMask{});
+  RL_CUDA_CHECK(cudaGetLastError());
+  return RL_OK;
+}
+
+extern "C" int rl_llm_sample_masked(const float* logits, int V, const int32_t* hist, int n_hist, float temperature, int top_k,
+                                    float top_p, float min_p, float repeat_penalty, float u, const int16_t* index,
+                                    int n_states, const uint8_t* accept, const int32_t* eog_ids, int n_eog, int32_t* state,
+                                    int32_t* out_id, void* workspace, size_t workspace_bytes, void* stream) {
+  RL_REQUIRE(logits && out_id && workspace && V > 0 && n_hist >= 0 && (hist || n_hist == 0), RL_EINVAL,
+             "rl_llm_sample_masked: bad arguments");
+  RL_REQUIRE(index && accept && state && n_states > 0 && n_states <= RL_GRAMMAR_MAX_STATES, RL_EINVAL,
+             "rl_llm_sample_masked: bad grammar (n_states=%d, 1 .. %d)", n_states, RL_GRAMMAR_MAX_STATES);
+  RL_REQUIRE(n_eog >= 0 && n_eog <= RL_LLM_MAX_EOG && (eog_ids || n_eog == 0), RL_EINVAL,
+             "rl_llm_sample_masked: n_eog=%d (0 .. %d)", n_eog, RL_LLM_MAX_EOG);
+  RL_REQUIRE(n_hist <= kSampleThreads, RL_EINVAL, "rl_llm_sample_masked: n_hist=%d > %d", n_hist, kSampleThreads);
+  RL_REQUIRE(top_k >= 1 && top_k <= RL_LLM_MAX_TOP_K, RL_EINVAL, "rl_llm_sample_masked: top_k=%d unsupported (1 .. %d)",
+             top_k, RL_LLM_MAX_TOP_K);
+  RL_REQUIRE(temperature >= 0.f && top_p > 0.f && top_p <= 1.f && min_p >= 0.f && min_p <= 1.f && repeat_penalty > 0.f &&
+             u >= 0.f && u < 1.f, RL_EINVAL, "rl_llm_sample_masked: temperature=%g top_p=%g min_p=%g repeat_penalty=%g "
+             "u=%g out of range", temperature, top_p, min_p, repeat_penalty, u);
+  RL_REQUIRE(workspace_bytes >= rl_llm_sample_workspace_bytes(V), RL_ENOSPACE, "rl_llm_sample_masked: workspace too small");
+  SampleMask m{index, accept, state, n_states, {}};
+  for (int e = 0; e < RL_LLM_MAX_EOG; ++e) m.eog[e] = e < n_eog ? eog_ids[e] : -1;
+  sample_kernel<true><<<1, kSampleThreads, 0, (cudaStream_t)stream>>>(logits, V, hist, n_hist, temperature, top_k, top_p,
+                                                                      min_p, repeat_penalty, u,
+                                                                      reinterpret_cast<float*>(workspace), out_id, m);
   RL_CUDA_CHECK(cudaGetLastError());
   return RL_OK;
 }

@@ -15,7 +15,10 @@ installed), but two pieces of the hot path are pure NumPy/SciPy once their impor
 * ``raglite/_split_sentences.py`` -- ``split_sentences`` and ``markdown_sentence_boundaries``, with wtpsplit-lite's
   ``SaT`` replaced by a fake that returns seeded float32 probabilities;
 * ``raglite/_split_chunklets.py`` and ``raglite/_split_chunks.py`` -- ``split_chunklets`` (with its Markdown boundaries
-  and statement counts) and ``split_chunks`` (with the cost vector it hands to ``linprog``).
+  and statement counts) and ``split_chunks`` (with the cost vector it hands to ``linprog``);
+* ``raglite/_chatml_function_calling.py`` -- the chat handler's jinja template rendered on seeded message lists, and
+  the handler itself run over a scripted ``Llama`` that records each completion's prompt, grammar and settings
+  (``tests/golden/chatml_tools.json``).
 
 This script loads those two files *unmodified from where they lie* under a synthetic ``raglite``
 package whose heavy dependencies are replaced by stubs, and whose embedder is
@@ -441,6 +444,135 @@ def golden_split_chunks() -> None:
     print("split_chunks", len(cases), "cases,", sum(c["solved"] for c in cases), "solved")
 
 
+def golden_chatml_tools() -> None:
+    """The function-calling chat handler: its template rendered with jinja2 as the handler renders it, and the handler
+    run over a scripted Llama (each completion returns a given raw output cut at its first stop string, as
+    llama-cpp-python's create_completion does), recording every completion's prompt, grammar and settings."""
+    import ast
+
+    import jinja2
+    from jinja2.sandbox import ImmutableSandboxedEnvironment
+
+    src = (REF / "_chatml_function_calling.py").read_text()
+    tree = ast.parse(src)
+    tmpl = next(ast.literal_eval(n.value) for n in ast.walk(tree) if isinstance(n, ast.Assign)
+                and any(getattr(t, "id", "") == "function_calling_template" for t in n.targets))
+    render = ImmutableSandboxedEnvironment(undefined=jinja2.StrictUndefined).from_string(tmpl).render
+
+    def tool(name: str, desc: str | None, props: dict) -> dict:
+        f = {"name": name, "parameters": {"type": "object", "properties": props, "required": list(props),
+                                          "additionalProperties": False}}
+        if desc is not None:
+            f["description"] = desc
+        return {"type": "function", "function": f}
+
+    kb = tool("search_knowledge_base", "Search the knowledge base.\nIMPORTANT: You MAY NOT use this function if the "
+              "question can be answered with common knowledge or straightforward reasoning.\nFor multi-faceted "
+              "questions, call this function once for each facet.",
+              {"query": {"type": "string", "description": "The `query` string MUST be a precise single-faceted question "
+                         "in the user's language.\nThe `query` string MUST resolve all pronouns to explicit nouns."}})
+    odd = tool("lookup", '  Quotes "q", \'s\', <tag> & amp; café  ', {"k": {"type": "integer", "description": "a<b"}})
+    plain = tool("plain", None, {"x": {"type": "string", "maxLength": 8}})
+    call = {"role": "assistant", "content": None, "tool_calls": [
+        {"id": "call__0_search_knowledge_base_x", "type": "function",
+         "function": {"name": "search_knowledge_base", "arguments": '{"query": "What is a fox?"}'}},
+        {"id": "call__1_search_knowledge_base_x", "type": "function",
+         "function": {"name": "search_knowledge_base", "arguments": '{"query": "dogs"}'}}]}
+    toolmsg = {"role": "tool", "content": '{"documents": [{"id": "d"}]}', "tool_call_id": "call__0_x"}
+    lists = {
+        "user": [{"role": "user", "content": "What colour is the fox?"}],
+        "user_sys_appended": [{"role": "user", "content": "Hi & <b>"}, {"role": "system", "content": ""}],
+        "system_user": [{"role": "system", "content": "Be brief."}, {"role": "user", "content": "Tell me 'this'."}],
+        "history": [{"role": "system", "content": "S"}, {"role": "user", "content": "q1"},
+                    {"role": "assistant", "content": "a1"}, {"role": "user", "content": "q2"}],
+        "tool_round": [{"role": "user", "content": "What colour is the fox?"}, call, toolmsg,
+                       {**toolmsg, "tool_call_id": "call__1_x"}],
+        "tool_round_answered": [{"role": "user", "content": "Q"}, call, toolmsg, {"role": "assistant", "content": "A."}],
+    }
+    toolsets = {"kb": [kb], "odd": [odd, kb], "plain": [plain]}
+    renders = []
+    for ln, msgs in lists.items():
+        renders.append({"messages": ln, "tools": None, "tool_calls": False,
+                        "text": render(messages=msgs, tools=[], tool_calls=None, add_generation_prompt=True)})
+        for tn, tools in toolsets.items():
+            renders.append({"messages": ln, "tools": tn, "tool_calls": True,
+                            "text": render(messages=msgs, tools=tools, tool_calls=True, add_generation_prompt=True)})
+
+    class Grammar:
+        def __init__(self, kind: str, text: str) -> None:
+            self.kind, self.text = kind, text
+
+    class LlamaGrammar:
+        @staticmethod
+        def from_string(text: str, verbose: bool = False) -> Grammar:  # noqa: ARG004
+            return Grammar("gbnf", text)
+
+        @staticmethod
+        def from_json_schema(text: str, verbose: bool = False) -> Grammar:  # noqa: ARG004
+            return Grammar("json_schema", text)
+
+    class ScriptedLlama:
+        verbose = False
+
+        def __init__(self, raw: list[str]) -> None:
+            self.raw, self.calls = list(raw), []
+
+        def create_completion(self, prompt: str, **kw):  # noqa: ANN003, ANN202
+            raw = self.raw.pop(0)
+            stops = kw.get("stop") or []
+            cut = min([i for i in (raw.find(x) for x in stops) if i >= 0], default=len(raw))
+            g = kw.get("grammar")
+            self.calls.append({"prompt": prompt, "grammar": None if g is None else [g.kind, g.text],
+                               "temperature": kw["temperature"], "stop": list(stops), "max_tokens": kw["max_tokens"]})
+            return {"id": "cmpl-x", "created": 0, "model": "m",
+                    "choices": [{"text": raw[:cut], "index": 0, "logprobs": None, "finish_reason": "stop"}]}
+
+    class _Lazy(types.ModuleType):
+        def __getattr__(self, name):  # noqa: ANN001, ANN204
+            return type(name, (), {})
+
+    lazy = _Lazy("raglite._lazy_llama")
+    lazy.llama = _Lazy("llama")
+    lazy.llama_types = _Lazy("llama_types")
+    lazy.llama_grammar = types.SimpleNamespace(LlamaGrammar=LlamaGrammar)
+    lazy.llama_chat_format = types.SimpleNamespace(_convert_completion_to_chat=lambda c, stream=False: c)  # noqa: ARG005
+    sys.modules.setdefault("raglite", types.ModuleType("raglite"))
+    sys.modules["raglite._lazy_llama"] = lazy
+    handler = _load("raglite._chatml_function_calling_ref", REF / "_chatml_function_calling.py")
+
+    fn = "functions.search_knowledge_base:"
+    args = ['{"query": "What colour is the fox?"}', '{ "query":"dogs" }\n ', '{"query": "caf\\u00e9 <&>"}']
+    end = "<|im_end|>"
+    scenarios = {
+        "message": ("auto", "kb", ["<message>", "The fox is brown." + end]),
+        "think_message": ("auto", "kb", ["<think>\nmaybe not</think>\n\n<message>", "Brown." + end]),
+        "one_call": ("auto", "kb", ["<function_calls>\n" + fn, args[0] + end, "</function_calls>"]),
+        "two_calls": ("auto", "kb", ["<function_calls>\n" + fn, args[0] + end, fn, args[1] + end, end]),
+        "think_call": ("auto", "kb", ["<think>\nsearch</think>\n\n<function_calls>\n" + fn, args[2] + end,
+                                      "</function_calls>"]),
+        "cap": ("auto", "kb", ["<function_calls>\n" + fn] + [x for i in range(17) for x in (
+            '{"query": "q%d"}' % i + end, fn)]),
+        "unknown_name": ("auto", "odd", ["<function_calls>\nfunctions.lookup:", '{"k": 3}' + end, end]),
+        "fixed": ({"type": "function", "function": {"name": "plain"}}, "plain",
+                  ["<function_calls>\nfunctions.plain:", '{"x": "abc"}' + end, "<|endoftext|>"]),
+    }
+    protocol = []
+    for name, (choice, tn, raw) in scenarios.items():
+        for ln in ("user",) if name == "cap" else ("user", "system_user"):
+            llm = ScriptedLlama(raw)
+            out = handler.chatml_function_calling_with_streaming(llm, [dict(m) for m in lists[ln]],
+                                                                 tools=toolsets[tn], tool_choice=choice,
+                                                                 temperature=0.6, top_p=0.95, top_k=20, min_p=0.0)
+            msg = out["choices"][0].get("message")
+            result = ({"tool_calls": [[c["function"]["name"], c["function"]["arguments"]] for c in msg["tool_calls"]]}
+                      if msg else {"text": out["choices"][0]["text"]})
+            protocol.append({"scenario": name, "messages": ln, "tools": tn, "tool_choice": choice, "raw": raw,
+                             "calls": llm.calls, "result": result, "unused_raw": len(llm.raw)})
+    data = {"lists": lists, "toolsets": toolsets, "renders": renders, "protocol": protocol}
+    (GOLDEN / "chatml_tools.json").write_text(json.dumps(data, ensure_ascii=False) + "\n")
+    print("chatml_tools", len(renders), "renders,", len(protocol), "protocol runs")
+
+
 if __name__ == "__main__":
     GOLDEN.mkdir(parents=True, exist_ok=True)
     golden_rrf()
@@ -451,3 +583,4 @@ if __name__ == "__main__":
     golden_split_sentences()
     golden_split_chunklets()
     golden_split_chunks()
+    golden_chatml_tools()
